@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- audio tokens/sec of the VALL-E AR+NAR decode hot path on B200.
+"""bench.py -- audio tokens/sec of the VALL-E AR+NAR decode hot path on H100.
 
 The JSON line also carries, as sub-objects measured in the same run (N=1 unless noted): `parity` (the timed bf16
 batch holds the inputs of the reference fixture big_full as utterance 0: token-match rate / first divergence vs the
@@ -7,7 +7,7 @@ reference's codes, and the fp32 engine's bit-exactness on the same inputs), `par
 roofline), `config2` (NAR B=32 x L=1500), `config3` (256 prompts, strong scaling, every N), `config4` (EnCodec
 encode + decode), `roofline_b1` / `p50_utt_latency_ms` (configs[1]), `cpu_baseline`.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" = one pass of the hot path over one batch of synthetic utterances per GPU:
@@ -53,6 +53,9 @@ def parse():
                     help="BASELINE configs[3]: prompts of the strong-scaling job sharded over the ranks (0 = skip)")
     ap.add_argument("--no-extra", action="store_true",
                     help="skip the sub-objects (parity, parity_mode, config2/3/4, batch-1 latency, cpu_baseline)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the codes of the last timed step as DIR/codes.npy (float32 [B, frames, 8], -1 past "
+                         "an utterance's end) and DIR/code_lengths.npy, for comparing two builds output for output")
     return ap.parse_args()
 
 
@@ -62,7 +65,7 @@ def peaks():
         j = json.load(open(p))
         return dict(hbm_gbs=j["hbm_gbs"], tflops=j.get("bf16_tflops_sustained", j["bf16_tflops"]),
                     tflops_burst=j["bf16_tflops"], source="MEASURED_PEAKS.json (measured)")
-    return dict(hbm_gbs=6650.0, tflops=1400.0, tflops_burst=1590.0, source="B200_PROFILING.md fallback")
+    return dict(hbm_gbs=3350.0, tflops=989.0, tflops_burst=989.0, source="H100 SXM data sheet (not measured)")
 
 
 # ----------------------------------------------------------------------------- synthetic workload
@@ -369,6 +372,18 @@ def config4_block(dev, n_utt=64, chunk=32):
             "wav_out_shape": list(out.shape)}
 
 
+def dump_codes(out_dir, codes):
+    """codes: the per-utterance [frames, N_Q] code matrices one timed step returned"""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    lens = [int(c.shape[0]) for c in codes]
+    arr = np.full((len(codes), max(lens), N_Q), -1.0, dtype=np.float32)
+    for i, c in enumerate(codes):
+        arr[i, :lens[i]] = c.detach().cpu().numpy()
+    np.save(os.path.join(out_dir, "codes.npy"), arr)
+    np.save(os.path.join(out_dir, "code_lengths.npy"), np.asarray(lens, dtype=np.float32))
+
+
 # ----------------------------------------------------------------------------- main
 def main():
     a = parse()
@@ -462,7 +477,7 @@ def main():
         ar_ms = nar_ms = pre_ms = 0.0
         t_wall = time.perf_counter()
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        utt0 = None
+        utt0 = codes = None
         ev0.record()
         for i in range(steps):
             codes = one_step(*batches[i % 2], e2e)
@@ -478,13 +493,15 @@ def main():
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return dict(ms=float(t.item()), wall_ms=wall, launches=eng.kernel_launches() - n0,
-                    ar_ms=ar_ms, nar_ms=nar_ms, prefill_ms=pre_ms, steps=eng.stats.ar_steps, utt0=utt0)
+                    ar_ms=ar_ms, nar_ms=nar_ms, prefill_ms=pre_ms, steps=eng.stats.ar_steps, utt0=utt0, codes=codes)
 
     clocks = Clocks(local)
     if rank == 0:
         clocks.start()
     r = timed(False, a.steps, a.warmup)
     clk = clocks.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_codes(a.dump_outputs, r["codes"])
     re = timed(True, a.steps, max(1, min(a.warmup, 1)))
 
     tokens_step = B * frames * N_Q                     # per GPU per step
@@ -498,18 +515,6 @@ def main():
     ar_bytes = ar_step_bytes(B, mean_len, esize)
     ar_step_s = (r["ar_ms"] / a.steps) / 1000.0 / max(1, r["steps"])
     ach = ar_bytes / ar_step_s / 1e9
-    # DRAM bytes of one decode step from the committed ncu capture (tools/ar_step_traffic.py), if there is one
-    traffic, traffic_src = None, None
-    for tp in ("round2b_ar_step_traffic_fold.json", "round2_ar_step_traffic.json", "round1_ar_step_traffic.json"):
-        tp = os.path.join(ROOT, "profiles", tp)
-        if B == 64 and esize == 2 and os.path.exists(tp):
-            with open(tp) as f:
-                tj = json.load(f)
-            traffic = tj["traffic_bytes"]
-            traffic_src = (f"profiles/{os.path.basename(tp)}: ncu dram__bytes_read+write over the "
-                           f"{tj['kernels_in_step']} kernels of one step at context {tj['context_len']} "
-                           f"(algorithmic {tj['algorithmic_bytes']:.4g} B)")
-            break
     nar_fl = 7 * nar_pass_flops(B, S_TEXT + T_PROMPT + frames, frames)
     nar_s = (r["nar_ms"] / a.steps) / 1000.0
     line = {
@@ -519,7 +524,7 @@ def main():
         "config": {"workload": f"e2e AR+NAR infer: {B} utterances/GPU x (S={S_TEXT}, {T_PROMPT}-frame prompt) -> "
                                f"{frames} frames x {N_Q} codebooks, greedy, d={D_MODEL}/{N_HEAD}h/{N_LAYER}L",
                    "batch_per_gpu": B, "parallelism": f"dp{world} (independent utterances, one final all-gather)",
-                   "l2": "working set (weights + KV cache > 1 GB) exceeds the 126 MB L2; inputs alternate between 2 batches"},
+                   "l2": "working set (weights + KV cache > 1 GB) exceeds the 50 MB L2; inputs alternate between 2 batches"},
         "gpu_launches": r["launches"],
         "phase_ms_per_step": {"prefill": r["prefill_ms"] / a.steps, "ar": r["ar_ms"] / a.steps,
                               "nar": r["nar_ms"] / a.steps, "ar_decode_steps": r["steps"]},
@@ -529,8 +534,7 @@ def main():
                      "chain": ("LayerNorms folded into the projections, 6 launches per layer"
                                if getattr(eng, "ar_head_fold", None) is not None else "8 launches per layer"),
                      "bound": "hbm", "achieved": ach, "peak": pk["hbm_gbs"], "unit": "GB/s",
-                     "frac": ach / pk["hbm_gbs"], "traffic": traffic, "traffic_source": traffic_src,
-                     "peak_source": pk["source"],
+                     "frac": ach / pk["hbm_gbs"], "peak_source": pk["source"],
                      "algorithmic_bytes_per_launch": ar_bytes, "launch_seconds": ar_step_s},
         "roofline_nar": {"kernel": "7 NAR passes (QKV/out/FFN GEMMs + attention + heads)", "bound": "tensor",
                          "achieved": nar_fl / nar_s / 1e12 if nar_s > 0 else None, "peak": pk["tflops"],

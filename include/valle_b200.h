@@ -1,5 +1,5 @@
 /*
- * valle_b200.h -- C ABI of libvalle_b200.so: the sm_100a (B200) VALL-E decoding engine.
+ * valle_b200.h -- C ABI of libvalle_b200.so: the sm_90a (H100) VALL-E decoding engine.
  *
  * Drop-in boundary (SURVEY.md section 8b).  Every entry point takes raw device pointers,
  * explicit sizes and a cudaStream_t (passed as void*); there are no torch / C++ types in any
@@ -105,7 +105,7 @@ int vb_adaln_project(const float *W, const float *b, const float *emb, int d, fl
  *   C[M,N] = epi( A[M,K] * W[N,K]^T + bias[N] )
  *   VB_EPI_NONE / VB_EPI_RELU: C has dtype c_dtype.  VB_EPI_RESIDUAL: C is fp32 and is
  *   accumulated in place (C += ...), i.e. the residual add of transformer.py:297-302.
- *   a_dtype must equal w_dtype.  bf16 operands use the tcgen05/TMEM kernel when M is large,
+ *   a_dtype must equal w_dtype.  bf16 operands use the wgmma/TMA kernel when M is large,
  *   fp32 operands the exact-order SIMT kernel. */
 int vb_linear(const void *A, int a_dtype, int64_t lda, const void *W, int w_dtype, const float *bias,
               void *C, int c_dtype, int64_t ldc, int64_t M, int N, int K, int epilogue,
@@ -321,8 +321,8 @@ int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb
  * the cache -> out-proj -> LN -> FFN), then vb_ar_head_step.  Safe to capture in a CUDA graph
  * (no host reads; launch geometry depends only on B and cache_cap).  bf16 decoders with
  * vb_decoder_set_decode_fold + head->fold run the LayerNorm-folded chain (6 launches per layer; the
- * residual stream is assembled by bulk reductions whose order over the split-K slabs is not fixed:
- * last-bit differences between runs, VB_DECODE_FOLD=0 selects the fixed-order 8-launch chain). */
+ * residual stream is assembled by the split-K projections themselves, the splits of a tile adding up in fixed order
+ * inside a thread-block cluster; VB_DECODE_FOLD=0 selects the 8-launch chain).  Both are run-to-run deterministic. */
 int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st, void *workspace,
                       size_t workspace_bytes, vb_stream_t stream);
 

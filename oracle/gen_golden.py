@@ -13,6 +13,7 @@ bug), and a few raw logit rows for tolerance checks.
 from __future__ import annotations
 
 import os
+import random
 import sys
 import time
 
@@ -254,6 +255,53 @@ def gen_switches(ref, only=()):
                                 codes=codes.to(torch.int16), forward=fw))
 
 
+def _layout(m):
+    sd = m.state_dict()
+    return dict(keys=list(sd.keys()), shapes=[tuple(v.shape) for v in sd.values()], checksums=checksums(sd),
+                params=[n for n, _ in m.named_parameters()], buffers=[n for n, _ in m.named_buffers()])
+
+
+def gen_ref_checks(ref):
+    """what tests/test_oracle.py and tests/test_boundary.py compare with the reference: its outputs on the seeded
+    inputs of test_oracle_vs_reference_inference_and_forward, and the checkpoint layout (keys, shapes, parameter /
+    buffer names, per-tensor fingerprints) of the reference class at the seeds those tests use"""
+    out = dict(inference={}, layout={})
+    for pm in (0, 1):
+        torch.manual_seed(0)
+        m = ref.VALLE(256, 4, 2, norm_first=True, add_prenet=False, prefix_mode=pm, share_embedding=True,
+                      nar_scale_factor=1.0, prepend_bos=False, num_quantizers=8).eval()
+        g = torch.Generator().manual_seed(21)
+        x = torch.randint(3, 100, (1, 7), generator=g)
+        y = torch.randint(0, 1024, (1, 15, 8), generator=g)
+        xl = torch.tensor([7], dtype=torch.int32)
+        with torch.no_grad():
+            greedy = m.inference(x, xl, y, None, top_k=1)
+            cont = m.continual(x, xl, y)
+            torch.manual_seed(3)
+            sampled = m.inference(x, xl, y, None, top_k=5, temperature=0.9)
+        xx = torch.randint(3, 100, (3, 9), generator=g)
+        xls = torch.tensor([9, 7, 5], dtype=torch.int32)
+        yy = torch.randint(0, 1024, (3, 40, 8), generator=g)
+        yls = torch.tensor([40, 33, 28], dtype=torch.int32)
+        m.rng = random.Random(0)
+        torch.manual_seed(5)
+        with torch.no_grad():
+            (_, _), loss, _ = m(xx, xls, yy, yls)
+        out["inference"][pm] = dict(checksums=checksums(m.state_dict()), x=x, y=y, xx=xx, yy=yy,
+                                    greedy=greedy.to(torch.int16), continual=cont.to(torch.int16),
+                                    sampled=sampled.to(torch.int16), loss=float(loss))
+    for prenet in (False, True):
+        torch.manual_seed(0)
+        m = ref.VALLE(256, 4, 2, norm_first=True, add_prenet=prenet, prefix_mode=1, share_embedding=True,
+                      nar_scale_factor=1.0, prepend_bos=False, num_quantizers=8)
+        out["layout"][("seed0", prenet)] = _layout(m)
+    torch.manual_seed(123)
+    m = ref.VALLE(256, 4, 2, norm_first=True, add_prenet=False, prefix_mode=1, share_embedding=True,
+                  nar_scale_factor=1.0, prepend_bos=False, num_quantizers=8)
+    out["layout"][("seed123", False)] = _layout(m)
+    save("ref_checks.pt", out)
+
+
 def main(argv):
     ref = load_reference()
     what = argv or ["tiny", "batch", "config0", "big_short"]
@@ -274,6 +322,8 @@ def main(argv):
         gen_topk(ref)
     if "big_full" in what:
         gen_big(ref, 47, 225, "big_full")  # BASELINE.json configs[1]: 3 s prompt -> 753 frames
+    if "ref_checks" in what:
+        gen_ref_checks(ref)
 
 
 if __name__ == "__main__":

@@ -1,6 +1,6 @@
 """TEST INFRASTRUCTURE ONLY -- CPU restatement of the reference VALL-E hot path.
 
-This file is the *oracle* for the sm_100a engine in `valle_b200/`.  It restates,
+This file is the *oracle* for the sm_90a engine in `valle_b200/`.  It restates,
 in explicit torch-CPU fp32 arithmetic on a plain `state_dict`, what
 lifeiteng/vall-e computes in
 

@@ -1,4 +1,4 @@
-"""tcgen05/TMEM GEMM (bf16) against a torch fp32 reference of the same op on the same bf16-rounded
+"""wgmma GEMM (bf16; the test names keep the kernel's former tcgen05 name) against a torch fp32 reference of the same op on the same bf16-rounded
 operands.  Tolerance: fp32 accumulation of bf16 products -> |err| <= 2e-3 * sqrt(K/1024) abs on
 O(1) outputs (bf16 output rounding adds 2^-8 relative)."""
 import pytest
@@ -38,16 +38,16 @@ def test_tcgen05_gemm_matches_fp32_reference(M, N, K, epi):
 
 
 def test_tcgen05_matches_simt_kernel_bitwise_inputs():
-    """same bf16 operands through the CUDA-core kernel (VB_DISABLE_TCGEN05 is read per call)."""
+    """same bf16 operands through the CUDA-core kernel (VB_DISABLE_WGMMA is read per call)."""
     import os
     from valle_b200 import ops
     g = torch.Generator().manual_seed(5)
     a = torch.randn(257, 1024, generator=g).bfloat16().to(DEV)
     w = (torch.randn(1024, 1024, generator=g) / 32).bfloat16().to(DEV)
     o1 = ops.linear(a, w, None, out_dtype=torch.float32)
-    os.environ["VB_DISABLE_TCGEN05"] = "1"
+    os.environ["VB_DISABLE_WGMMA"] = "1"
     try:
         o2 = ops.linear(a, w, None, out_dtype=torch.float32)
     finally:
-        del os.environ["VB_DISABLE_TCGEN05"]
+        del os.environ["VB_DISABLE_WGMMA"]
     assert torch.allclose(o1, o2, atol=1e-3, rtol=1e-4), (o1 - o2).abs().max()

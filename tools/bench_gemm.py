@@ -1,5 +1,5 @@
-"""Microbenchmark of the tcgen05 GEMM on the NAR shapes of BASELINE.json configs[2] (B=32 x L=1500).
-CUDA-event timing, L2 flushed between iterations by the shapes themselves (A+C > 126 MB)."""
+"""Microbenchmark of the wgmma GEMM on the NAR shapes of BASELINE.json configs[2] (B=32 x L=1500).
+CUDA-event timing, L2 flushed between iterations by the shapes themselves (A+C > 50 MB)."""
 import json
 import os
 import sys

@@ -1,8 +1,9 @@
-"""Per-kernel counts of the Blackwell-native SASS instructions in libvalle_b200.so (cuobjdump -sass):
-UTC*MMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st, UTMALDG/UTMASTG/UTMAREDG = TMA tensor load/store/reduce,
-UBLKCP = cp.async.bulk, UTMAPF/UTMACCTL = TMA prefetch / descriptor control, HMMA = legacy mma.sync.
+"""Per-kernel counts of the Hopper-native SASS instructions in libvalle_b200.so (cuobjdump -sass):
+HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / arrive / wait, UTMALDG/UTMASTG/UTMAREDG = TMA tensor
+load/store/reduce, UBLKCP = cp.async.bulk, UTMAPF = TMA descriptor prefetch, SYNCS = mbarrier operations,
+HMMA = warp-level mma.sync, LDGSTS = cp.async.
 
-    python tools/sass_summary.py [lib.so] > profiles/sass_summary.txt
+    python tools/sass_summary.py [lib.so]
 """
 import collections
 import os
@@ -12,7 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "valle_b200", "lib", "libvalle_b200.so")
-PAT = re.compile(r"\b(UTC[A-Z]*MMA|LDTM|STTM|UTMALDG|UTMASTG|UTMAREDG|UBLKCP|UBLKPF|UTMAPF|UTCBAR|SYNCS|HMMA|LDGSTS|UTCCP)\b")
+PAT = re.compile(r"\b(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UTMAREDG|UBLKCP|UTMAPF|SYNCS|HMMA|LDGSTS)\b")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
 cur, tab = None, collections.OrderedDict()
 for line in out.splitlines():
@@ -26,8 +27,8 @@ for line in out.splitlines():
             tab[cur][op] += 1
         tab[cur]["_instr"] += 1 if re.search(r"/\*[0-9a-f]{4}\*/", line) else 0
 dem = subprocess.run(["c++filt"], input="\n".join(tab), capture_output=True, text=True).stdout.splitlines()
-cols = ["UTCHMMA", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UTMAREDG", "UBLKCP", "UBLKPF", "SYNCS", "HMMA", "LDGSTS"]
-print(f"# {os.path.relpath(lib, ROOT)}: SASS instruction counts per kernel (cuobjdump -sass, sm_100a)")
+cols = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAREDG", "UBLKCP", "UTMAPF", "SYNCS", "HMMA", "LDGSTS"]
+print(f"# {os.path.relpath(lib, ROOT)}: SASS instruction counts per kernel (cuobjdump -sass, sm_90a)")
 print(f"{'kernel':90s} " + " ".join(f"{c:>8s}" for c in cols))
 tot = collections.Counter()
 for (name, cnt), d in zip(tab.items(), dem):

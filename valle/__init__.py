@@ -1,4 +1,4 @@
-"""`valle` -- the reference's package name, served by the B200 engine.
+"""`valle` -- the reference's package name, served by the H100 engine.
 
 A user of lifeiteng/vall-e switches by putting this repository ahead of the reference on `sys.path`:
 `from valle.models import get_model, add_model_arguments`, `from valle.data import AudioTokenizer,

@@ -99,8 +99,8 @@ VB_API int vb_linear(const void *A, int a_dtype, int64_t lda, const void *W, int
   VB_CHECK_ARG(epilogue >= VB_EPI_NONE && epilogue <= VB_EPI_RESIDUAL, "vb_linear: bad epilogue %d", epilogue);
   VB_CHECK_ARG(M >= 0 && N > 0 && K > 0, "vb_linear: bad shape M=%lld N=%d K=%d", (long long)M, N, K);
   cudaStream_t s = (cudaStream_t)stream;
-  if (a_dtype == VB_BF16 && tcgen05_gemm_supported(M, N, K, lda, ldc))
-    return launch_gemm_tcgen05((const bf16 *)A, lda, (const bf16 *)W, bias, C, c_dtype, ldc, M, N, K,
+  if (a_dtype == VB_BF16 && wgmma_gemm_supported(M, N, K, lda, ldc))
+    return launch_gemm_wgmma((const bf16 *)A, lda, (const bf16 *)W, bias, C, c_dtype, ldc, M, N, K,
                                epilogue, s);
   return launch_gemm_simt(A, a_dtype, lda, W, bias, C, c_dtype, ldc, M, N, K, epilogue, s);
 }
@@ -526,15 +526,13 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   StepWs w = carve_step_ws(D, B, st->cache_cap, workspace);
   float *x = st->x_cur;
   if (use_tc_decode(D, B)) {
-    // bf16 tensor-core path: LayerNorm(+pending residual) -> swap-AB split-K tcgen05 projections whose
+    // bf16 tensor-core path: LayerNorm(+pending residual) -> swap-AB split-K wgmma projections whose
     // partial sums are consumed by the next kernel in the chain (7 launches per layer, PDL-chained)
     const bool pdl = use_pdl();
-    // Tuning of the chain (measured on B200 at d=1024 / d_ff=4096 / B=64, profiles/round1_summary.md): split-K wide
-    // enough to fill the SMs is not the optimum for the projections whose partial sums a reduce kernel has to add
-    // up again (FFN2: 9 splits beat 18, QKV: 5 beat 6, FFN1: 2 beat 4); 40 % of the KV streams prefetched into L2
-    // beat 20 / 60 %.
-    // (40 % for the 8-launch chain; the folded chain leaves the projections less time ahead of the attention launch:
-    //  30-35 % measured 1-2 % better than 40 %)
+    // Split-K wide enough to fill the SMs is not the optimum for the projections whose partial sums a reduce kernel
+    // has to add up again, hence the fixed split counts below; the share of the KV streams prefetched into L2 is
+    // smaller in the folded chain, which leaves the projections less time ahead of the attention launch.  These
+    // defaults have not been re-tuned on H100 (VB_SPLITS_* / VB_KV_PREFETCH_PCT override them).
     const bool fold_on = dec->fold_qkv && dec->fold_ffn1 && head->fold.wf && tune("VB_DECODE_FOLD", 1) != 0;
     const int pf_env = tune("VB_KV_PREFETCH_PCT", fold_on ? 35 : 40);
     const int pf_pct = B >= 16 ? pf_env : 0;
@@ -545,7 +543,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     const int qkv_splits = qkv_env > 0 ? qkv_env : std::max(1, std::min(5, d / 128));
     const int ffn2_splits = ffn2_env > 0 ? ffn2_env : std::max(1, std::min(9, dff / 128));
     // folded chain: no reduce kernel pays for more slabs, and with <= 6 k-blocks per CTA the weight ring never wraps
-    const int ffn2_fold = ffn2_env > 0 ? ffn2_env : std::max(1, std::min(11, dff / 128));
+    const int ffn2_fold = ffn2_env > 0 ? ffn2_env : std::max(1, std::min(8, dff / 128));
     const int ffn1_splits = ffn1_env > 0 ? ffn1_env : std::max(1, std::min(2, d / 128));
     float *P = (float *)w.gemm_ws;
     Pending pend;
@@ -565,7 +563,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     };
     if (fold_on) {
       // Folded chain, 6 launches per layer: the residual stream x is assembled in place by the split-K projections that
-      // produce it (red.global.add of every split's tile), the projections that consume it read the fp32 rows and carry
+      // produce it (the splits of a tile as a cluster, summed over DSMEM in fixed order), the projections that consume it read the fp32 rows and carry
       // the LayerNorm in their weights (vb_ln_fold), the rows' moments travel with the partial sums:
       //   QKV'(x) -> attention (+ moments, KV append) -> out-proj (+= x) -> FFN1'(x) -> ReLU reduce (+ moments) -> FFN2 (+= x)
       const int qkv_f = qkv_env > 0 ? qkv_env : std::max(1, std::min(5, d / 128));

@@ -4,7 +4,7 @@
 //     parity mode.  Also fills the KV cache.
 //   * attn_decode      : one query row per (utterance, head) against the growing KV cache.
 //     HBM-bound: 16-byte coalesced K/V reads, warp-shuffle dot products and softmax
-//     reductions, split-KV across CTAs when B*H is too small to fill 148 SMs.
+//     reductions, split-KV across CTAs when B*H is too small to fill 132 SMs.
 //
 // Reference arithmetic: F.multi_head_attention_forward as called from
 // valle/modules/activation.py:408-427; masks valle/models/valle.py:1010-1033 (AR) / none (NAR).
@@ -204,15 +204,9 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k<<<grid, 256, smem, s>>>((const float *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, (float *)out,
                               (float *)kcache, (float *)vcache, cache_seq_stride, cache_cap, dense_mask, dense_ld, dc);
-  } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && kcache == nullptr && getenv("VB_ATTN_SIMT") == nullptr &&
-             attention_tcgen05_enabled()) {
-    // 128-row query tiles on tcgen05/TMEM; a ragged last tile is shifted back to [L-128, L) (overlap, rows are
-    // independent) so that a length like 1025 costs 9 tiles, not 9 tiles plus a 64-row warp-level pass
-    return launch_attention_tcgen05((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                    max_seqlen, mask_mode, (bf16 *)out, 2, s);
   } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && getenv("VB_ATTN_SIMT") == nullptr) {
-    return launch_attention_mma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode,
-                                (bf16 *)out, (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, 0, s);
+    return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
+                                  mask_mode, (bf16 *)out, (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, s);
   } else if (dtype == VB_BF16) {
     auto k = attn_varlen_simt_kernel<bf16>;
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -554,8 +548,6 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   for (int i = 0; i < 8; ++i) qf[i] = qs[j8 + i];
   float lmax = -CUDART_INF_F;
   const bool new_here = has_new && pos >= c0 && pos < c1;  // the current token's key lives in smem
-  // (refilling the registers of a half batch with the next batch's rows as soon as that half is consumed -- loads always
-  //  in flight per warp -- measured the same: CTA duration 15.2 vs 15.3 us, profiles/round2_summary.md)
   for (int base = 0; base < n; base += 16 * U) {
     if (base > 0) {
 #pragma unroll
@@ -730,10 +722,9 @@ int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, in
   } else {
     // score buffer: the chunk of one split, rounded as the kernel rounds it (+16), in 1 KB steps
     const size_t sc_bytes = align_up((size_t)((cache_cap + ns - 1) / ns + 32) * sizeof(float), 1024);
-    // VB_ATTN_CARVEOUT: shared-memory carve-out (percent) preferred for this kernel; -1 = the driver's choice.  72 % =
-    // the 164 KB partition the projections of the chain run with: the driver's own pick for this (small) footprint
-    // measured 1.5-3 % slower over the AR phase (the SMs re-partition on the way in and out of every attention launch),
-    // the largest carve-out 25 % slower per launch (no L1 left for the loads in flight)
+    // VB_ATTN_CARVEOUT: shared-memory carve-out (percent) preferred for this kernel; -1 = the driver's choice.  A fixed
+    // carve-out keeps the SMs from re-partitioning on the way in and out of every attention launch of the chain; the
+    // largest carve-out leaves no L1 for the loads in flight.  (Default not re-tuned on H100.)
     static int carve_set[64];
     static bool carve_init = false;
     if (!carve_init) {

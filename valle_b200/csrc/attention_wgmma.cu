@@ -1,0 +1,250 @@
+// bf16 flash attention for packed ragged sequences (head_dim 64) on the Hopper tensor cores (wgmma / TMA /
+// mbarrier) -- the L x L attention of the 7 NAR passes, the AR prefill (which also fills the KV cache here) and the
+// training forward in bf16 mode: softmax(q k^T / 8 + mask) v with online softmax
+// (F.multi_head_attention_forward, valle/modules/activation.py:408-427; no mask for NAR
+// valle/models/valle.py:1125-1127, key-padding / causal rules of valle.py:835-861,921-925, kv_len(i) = max(S, i + 1)).
+//
+// One CTA = 128 query rows of one (sequence, head); 288 threads, two CTAs per SM (one CTA's softmax overlaps the
+// other's MMAs):
+//   warpgroups 0-1 query rows [64 g, 64 g + 64): S = Q K^T by wgmma m64n64k16 (both operands K-major in shared memory),
+//                  mask + online softmax on the accumulator fragments, O += P V by wgmma with P straight from
+//                  registers as the A operand and V as the MN-major B operand exactly as TMA lands it
+//   warp 8         TMA producer (one thread): the two 64-row Q boxes once, then 64-key K and V boxes (128B-swizzled
+//                  64 x 64 boxes of the packed [M, 3d] qkv matrix) through a kStages-deep mbarrier ring
+#include <math_constants.h>
+
+#include "common.cuh"
+#include "kernels.cuh"
+#include "sm90_ptx.cuh"
+
+namespace vb {
+namespace fa3 {
+
+using namespace tc;
+
+constexpr int HD = 64, BQ = 128, BKV = 64;
+constexpr int kThreads = 288;
+constexpr int kStages = 3;
+constexpr int kBoxBytes = 64 * HD * 2;        // 8 KB: one 64-row x 64-column bf16 box
+constexpr int kQBytes = 2 * kBoxBytes;        // 16 KB
+constexpr int kStageBytes = 2 * kBoxBytes;    // K + V
+constexpr int kSmemBytes = kQBytes + kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+
+// MN-major, 128-byte swizzle descriptor: a [K rows x 64 MN] tile stored as rows of 128 bytes (8 rows = one
+// 1024-byte swizzle atom); 1024 B between 8-row groups along K (the single 128-byte atom column along MN needs no
+// second stride)
+__device__ __forceinline__ uint64_t make_smem_desc_mn(uint32_t smem_addr) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)(1024 >> 4) << 16;
+  d |= (uint64_t)(1024 >> 4) << 32;
+  d |= (uint64_t)1 << 62;
+  return d;
+}
+__device__ __forceinline__ float ex2(float x) {  // 2^x; ex2(-inf) = 0
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+__device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
+  __nv_bfloat162 p = __floats2bfloat162_rn(lo, hi);
+  return *reinterpret_cast<uint32_t *>(&p);
+}
+
+__global__ void __launch_bounds__(kThreads, 2)
+attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
+                  const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens, int seg1_start,
+                  int mask_mode, bf16 *__restrict__ out, bf16 *__restrict__ kcache, bf16 *__restrict__ vcache,
+                  int64_t cache_seq_stride, int cache_cap) {
+  const int b = blockIdx.z, h = blockIdx.y;
+  const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
+  const int q0 = blockIdx.x * BQ;
+  if (q0 >= L) return;
+  const int S = (mask_mode != VB_MASK_FULL) ? text_lens[b] : 0;
+  const int c1 = (mask_mode >= VB_MASK_PADDED_AR) ? seg1_lens[b] : 0;
+  const int d = n_head * HD;
+  const int q_hi = min(q0 + BQ, L);
+  const int kv_max = (mask_mode == VB_MASK_VALLE_AR) ? max(S, q_hi) : L;
+  const int n_tiles = (kv_max + BKV - 1) / BKV;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *sq = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  uint8_t *ring = sq + kQBytes;
+  uint64_t *bars = reinterpret_cast<uint64_t *>(ring + kStages * kStageBytes);
+  uint64_t *q_bar = bars, *full_bar = bars + 1, *empty_bar = bars + 1 + kStages;
+
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_qkv);
+    mbar_init(q_bar, 1);
+    for (int i = 0; i < kStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 2) {
+    if (t == 0) {
+      mbar_expect_tx(q_bar, kQBytes);
+      tma_load_2d(&tmap_qkv, q_bar, sq, h * HD, r0 + q0);
+      tma_load_2d(&tmap_qkv, q_bar, sq + kBoxBytes, h * HD, r0 + q0 + 64);
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int it = 0; it < n_tiles; ++it) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t *dst = ring + stage * kStageBytes;
+        mbar_expect_tx(&full_bar[stage], kStageBytes);
+        tma_load_2d(&tmap_qkv, &full_bar[stage], dst, d + h * HD, r0 + it * BKV);
+        tma_load_2d(&tmap_qkv, &full_bar[stage], dst + kBoxBytes, 2 * d + h * HD, r0 + it * BKV);
+        if (++stage == kStages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+    }
+    return;
+  }
+
+  // ===== consumers =====
+  const int half = wg;
+  const int row_a = q0 + half * 64 + wg_row(t, 0), row_b = row_a + 8;  // the two query rows of this thread
+  const RowMask lim_a = make_row_mask(mask_mode, row_a, L, S, seg1_start, c1);
+  const RowMask lim_b = make_row_mask(mask_mode, row_b, L, S, seg1_start, c1);
+  const float sc = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+  const uint64_t qdesc = make_smem_desc(smem_u32(sq + half * kBoxBytes));
+
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m_a = -CUDART_INF_F, m_b = -CUDART_INF_F, l_a = 0.f, l_b = 0.f;
+
+  mbar_wait(q_bar, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int it = 0; it < n_tiles; ++it) {
+    const int j0 = it * BKV;
+    mbar_wait(&full_bar[stage], phase);
+    uint8_t *sk = ring + stage * kStageBytes, *sv = sk + kBoxBytes;
+    // ---- S = Q K^T (64 query rows x 64 keys per warpgroup) ----
+    float s[32];
+    const uint64_t kdesc = make_smem_desc(smem_u32(sk));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < HD / WGMMA_K; ++k) wgmma_m64n64k16(s, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    // ---- the prefill fills the KV cache: warpgroup `half` copies key tile q0 + 64 half (rows < L) ----
+    if (kcache != nullptr && j0 == q0 + half * 64) {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int idx = t + i * 128;
+        const int r = idx >> 3, c = idx & 7;
+        if (j0 + r < L) {
+          const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + j0 + r) * HD + c * 8;
+          const int so = r * 128 + ((c ^ (r & 7)) << 4);
+          *reinterpret_cast<uint4 *>(kcache + off) = *reinterpret_cast<const uint4 *>(sk + so);
+          *reinterpret_cast<uint4 *>(vcache + off) = *reinterpret_cast<const uint4 *>(sv + so);
+        }
+      }
+    }
+    // ---- mask + online softmax on the fragments: register i holds row (i >> 1) & 1 ? b : a, key wg_col(t, i) ----
+    float mx_a = -CUDART_INF_F, mx_b = -CUDART_INF_F;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int c = j0 + wg_col(t, i);
+      if ((i >> 1) & 1) {
+        s[i] = lim_b.ok(c) ? s[i] * sc : -CUDART_INF_F;
+        mx_b = fmaxf(mx_b, s[i]);
+      } else {
+        s[i] = lim_a.ok(c) ? s[i] * sc : -CUDART_INF_F;
+        mx_a = fmaxf(mx_a, s[i]);
+      }
+    }
+    mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
+    mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
+    mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
+    mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
+    const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
+    const float mu_a = mn_a == -CUDART_INF_F ? 0.f : mn_a, mu_b = mn_b == -CUDART_INF_F ? 0.f : mn_b;
+    const float corr_a = ex2(m_a - mu_a), corr_b = ex2(m_b - mu_b);
+    m_a = mn_a;
+    m_b = mn_b;
+    float rs_a = 0.f, rs_b = 0.f;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      if ((i >> 1) & 1) {
+        s[i] = ex2(s[i] - mu_b);
+        rs_b += s[i];
+        o[i] *= corr_b;
+      } else {
+        s[i] = ex2(s[i] - mu_a);
+        rs_a += s[i];
+        o[i] *= corr_a;
+      }
+    }
+    l_a = l_a * corr_a + rs_a;  // per-thread partial row sums (quad-reduced at the end)
+    l_b = l_b * corr_b + rs_b;
+    // ---- O += P V: P from registers (k-step ks = keys 16 ks .. +16 = accumulator registers 8 ks .. 8 ks + 7) ----
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      pa[ks][0] = pack_bf16(s[8 * ks + 0], s[8 * ks + 1]);
+      pa[ks][1] = pack_bf16(s[8 * ks + 2], s[8 * ks + 3]);
+      pa[ks][2] = pack_bf16(s[8 * ks + 4], s[8 * ks + 5]);
+      pa[ks][3] = pack_bf16(s[8 * ks + 6], s[8 * ks + 7]);
+    }
+    const uint64_t vdesc = make_smem_desc_mn(smem_u32(sv));
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs_tb(o, pa[ks], vdesc + (uint64_t)(ks * (16 * 128 >> 4)));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    if (++stage == kStages) {
+      stage = 0;
+      phase ^= 1;
+    }
+  }
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
+  l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 1);
+  l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+  const float inv_a = 1.f / l_a, inv_b = 1.f / l_b;
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    const bool rb = (i >> 1) & 1;
+    const int row = rb ? row_b : row_a;
+    if (row >= L) continue;
+    const float inv = rb ? inv_b : inv_a;
+    *reinterpret_cast<uint32_t *>(out + (int64_t)(r0 + row) * d + h * HD + wg_col(t, i)) =
+        pack_bf16(o[i] * inv, o[i + 1] * inv);
+  }
+}
+
+}  // namespace fa3
+
+int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
+                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                           int mask_mode, bf16 *out, bf16 *kcache, bf16 *vcache, int64_t cache_seq_stride,
+                           int cache_cap, cudaStream_t s) {
+  if (M == 0 || B == 0) return VB_OK;
+  VB_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0, "wgmma attention: qkv must be 16-byte aligned");
+  CUtensorMap tm;
+  VB_TRY(tc::make_tmap(&tm, qkv, M, 3 * n_head * fa3::HD, 3 * (int64_t)n_head * fa3::HD, 64));
+  static PerDeviceOnce once;
+  if (once.first())
+    VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fa3::kSmemBytes));
+  dim3 grid((max_seqlen + fa3::BQ - 1) / fa3::BQ, n_head, B);
+  fa3::attn_wgmma_kernel<<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(tm, n_head, cu_seqlens, text_lens, seg1_lens,
+                                                                      seg1_start, mask_mode, out, kcache, vcache,
+                                                                      cache_seq_stride, cache_cap);
+  VB_LAUNCH_CHECK();
+  return VB_OK;
+}
+
+}  // namespace vb

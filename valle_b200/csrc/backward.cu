@@ -2,7 +2,7 @@
 // valle/bin/trainer.py:674): the gradients torch.autograd would produce for the reference's modules, computed by
 // hand-written kernels behind the C ABI.
 //
-//   * GEMM gradients reuse the forward GEMM kernels (tcgen05 for bf16 operands, exact-order CUDA-core for fp32):
+//   * GEMM gradients reuse the forward GEMM kernels (wgmma for bf16 operands, exact-order CUDA-core for fp32):
 //       dgrad  dX[M,K] = dY[M,N] W[N,K]        = linear(dY, W^T)          (W^T kept by the caller per step)
 //       wgrad  dW[N,K] += dY^T[N,M] X[M,K]     = linear(dY^T, X^T) with the fp32 accumulate epilogue
 //     the two activation transposes are explicit memory-bound passes (transpose_pad_kernel);
@@ -514,7 +514,7 @@ __global__ void cast_kernel(const float *__restrict__ in, TD *__restrict__ out, 
 
 int launch_cast_from_f32(const float *in, void *out, int dtype, int64_t n, cudaStream_t s) {
   if (n == 0) return VB_OK;
-  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 148 * 16);
+  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 132 * 16);
   if (dtype == VB_F32)
     cast_kernel<float><<<grid, 256, 0, s>>>(in, (float *)out, n);
   else
@@ -551,7 +551,7 @@ int launch_colsum(const void *in, int dtype, int64_t ld, int64_t R, int N, float
 
 int launch_dropout(const void *in, void *out, int dtype, int64_t n, const DropCfg &cfg, cudaStream_t s) {
   if (n == 0) return VB_OK;
-  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 148 * 16);
+  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 132 * 16);
   if (dtype == VB_F32)
     bw::dropout_kernel<float><<<grid, 256, 0, s>>>((const float *)in, (float *)out, n, cfg);
   else
@@ -562,7 +562,7 @@ int launch_dropout(const void *in, void *out, int dtype, int64_t n, const DropCf
 
 int launch_dropout_add(float *x, const float *t, int64_t n, const DropCfg &cfg, cudaStream_t s) {
   if (n == 0) return VB_OK;
-  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 148 * 16);
+  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 132 * 16);
   bw::dropout_add_kernel<<<grid, 256, 0, s>>>(x, t, n, cfg);
   VB_LAUNCH_CHECK();
   return VB_OK;
@@ -570,7 +570,7 @@ int launch_dropout_add(float *x, const float *t, int64_t n, const DropCfg &cfg, 
 
 int launch_relu_bwd(void *dh, const void *h, int dtype, int64_t n, float scale, cudaStream_t s) {
   if (n == 0) return VB_OK;
-  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 148 * 16);
+  const unsigned grid = (unsigned)std::min<int64_t>((n + 255) / 256, 132 * 16);
   if (dtype == VB_F32)
     bw::relu_bwd_kernel<float><<<grid, 256, 0, s>>>((float *)dh, (const float *)h, n, scale);
   else

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of libvalle_b200.so.
+// Shared helpers for the sm_90a kernels of libvalle_b200.so.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -204,7 +204,7 @@ inline int sm_count() {
   if (n[slot] == 0) {
     int v = 0;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    n[slot] = v > 0 ? v : 148;
+    n[slot] = v > 0 ? v : 132;
   }
   return n[slot];
 }

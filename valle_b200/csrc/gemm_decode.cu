@@ -1,16 +1,17 @@
 // Skinny (decode) projections on the tensor cores: out[b, n] = epi( sum_k act[b,k] W[n,k] + bias[n] ),
 // b < B <= 64 rows of the AR decode step, bf16 operands, fp32 accumulate.
 //
-// HBM-bound weight streaming (AI <= 64 FLOP/B): the weight matrix is the M=128-row operand of
-// tcgen05.mma ("swap-AB"), the B <= 64 activation rows are the N=64 operand, so every weight byte is
-// read exactly once per step at full TMA throughput and 148 SMs are filled by split-K:
+// HBM-bound weight streaming (AI <= 64 FLOP/B): the weight matrix is the M operand of wgmma
+// ("swap-AB"), the B <= 64 activation rows are the N=64 operand, so every weight byte is
+// read exactly once per step at full TMA throughput and the 132 SMs are filled by split-K:
 //   grid = (N_out/128 tiles, S splits); CTA (t, s) streams W[t*128 .. +128, k-range(s)] through a
-//   TMA/mbarrier ring into tcgen05.mma (M=128, N=64, K=16), accumulates in 64 TMEM columns, and
+//   TMA/mbarrier ring into wgmma (2 x m64n64k16 per k-step), accumulates in registers, and
 //   either applies the fused epilogue itself (S == 1: +bias, ReLU -> bf16, residual, QKV scatter) or
 //   writes its fp32 partial tile to partials[split][b][n]; the CONSUMER kernel (residual + LayerNorm,
 //   the KV-cache attention prologue, the sampler) sums the S partials in fixed order 0..S-1, which
-//   keeps the result deterministic and costs no extra launch.
-//   Programmatic dependent launch: barrier/TMEM setup and the first kStages WEIGHT tiles (which do
+//   keeps the result deterministic and costs no extra launch.  A residual update of the folded chain has no
+//   consumer: the S splits of a tile form a thread-block cluster and add their tiles over DSMEM in fixed order.
+//   Programmatic dependent launch: barrier setup and the first kStages WEIGHT tiles (which do
 //   not depend on the previous kernel) are issued before griddepcontrol.wait, so weight streaming
 //   overlaps the tail of the previous kernel in the CUDA graph.
 //
@@ -20,28 +21,29 @@
 
 #include "common.cuh"
 #include "kernels.cuh"
-#include "tcgen05_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace vb {
 namespace dg {
 
+constexpr int kMaxClusterSplits = 8;  // portable thread-block cluster size
+
 using namespace tc;
 
-constexpr int TM = 128;      // weight rows per tile (UMMA M)
-constexpr int TN = 64;       // activation rows (UMMA N)
-constexpr int kStages = 6;   // (8 stages -- every weight tile of FFN1 / FFN2 in flight before the dependency wait --
-                             // measured no faster: 5.6 vs 5.3-5.6 us per launch)
+constexpr int TM = 128;      // weight rows per tile (two wgmma M=64 halves)
+constexpr int TN = 64;       // activation rows (wgmma N)
+constexpr int kStages = 6;
 constexpr int kWBytes = TM * BK * 2;  // 16 KB
 constexpr int kXBytes = TN * BK * 2;  // 8 KB
 constexpr int kStageBytes = kWBytes + kXBytes;
 constexpr int kSmemBytes = kStages * kStageBytes + 1024 + 256;
 constexpr int kThreads = 256;
-constexpr int kTmemCols = 64;
+static_assert(kStages * kStageBytes >= TN * TM * 4, "the epilogue stages the fp32 tile in the ring");
 
 struct Epi {
   int mode;  // DG_* below
-  int red;   // DG_RESIDUAL with split-K, no partials: 1 = every split adds its tile into out_f32 by a TMA bulk reduction
-             // (order of the splits not fixed), 2 = the splits of a tile are a cluster and reduce over DSMEM in fixed order
+  int red;   // DG_RESIDUAL with split-K, no partials: the splits of a tile are a thread-block cluster and add their
+             // tiles into out_f32 over DSMEM in fixed order 0..S-1 (run-to-run identical)
   int N, B;  // valid output features / rows
   const float *bias;
   float *out_f32;      // [B, ld_out] (RESIDUAL: in/out; F32: out; QKV: q)
@@ -77,15 +79,35 @@ __device__ __forceinline__ void apply_epi(const Epi &e, int n, int b, float v) {
   }
 }
 
+// swap-AB on wgmma: the weight tile is the A operand (two m64 halves), the activation rows the N = 64 B operand
+__device__ __forceinline__ void decode_mma_stage(float (&acc0)[32], float (&acc1)[32], uint32_t w_addr, uint32_t x_addr) {
+  const uint64_t a0 = make_smem_desc(w_addr), a1 = make_smem_desc(w_addr + 64 * 128), bd = make_smem_desc(x_addr);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < BK / WGMMA_K; ++k) {
+    wgmma_m64n64k16(acc0, a0 + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), 1);
+    wgmma_m64n64k16(acc1, a1 + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), 1);
+  }
+  wgmma_commit();
+}
+// accumulator fragments -> sv[b][feature] ([TN][TM] fp32, row b = activation row)
+__device__ __forceinline__ void decode_stage_tile(const float (&acc0)[32], const float (&acc1)[32], float *sv, int t) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int nl = wg_row(t, i), b = wg_col(t, i);
+    sv[b * TM + nl] = acc0[i];
+    sv[b * TM + 64 + nl] = acc1[i];
+  }
+}
+
+// 256 threads: warp 0 TMA producer, warps 1-3 KV-cache L2 prefetch, warps 4-7 the MMA warpgroup and the epilogue
 __global__ void __launch_bounds__(kThreads, 1)
-gemm_decode_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
-                   const __grid_constant__ CUtensorMap tmap_red, int num_kb, float *__restrict__ partials, int ldp,
+gemm_decode_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x, int num_kb, float *__restrict__ partials, int ldp,
                    Epi epi, KvPrefetch pf) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *bars = reinterpret_cast<uint64_t *>(tiles + kStages * kStageBytes);
-  uint64_t *full_bar = bars, *empty_bar = bars + kStages, *tmem_full = bars + 2 * kStages;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_full + 1);
+  uint64_t *full_bar = bars, *empty_bar = bars + kStages;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x, split = blockIdx.y, splits = gridDim.y;
@@ -98,25 +120,15 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmap_w);
     prefetch_tmap(&tmap_x);
-    if (epi.red) prefetch_tmap(&tmap_red);
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 4);  // one arrive per MMA warp
     }
-    mbar_init(tmem_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -145,91 +157,56 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(TM, TN);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int i = 0; i < nkb; ++i) {
-        mbar_wait(&full_bar[stage], phase);
-        tcgen05_fence_after();
-        const uint32_t w_addr = smem_u32(tiles + stage * kStageBytes);
-        const uint64_t adesc = make_smem_desc(w_addr);
-        const uint64_t bdesc = make_smem_desc(w_addr + kWBytes);
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k)
-          umma_bf16(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (i | k) != 0);
-        tcgen05_commit(&empty_bar[stage]);
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      tcgen05_commit(tmem_full);
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    const int q = warp & 3;
-    const int nl = q * 32 + lane;  // feature within the tile
-    const int n = tile * TM + nl;
-    float v[TN];
+  } else if (warp < 4) {
     // idle until the accumulator is complete: pull a slice of an upcoming layer's KV cache into L2
-    kv_prefetch(pf, (blockIdx.y * gridDim.x + blockIdx.x) * 4 + q, gridDim.x * gridDim.y * 4);
+    kv_prefetch(pf, (blockIdx.y * gridDim.x + blockIdx.x) * 3 + (warp - 1), gridDim.x * gridDim.y * 3);
     pdl_wait();
-    if (nkb > 0) {
-      mbar_wait(tmem_full, 0);
-      tcgen05_fence_after();
-      uint32_t r[32];
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16), r);
+  } else {
+    const int t = threadIdx.x - 128;
+    float acc0[32], acc1[32];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-      tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + 32u, r);
-#pragma unroll
-      for (int i = 0; i < 32; ++i) v[32 + i] = __uint_as_float(r[i]);
-    } else {
-#pragma unroll
-      for (int i = 0; i < TN; ++i) v[i] = 0.f;
+    for (int i = 0; i < 32; ++i) acc0[i] = acc1[i] = 0.f;
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
+    for (int i = 0; i < nkb; ++i) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t w_addr = smem_u32(tiles + stage * kStageBytes);
+      decode_mma_stage(acc0, acc1, w_addr, w_addr + kWBytes);
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == kStages) {
+        stage = 0;
+        phase ^= 1;
+      }
     }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc0);
+    wgmma_fence_regs(acc1);
+    pdl_wait();
+    // every TMA load has landed and every MMA has retired: the ring is free for the [TN][TM] fp32 tile
+    float *sv = reinterpret_cast<float *>(tiles);
+    decode_stage_tile(acc0, acc1, sv, t);
+    asm volatile("bar.sync 1, 128;" ::: "memory");
+    const int nl = t;  // feature within the tile
+    const int n = tile * TM + nl;
     if (splits == 1) {
-      // stage the tile through (now idle) pipeline shared memory so rows can be walked dynamically
-      float *sv = reinterpret_cast<float *>(tiles);  // [TN][TM]
-#pragma unroll
-      for (int b = 0; b < TN; ++b) sv[b * TM + nl] = v[b];
-      __syncwarp();
       if (n < epi.N)
         for (int b = 0; b < epi.B; ++b) apply_epi(epi, n, b, sv[b * TM + nl]);
-    } else if (epi.red == 1) {
-      // residual stream assembled in place: x[0:B, tile] += this split's tile (+ bias once, from split 0).  The tile
-      // is staged row-major in the (now idle) pipeline shared memory and handed to the TMA engine as ONE bulk tensor
-      // reduction (rows past B are clipped by the tensor map); per-lane red.global.add measured 2 us slower per launch.
-      float *sv = reinterpret_cast<float *>(tiles);  // [TN][TM]
-      const float bias = (split == 0 && epi.bias && n < epi.N) ? epi.bias[n] : 0.f;
-#pragma unroll
-      for (int b = 0; b < TN; ++b) sv[b * TM + nl] = v[b] + bias;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (q == 0 && lane == 0) {
-        tma_reduce_add_2d(&tmap_red, sv, tile * TM, 0);
-        tma_store_commit();
-        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // performed before this CTA retires (waiting only for
-                                                                  // the shared-memory read measured the same)
-      }
-    } else if (epi.red == 2) {
-      // deterministic variant: the CTAs of a tile (its `splits` splits) form a thread-block cluster; every CTA parks
-      // its tile in shared memory, then CTA r adds up rows [r R, (r+1) R) of all the tiles over DSMEM in fixed order
-      // 0..S-1 and updates the residual rows itself (plain read-modify-write, no atomics) -- after the barriers below
-      float *sv = reinterpret_cast<float *>(tiles);  // [TN][TM]
-#pragma unroll
-      for (int b = 0; b < TN; ++b) sv[b * TM + nl] = v[b];
-    } else {
-      // partials[split][b][n]: for a fixed row b consecutive lanes write consecutive features
+    } else if (!epi.red) {
+      // partials[split][b][n]: for a fixed row b consecutive threads write consecutive features
       float *mine = partials + (int64_t)split * TN * ldp + n;
-#pragma unroll
-      for (int b = 0; b < TN; ++b) mine[(int64_t)b * ldp] = v[b];
+#pragma unroll 8
+      for (int b = 0; b < TN; ++b) mine[(int64_t)b * ldp] = sv[b * TM + nl];
     }
+    // epi.red: the tile stays in shared memory for the cluster reduction below
   }
   __syncwarp();
-  if (epi.red == 2 && splits > 1) {
+  // residual update x[0:B, tile] += sum of the splits' tiles + bias: the CTAs of a tile (its `splits` splits) form a
+  // thread-block cluster; every CTA has parked its tile in shared memory, CTA r adds up rows [r R, (r+1) R) of all the
+  // tiles over DSMEM in fixed order 0..S-1 and updates those residual rows itself (plain read-modify-write, no atomics),
+  // so the result does not depend on which split finishes first
+  if (epi.red && splits > 1) {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
     if (warp >= 4) {
       const int nl = (warp & 3) * 32 + lane, n = tile * TM + nl;
@@ -238,22 +215,22 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
       const uint32_t sv_addr = smem_u32(tiles) + (uint32_t)nl * 4u;
       const float bias = (epi.bias && n < epi.N) ? epi.bias[n] : 0.f;
       // remote address of this thread's column in every rank's tile (rank j == split j: the cluster is a y column)
-      uint32_t ra[8];
+      uint32_t ra[kMaxClusterSplits];
 #pragma unroll
-      for (int j = 0; j < 8; ++j)
+      for (int j = 0; j < kMaxClusterSplits; ++j)
         asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra[j]) : "r"(sv_addr), "r"(min(j, splits - 1)));
 #pragma unroll 2
       for (int b = b_lo; b < b_hi; ++b) {
-        float t[8];
+        float t[kMaxClusterSplits];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {   // all ranks' values requested before the first add (DSMEM latency ~200 clocks)
+        for (int j = 0; j < kMaxClusterSplits; ++j) {   // all ranks' values requested before the first add (DSMEM latency ~200 clocks)
           t[j] = 0.f;
           if (j < splits)
             asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(t[j]) : "r"(ra[j] + (uint32_t)(b * TM * 4)) : "memory");
         }
         float acc = t[0];
 #pragma unroll
-        for (int j = 1; j < 8; ++j) acc += t[j];   // fixed order 0..S-1
+        for (int j = 1; j < kMaxClusterSplits; ++j) acc += t[j];   // fixed order 0..S-1
         if (n < epi.N) {
           float *o = epi.out_f32 + (int64_t)b * epi.ld_out + n;
           *o = *o + (acc + bias);
@@ -262,12 +239,6 @@ gemm_decode_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
     }
     // nobody leaves while its tile may still be read
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols));
   }
   vb_trace(TR_GEMM * 2 + 1);
 }
@@ -285,19 +256,15 @@ constexpr int kXfBytes = TN * BK * 4;  // 16 KB fp32 box
 constexpr int kStageBytesX = kWBytes + kXBytes + kXfBytes;  // 40 KB
 constexpr int kSmemBytesX = kStagesX * kStageBytesX + 1024 + 512;   // + alignment slack, barriers
 
-constexpr int kThreadsX = 448;  // warp 0 TMA, 1 MMA, 2..9 converters (4..7 also the epilogue), 10..13 KV prefetch
+constexpr int kThreadsX = 384;  // warp 0 TMA, 1..3 KV prefetch, 4..11 converters = the two MMA warpgroups + epilogue
 
-// (register cap of two CTAs per SM: 72 registers, no spills -- with the 4-stage ring that leaves room for three CTAs of
-//  the attention launch that follows to become resident, and fetch their first K rows, while this kernel still runs)
-__global__ void __launch_bounds__(kThreadsX, 2)
+__global__ void __launch_bounds__(kThreadsX, 1)
 gemm_decode_x_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_xf,
                      int num_kb, float *__restrict__ partials, int ldp, float *__restrict__ stats, KvPrefetch pf) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t *tiles = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t *bars = reinterpret_cast<uint64_t *>(tiles + kStagesX * kStageBytesX);
-  uint64_t *wfull = bars, *xfull = bars + kStagesX, *bfull = bars + 2 * kStagesX, *empty_bar = bars + 3 * kStagesX,
-           *tmem_full = bars + 4 * kStagesX;
-  uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(tmem_full + 1);
+  uint64_t *wfull = bars, *xfull = bars + kStagesX, *bfull = bars + 2 * kStagesX, *empty_bar = bars + 3 * kStagesX;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x, split = blockIdx.y, splits = gridDim.y;
@@ -315,20 +282,11 @@ gemm_decode_x_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_co
       mbar_init(&wfull[i], 1);
       mbar_init(&xfull[i], 1);
       mbar_init(&bfull[i], 8);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);
     }
-    mbar_init(tmem_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp == 0) {
     if (lane == 0) {
@@ -359,37 +317,21 @@ gemm_decode_x_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_co
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc(TM, TN);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int i = 0; i < nkb; ++i) {
-        mbar_wait(&wfull[stage], phase);
-        mbar_wait(&bfull[stage], phase);
-        tcgen05_fence_after();
-        const uint32_t w_addr = smem_u32(tiles + stage * kStageBytesX);
-        const uint64_t adesc = make_smem_desc(w_addr);
-        const uint64_t bdesc = make_smem_desc(w_addr + kWBytes);
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k)
-          umma_bf16(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (i | k) != 0);
-        tcgen05_commit(&empty_bar[stage]);
-        if (++stage == kStagesX) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-      tcgen05_commit(tmem_full);
-    }
-    __syncwarp();
-  } else if (warp < 10) {
-    // ---- converters: warp cw owns rows cw*8 .. +8 of every k-block; lane = (row parity, float4 of the row) ----
-    const int cw = warp - 2;
+  } else if (warp < 4) {
+    // idle warps: pull a slice of an upcoming layer's KV cache into L2 while the weight tiles stream
+    kv_prefetch(pf, (blockIdx.y * gridDim.x + blockIdx.x) * 3 + (warp - 1), gridDim.x * gridDim.y * 3);
+    pdl_wait();
+  } else {
+    // ---- converters: warp cw owns rows cw*8 .. +8 of every k-block; lane = (row parity, float4 of the row).
+    //      Once all 8 warps have converted a stage, warpgroup h (warps 4 + 4h ..) multiplies weight rows [64 h, +64).
+    const int cw = warp - 4, h = cw >> 2, t = threadIdx.x & 127;
     const int rsub = lane >> 4, f = lane & 15;
     float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};
+    float acc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
     pdl_wait();
-    int stage = 0;
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int i = 0; i < nkb; ++i) {
       mbar_wait(&xfull[stage], phase);
@@ -411,11 +353,25 @@ gemm_decode_x_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_co
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       __syncwarp();
       if (lane == 0) mbar_arrive(&bfull[stage]);
+      mbar_wait(&bfull[stage], phase);
+      mbar_wait(&wfull[stage], phase);
+      const uint32_t w_addr = smem_u32(tiles + stage * kStageBytesX) + h * (64 * 128);
+      const uint64_t adesc = make_smem_desc(w_addr), bdesc = make_smem_desc(smem_u32(xb));
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BK / WGMMA_K; ++k)
+        wgmma_m64n64k16(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
       if (++stage == kStagesX) {
         stage = 0;
         phase ^= 1;
       }
     }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
     if (tile < kLnFoldMaxCopies && stats != nullptr) {  // moments of this split's k-range: stats[tile][split][row][2]
 #pragma unroll
       for (int it = 0; it < 4; ++it) {
@@ -431,38 +387,10 @@ gemm_decode_x_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_co
         }
       }
     }
-    if (warp >= 4 && warp < 8) {  // ---- epilogue: fp32 partial tile of this split, 32 rows at a time ----
-      const int q = warp & 3;
-      const int n = tile * TM + q * 32 + lane;
-      float *mine = partials + (int64_t)split * TN * ldp + n;
-      if (nkb > 0) {
-        mbar_wait(tmem_full, 0);
-        tcgen05_fence_after();
-      }
+    // ---- epilogue: fp32 partial tile of this split, partials[split][b][n], straight from the fragments ----
+    float *mine = partials + (int64_t)split * TN * ldp + tile * TM + h * 64;
 #pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t r[32];
-        if (nkb > 0) {
-          tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 32), r);
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) r[i] = 0u;
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mine[(int64_t)(half * 32 + i) * ldp] = __uint_as_float(r[i]);
-      }
-    }
-  } else {
-    // idle warps: pull a slice of an upcoming layer's KV cache into L2 while the weight tiles stream
-    kv_prefetch(pf, (blockIdx.y * gridDim.x + blockIdx.x) * 4 + (warp - 10), gridDim.x * gridDim.y * 4);
-    pdl_wait();
-  }
-  __syncwarp();
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols));
+    for (int i = 0; i < 32; ++i) mine[(int64_t)wg_col(t, i) * ldp + wg_row(t, i)] = acc[i];
   }
   vb_trace(TR_GEMM * 2 + 1);
 }
@@ -495,22 +423,20 @@ int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, in
   const int tiles = (N + dg::TM - 1) / dg::TM;
   const int num_kb = K / tc::BK;
   int splits = force_splits > 0 ? std::min(force_splits, std::min(kMaxForcedSplits, num_kb)) : pick_splits(tiles, num_kb);
+  // the splits of a residual update form one thread-block cluster: at most the portable cluster size
+  if (red_add) splits = std::min(splits, dg::kMaxClusterSplits);
   const int ldp = tiles * dg::TM;
   if (splits > 1 && !red_add)
     VB_CHECK_ARG(partials && partial_bytes >= (size_t)splits * dg::TN * ldp * sizeof(float),
                  "gemm_decode: partial buffer too small");
   if (out_splits) *out_splits = red_add ? 1 : splits;  // nothing left for a consumer to add up
   if (out_ldp) *out_ldp = ldp;
-  CUtensorMap tw, tx, tr;
+  CUtensorMap tw, tx;
   VB_TRY(tc::make_tmap(&tw, W, N, K, K, dg::TM));
   VB_TRY(tc::make_tmap(&tx, act, B, K, ld_act, dg::TN));
-  if (red_add && splits > 1)
-    VB_TRY(tc::make_tmap_f32_dense(&tr, out_f32, B, N, ld_out, dg::TN, dg::TM));
-  else
-    tr = tw;  // unused
   dg::Epi e{};
   e.mode = mode; e.N = N; e.B = B; e.bias = bias;
-  e.red = (red_add && splits > 1) ? (tune("VB_RED_MODE", 1) == 2 && splits <= 8 ? 2 : 1) : 0;
+  e.red = red_add && splits > 1;
   e.out_f32 = out_f32; e.out_bf16 = out_bf16; e.ld_out = ld_out;
   if (mode == DG_QKV && splits == 1) {
     VB_CHECK_ARG(qkv != nullptr, "gemm_decode: qkv scatter parameters missing");
@@ -529,14 +455,12 @@ int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, in
   KvPrefetch pf0{};
   if (pf) pf0 = *pf;
   VB_CUDA(launch_kernel_cluster(dg::gemm_decode_kernel, dim3(tiles, splits), dim3(dg::kThreads), dg::kSmemBytes, s, pdl,
-                                dim3(1, e.red == 2 ? splits : 1, 1), tw, tx, tr, num_kb, partials, ldp, e, pf0));
+                                dim3(1, e.red ? splits : 1, 1), tw, tx, num_kb, partials, ldp, e, pf0));
   count_launch();
   return VB_OK;
 }
 
 // projection of the fp32 rows x[B, K] by LayerNorm-folded weights: fp32 partial tiles + the rows' moments per split
-// (linear1 + ReLU finished inside this launch -- the splits of a tile as a thread-block cluster reducing over DSMEM --
-//  was built and measured slower: 9.5 + 8.2 us for FFN1 + FFN2 against 5.0 + 2.7 + 7.4 us with relu_reduce_kernel)
 int launch_gemm_decode_x(const float *x, int B, int64_t ldx, const bf16 *Wf, int N, int K, int force_splits,
                          float *partials, size_t partial_bytes, float *stats, int *out_splits, int *out_ldp,
                          int *out_copies, const KvPrefetch *pf, bool pdl, cudaStream_t s) {

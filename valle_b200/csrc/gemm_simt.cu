@@ -1,7 +1,7 @@
 // CUDA-core (FFMA) linear layers:
 //   * gemm_simt_kernel : C[M,N] = epi(A[M,K] W[N,K]^T + b), fp32 accumulate in fixed k order.
 //     This is the exact-order path used for fp32 parity (greedy tokens bit-exact vs the
-//     reference) and for shapes the tcgen05 kernel does not take (N=1025 head, tiny K).
+//     reference) and for shapes the wgmma kernel does not take (N=1025 head, tiny K).
 //   * gemv_kernel      : skinny M (decode rows, M<=64), weight-streaming, HBM-bound.  One warp
 //     per output column, 16-byte streaming loads of W, activations (optionally LayerNorm'ed in
 //     the prologue) staged in shared memory, warp-shuffle reduction.

@@ -61,7 +61,7 @@ __device__ __forceinline__ RowMask make_row_mask(int mode, int qr, int L, int S,
 // L2 prefetch of a slice of an upcoming layer's K and V cache, issued by the otherwise idle warps of the
 // split-K decode projections (gemm_decode.cu) while their weight tiles stream: the projection chain is latency
 // bound and leaves HBM mostly idle, the KV-cache attention that follows is HBM bound -- the slice [lo_pct, hi_pct)
-// of every (utterance, head) stream is pulled into the 126 MB L2 ahead of it.  Only a hint: the lengths may be
+// of every (utterance, head) stream is pulled into the 50 MB L2 ahead of it.  Only a hint: the lengths may be
 // one step stale (read before the dependency wait), which changes what is prefetched, never what is computed.
 struct KvPrefetch {
   const void *kbase, *vbase;  // caches of the target layer ([B, H, cap, 64]) or nullptr
@@ -124,12 +124,12 @@ int launch_gemv(const float *x, int64_t ldx, int B, const void *W, int w_dtype, 
                 int N, int K, float *out, int64_t ldo, const LnParams *ln, int epi_mode,
                 const QkvScatter *qkv, cudaStream_t s);
 
-// gemm_tcgen05.cu
-bool tcgen05_gemm_supported(int64_t M, int N, int K, int64_t lda, int64_t ldc);
-int launch_gemm_tcgen05(const bf16 *A, int64_t lda, const bf16 *W, const float *bias, void *C,
-                        int c_dtype, int64_t ldc, int64_t M, int N, int K, int epi, cudaStream_t s);
+// gemm_wgmma.cu
+bool wgmma_gemm_supported(int64_t M, int N, int K, int64_t lda, int64_t ldc);
+int launch_gemm_wgmma(const bf16 *A, int64_t lda, const bf16 *W, const float *bias, void *C,
+                      int c_dtype, int64_t ldc, int64_t M, int N, int K, int epi, cudaStream_t s);
 
-// gemm_decode.cu (swap-AB split-K tcgen05 projections for B <= 64 decode rows, bf16)
+// gemm_decode.cu (swap-AB split-K wgmma projections for B <= 64 decode rows, bf16)
 enum { DG_F32 = 0, DG_RESIDUAL = 1, DG_RELU_BF16 = 2, DG_QKV = 3 };
 constexpr int kMaxForcedSplits = 16;  // cap of a caller-chosen split-K count (sizes the partial workspace)
 size_t gemm_decode_workspace(int d_model, int d_ff);
@@ -150,7 +150,7 @@ struct LnFoldStats {
 constexpr int kLnFoldMaxCopies = 32;
 // Called by every lane of a (converged) warp whose threads share the row b: lane s fetches split s's pair, the warp
 // adds them up by shuffles -- ONE L2 round trip.  (A per-thread loop over the splits, however it is unrolled, ends up
-// as `splits` dependent round trips under the register caps of the consumer kernels: 2.3 us in the attention prologue.)
+// as `splits` dependent round trips under the register caps of the consumer kernels.)
 __device__ __forceinline__ float2 ln_fold_moments_load(const LnFoldStats &f, int b, int which) {
   const int lane = threadIdx.x & 31;
   const float *st = f.stats + (int64_t)(which % f.copies) * f.splits * 64 * 2;
@@ -182,16 +182,11 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
                             int seg1_start, int max_seqlen, int mask_mode, void *out, void *kcache, void *vcache,
                             int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
                             cudaStream_t s, const DropCfg *drop = nullptr);
-// attention_mma.cu (bf16 tensor-core flash attention)
-int launch_attention_mma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
-                         const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                         int mask_mode, bf16 *out, bf16 *kcache,
-                         bf16 *vcache, int64_t cache_seq_stride, int cache_cap, int tail_of_128, cudaStream_t s);
-// attention_tcgen05.cu (bf16 flash attention on tcgen05/TMEM; no KV-cache fill)
-bool attention_tcgen05_enabled();
-int launch_attention_tcgen05(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
-                             const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                             int mask_mode, bf16 *out, int skip_partial, cudaStream_t s);
+// attention_wgmma.cu (bf16 flash attention on wgmma / TMA; fills the KV cache when kcache != nullptr)
+int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
+                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                           int mask_mode, bf16 *out, bf16 *kcache, bf16 *vcache, int64_t cache_seq_stride,
+                           int cache_cap, cudaStream_t s);
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
 int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, int qkv_ldp, const float *qkv_bias,
                        int B, int n_head, int head_dim, void *kcache, void *vcache, int dtype,

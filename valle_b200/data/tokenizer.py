@@ -1,6 +1,6 @@
 """AudioTokenizer with the reference's interface (valle/data/tokenizer.py:211-254): EnCodec 24 kHz at
 6 kbps (8 codebooks of 1024), `.encode(wav) -> [(codes [B, 8, T'], None)]`, `.decode(frames) -> wav`,
-`.sample_rate`, `.channels`, `.device` -- running on the sm_100a kernels of libvalle_b200.so
+`.sample_rate`, `.channels`, `.device` -- running on the sm_90a kernels of libvalle_b200.so
 (`csrc/encodec.cu`: SConv1d / SConvTranspose1d with reflect padding and ELU pre-activation, the
 2-layer LSTM, the 8-stage residual VQ; `vb_linear` for the LSTM input projections, `vb_embed_sum`
 for the RVQ decode).

@@ -42,7 +42,7 @@ def get_model(params) -> nn.Module:
     name = params.model_name.lower()
     if name not in ("vall-e", "valle"):
         raise NotImplementedError(
-            f"valle_b200.get_model: model_name={params.model_name!r}: only VALL-E is on the B200 hot path "
+            f"valle_b200.get_model: model_name={params.model_name!r}: only VALL-E is on the H100 hot path "
             "(VALL-F and the debug Transformer are out of scope, SURVEY.md section 2 rows 1/7)")
     return VALLE(params.decoder_dim, params.nhead, params.num_decoder_layers, norm_first=params.norm_first,
                  add_prenet=params.add_prenet, prefix_mode=params.prefix_mode,

@@ -1,6 +1,6 @@
 """VALLE with the reference's constructor, parameter names / shapes (checkpoint layout), init order
 and `forward()` / `inference()` / `continual()` signatures (valle/models/valle.py:722-1238), so
-`bin/infer.py` and `bin/trainer.py` call it unchanged -- the loops underneath run on the sm_100a
+`bin/infer.py` and `bin/trainer.py` call it unchanged -- the loops underneath run on the sm_90a
 engine (`valle_b200.engine.ValleEngine`, libvalle_b200.so).  No CPU fallback.
 """
 from __future__ import annotations

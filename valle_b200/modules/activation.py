@@ -1,5 +1,5 @@
 """MultiheadAttention with the reference's constructor, parameter names and init order
-(valle/modules/activation.py:12-197); forward = sm_100a kernels (packed in-proj GEMM,
+(valle/modules/activation.py:12-197); forward = sm_90a kernels (packed in-proj GEMM,
 ragged attention, out-proj GEMM).  Self-attention, batch_first, the masks of the VALL-E path.
 """
 from __future__ import annotations

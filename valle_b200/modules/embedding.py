@@ -1,5 +1,5 @@
 """TokenEmbedding / SinePositionalEmbedding with the reference's constructor signatures,
-parameter names (checkpoint layout) and init order -- forward runs on the sm_100a kernels.
+parameter names (checkpoint layout) and init order -- forward runs on the sm_90a kernels.
 
 Mirrors valle/modules/embedding.py:21-97 (interface); arithmetic: csrc/embed_norm.cu.
 """

@@ -1,4 +1,4 @@
-"""VALLE.forward (training loss, valle/models/valle.py:762-959) on the sm_100a kernels.
+"""VALLE.forward (training loss, valle/models/valle.py:762-959) on the sm_90a kernels.
 
 Embeddings + sine PE, the AR stack over padded [text | audio] rows with the merged causal / key-padding rule, one
 NAR stage with AdaLN, the prediction heads (tensor-core GEMMs in bf16 mode), cross-entropy and top-10 accuracy.
