@@ -530,12 +530,15 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     // partial sums are consumed by the next kernel in the chain (7 launches per layer, PDL-chained)
     const bool pdl = use_pdl();
     // Split-K wide enough to fill the SMs is not the optimum for the projections whose partial sums a reduce kernel
-    // has to add up again, hence the fixed split counts below; the share of the KV streams prefetched into L2 is
-    // smaller in the folded chain, which leaves the projections less time ahead of the attention launch.  These
-    // defaults have not been re-tuned on H100 (VB_SPLITS_* / VB_KV_PREFETCH_PCT override them).
+    // has to add up again, hence the fixed split counts below (not re-tuned on H100; VB_SPLITS_* override them).
     const bool fold_on = dec->fold_qkv && dec->fold_ffn1 && head->fold.wf && tune("VB_DECODE_FOLD", 1) != 0;
-    const int pf_env = tune("VB_KV_PREFETCH_PCT", fold_on ? 35 : 40);
-    const int pf_pct = B >= 16 ? pf_env : 0;
+    // KV prefetch budget: a share of the L2 that one layer's weights, streaming through it at the same time, leave
+    // free (VB_KV_PREFETCH_L2_PCT, DESIGN section 7), spread evenly over the B x H streams as their leading rows.
+    // Lines evicted before the attention reads them would cost their HBM bytes twice.
+    const int64_t layer_w_bytes = (4 * (int64_t)d * d + 2 * (int64_t)d * dff) * (int64_t)ts;
+    const int64_t pf_budget = B >= 16 ? std::max<int64_t>(0, l2_bytes() - layer_w_bytes) *
+                                            tune("VB_KV_PREFETCH_L2_PCT", 60) / 100 : 0;
+    const int pf_rows = (int)std::min<int64_t>(st->cache_cap, pf_budget / (2 * (int64_t)B * D.n_head * hd * ts));
     const int qkv_env = tune("VB_SPLITS_QKV", 0);
     const int out_splits = tune("VB_SPLITS_OUT", 0);   // 0 = fill the SMs
     const int ffn1_env = tune("VB_SPLITS_FFN1", 0);
@@ -547,18 +550,18 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     const int ffn1_splits = ffn1_env > 0 ? ffn1_env : std::max(1, std::min(2, d / 128));
     float *P = (float *)w.gemm_ws;
     Pending pend;
-    // the four projections of the chain each prefetch a quarter of the first pf_pct % of the KV streams that the
+    // the four projections of the chain each prefetch a quarter of the first pf_rows rows of the KV streams that the
     // NEXT attention launch will read (QKV: this layer's, the other three: the following layer's)
     auto kv_slice = [&](int layer, int quarter) {
       KvPrefetch pf{};
-      if (pf_pct <= 0) return pf;
+      if (pf_rows <= 0) return pf;
       layer %= D.n_layer;
       pf.kbase = (char *)st->kcache + (size_t)layer * st->cache_layer_stride * ts;
       pf.vbase = (char *)st->vcache + (size_t)layer * st->cache_layer_stride * ts;
       pf.seq_stride_bytes = (int64_t)st->cache_seq_stride * (int64_t)ts;
       pf.B = B; pf.H = D.n_head; pf.cap = st->cache_cap; pf.row_bytes = (int)(hd * ts);
       pf.text_len = st->text_len; pf.prompt_len = st->prompt_len; pf.n_gen = st->n_gen;
-      pf.lo_pct = pf_pct * quarter / 4; pf.hi_pct = pf_pct * (quarter + 1) / 4;
+      pf.row_lo = pf_rows * quarter / 4; pf.row_hi = pf_rows * (quarter + 1) / 4;
       return pf;
     };
     if (fold_on) {

@@ -429,8 +429,11 @@ attn_decode_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, T *_
 // of K rows fetched ahead of the q/k/v prologue (and, with the fused QKV prologue, ahead of the dependency wait)
 // and the first batch of V rows fetched ahead of the block softmax: all CTAs of the single wave run their phases
 // in lock step, so without this the HBM pipe idles through every prologue / softmax / epilogue of the launch.
+// 8 CTAs per SM (<= 64 registers, which holds U = 4 K / V rows per thread without spilling): the 1,024 CTAs of B=64 x
+// 16 heads are then resident at once on the H100's 132 SMs.  At 7 per SM (U = 8, 72 registers) 100 of them waited for
+// the first wave to drain and then streamed their whole K and V alone.
 template <int U>
-__global__ void __launch_bounds__(128, 7)
+__global__ void __launch_bounds__(128, 8)
 attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, bf16 *__restrict__ kcache,
                    bf16 *__restrict__ vcache, int64_t cache_seq_stride, int cache_cap,
                    const int32_t *__restrict__ text_len, const int32_t *__restrict__ prompt_len,
@@ -439,7 +442,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
                    float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit) {
   // score buffer of the chunk: dynamic shared memory sized by the launch (cache_cap / nsplit keys), so that the
   // kernel's footprint -- and with it the shared-memory carve-out the driver picks, i.e. how much L1 is left to land
-  // the ~110 KB of K / V loads an SM keeps in flight -- follows the actual context instead of the 4096-key maximum
+  // the ~64 KB of K / V loads an SM keeps in flight -- follows the actual context instead of the 4096-key maximum
   extern __shared__ float sc[];
   __shared__ __align__(16) float qs[HD];
   __shared__ __align__(16) float knew[HD];
@@ -737,10 +740,10 @@ int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, in
     if (carve_set[dev & 63] != carve) {
       const int want = carve >= 0 ? carve : (int)cudaSharedmemCarveoutDefault;
       if (carve >= 0 || carve_set[dev & 63] != -2)
-        VB_CUDA(cudaFuncSetAttribute(attn_decode_2phase_pf_kernel<8>, cudaFuncAttributePreferredSharedMemoryCarveout, want));
+        VB_CUDA(cudaFuncSetAttribute(attn_decode_2phase_pf_kernel<4>, cudaFuncAttributePreferredSharedMemoryCarveout, want));
       carve_set[dev & 63] = carve;
     }
-    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<8>, grid, dim3(128), sc_bytes, s, pdl, q, qp, n_head,
+    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<4>, grid, dim3(128), sc_bytes, s, pdl, q, qp, n_head,
                           (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, text_len, prompt_len, n_gen,
                           finished, out, (bf16 *)out16, part_o, part_ml, ns));
   }

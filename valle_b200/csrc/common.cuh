@@ -208,6 +208,19 @@ inline int sm_count() {
   }
   return n[slot];
 }
+// L2 size in bytes of the CURRENT device (cached per device)
+inline int64_t l2_bytes() {
+  static int64_t n[64] = {0};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int slot = dev & 63;
+  if (n[slot] == 0) {
+    int v = 0;
+    cudaDeviceGetAttribute(&v, cudaDevAttrL2CacheSize, dev);
+    n[slot] = v > 0 ? v : (int64_t)50 << 20;
+  }
+  return n[slot];
+}
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is per (function, device): remember which devices were done
 struct PerDeviceOnce {

@@ -60,15 +60,16 @@ __device__ __forceinline__ RowMask make_row_mask(int mode, int qr, int L, int S,
 
 // L2 prefetch of a slice of an upcoming layer's K and V cache, issued by the otherwise idle warps of the
 // split-K decode projections (gemm_decode.cu) while their weight tiles stream: the projection chain is latency
-// bound and leaves HBM mostly idle, the KV-cache attention that follows is HBM bound -- the slice [lo_pct, hi_pct)
-// of every (utterance, head) stream is pulled into the 50 MB L2 ahead of it.  Only a hint: the lengths may be
-// one step stale (read before the dependency wait), which changes what is prefetched, never what is computed.
+// bound and leaves HBM mostly idle, the KV-cache attention that follows is HBM bound -- rows [row_lo, row_hi) of
+// every (utterance, head) stream (the leading rows, where every CTA of the attention starts) are pulled into L2
+// ahead of it.  Only a hint: the lengths may be one step stale (read before the dependency wait),
+// which changes what is prefetched, never what is computed.
 struct KvPrefetch {
   const void *kbase, *vbase;  // caches of the target layer ([B, H, cap, 64]) or nullptr
   int64_t seq_stride_bytes;   // bytes between utterances
   int B, H, cap, row_bytes;   // row_bytes = 64 * element size
   const int32_t *text_len, *prompt_len, *n_gen;
-  int lo_pct, hi_pct;
+  int row_lo, row_hi;
 };
 // worker = one warp; `n_workers` warps of the grid share the streams.  Lane i of a warp fetches the lengths of the
 // warp's i-th stream up front (the three dependent global loads per stream would otherwise serialise the loop).
@@ -94,7 +95,7 @@ __device__ __forceinline__ void kv_prefetch(const KvPrefetch &pf, int worker, in
     }
     const int pair = sidx >> 1;
     const int b = pair / pf.H, h = pair - b * pf.H;
-    const int r_lo = kv * pf.lo_pct / 100, r_hi = kv * pf.hi_pct / 100;
+    const int r_lo = min(kv, pf.row_lo), r_hi = min(kv, pf.row_hi);
     const char *p = (const char *)((sidx & 1) ? pf.vbase : pf.kbase) + (int64_t)b * pf.seq_stride_bytes +
                     ((int64_t)h * pf.cap + r_lo) * pf.row_bytes;
     const int lines = ((r_hi - r_lo) * pf.row_bytes) >> 7;  // 128-byte lines
