@@ -1,4 +1,5 @@
-"""Microbenchmark of the wgmma GEMM on the NAR shapes of BASELINE.json configs[2] (B=32 x L=1500).
+"""Microbenchmark of the wgmma GEMM on the NAR projection shapes: python tools/bench_gemm.py [M]
+M defaults to 48,000 (BASELINE.json configs[2], B=32 x L=1500); bench.py's NAR runs at M = 64 x 1,025 = 65,600.
 CUDA-event timing, L2 flushed between iterations by the shapes themselves (A+C > 50 MB)."""
 import json
 import os
@@ -12,7 +13,8 @@ from valle_b200 import _lib as L, ops  # noqa: E402
 dev = "cuda:0"
 M = int(sys.argv[1]) if len(sys.argv) > 1 else 48000
 shapes = [("qkv", 3072, 1024, L.VB_EPI_NONE, torch.bfloat16), ("out_proj", 1024, 1024, L.VB_EPI_RESIDUAL, torch.float32),
-          ("ffn1", 4096, 1024, L.VB_EPI_RELU, torch.bfloat16), ("ffn2", 1024, 4096, L.VB_EPI_RESIDUAL, torch.float32)]
+          ("ffn1", 4096, 1024, L.VB_EPI_RELU, torch.bfloat16), ("ffn2", 1024, 4096, L.VB_EPI_RESIDUAL, torch.float32),
+          ("head", 1024, 1024, L.VB_EPI_NONE, torch.float32)]
 res = {}
 for name, N, K, epi, cdt in shapes:
     a = torch.randn(M, K, device=dev).bfloat16()
