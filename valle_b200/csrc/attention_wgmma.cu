@@ -4,13 +4,18 @@
 // (F.multi_head_attention_forward, valle/modules/activation.py:408-427; no mask for NAR
 // valle/models/valle.py:1125-1127, key-padding / causal rules of valle.py:835-861,921-925, kv_len(i) = max(S, i + 1)).
 //
-// One CTA = 128 query rows of one (sequence, head); 288 threads, two CTAs per SM (one CTA's softmax overlaps the
+// One CTA = 128 query rows of one (sequence, head); 256 threads, two CTAs per SM (one CTA's softmax overlaps the
 // other's MMAs):
 //   warpgroups 0-1 query rows [64 g, 64 g + 64): S = Q K^T by wgmma m64n64k16 (both operands K-major in shared memory),
 //                  mask + online softmax on the accumulator fragments, O += P V by wgmma with P straight from
-//                  registers as the A operand and V as the MN-major B operand exactly as TMA lands it
-//   warp 8         TMA producer (one thread): the two 64-row Q boxes once, then 64-key K and V boxes (128B-swizzled
-//                  64 x 64 boxes of the packed [M, 3d] qkv matrix) through a kStages-deep mbarrier ring
+//                  registers as the A operand and V as the MN-major B operand exactly as TMA lands it.  Key tiles
+//                  that every row of the warpgroup sees skip the mask tests; a warp whose row maxima did not move
+//                  skips the rescale of O; a warpgroup whose 64 rows all lie past the sequence exits at once.
+//   thread 0       also issues the TMA: the Q boxes once, then 64-key K and V boxes (128B-swizzled 64 x 64 boxes of
+//                  the packed [M, 3d] qkv matrix) through a kStages-deep mbarrier ring.  Without a separate producer
+//                  warp the CTA is 8 warps, so two CTAs per SM may use 128 registers per thread (no spills).
+// Every query row gets the arithmetic of the plain masked loop (same tiles, mask decisions, expressions and wgmma
+// order), so the outputs are bitwise those of that loop; tests/test_attention_bitwise_gpu.py pins them.
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -23,8 +28,8 @@ namespace fa3 {
 using namespace tc;
 
 constexpr int HD = 64, BQ = 128, BKV = 64;
-constexpr int kThreads = 288;
-constexpr int kStages = 3;
+constexpr int kThreads = 256;
+constexpr int kStages = 4;
 constexpr int kBoxBytes = 64 * HD * 2;        // 8 KB: one 64-row x 64-column bf16 box
 constexpr int kQBytes = 2 * kBoxBytes;        // 16 KB
 constexpr int kStageBytes = 2 * kBoxBytes;    // K + V
@@ -51,6 +56,52 @@ __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   return *reinterpret_cast<uint32_t *>(&p);
 }
 
+// Scale (and, for kMask, mask) one 64-key tile of scores, then the online-softmax update of the thread's two rows:
+// s becomes P = 2^(s sc - m), l the per-thread partial row sums; corr is the factor O has to be rescaled by.
+// Register i of s holds row (i >> 1) & 1 ? b : a, key j0 + wg_col(t, i).  The scale is a separate rounded multiply
+// (never contracted with the subtraction that follows).
+template <bool kMask>
+__device__ __forceinline__ void online_softmax(float (&s)[32], int j0, int t, const RowMask &lim_a,
+                                               const RowMask &lim_b, float &m_a, float &m_b, float &l_a, float &l_b,
+                                               float &corr_a, float &corr_b) {
+  const float sc = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+  float mx_a = -CUDART_INF_F, mx_b = -CUDART_INF_F;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const int c = j0 + wg_col(t, i);
+    if ((i >> 1) & 1) {
+      s[i] = (!kMask || lim_b.ok(c)) ? __fmul_rn(s[i], sc) : -CUDART_INF_F;
+      mx_b = fmaxf(mx_b, s[i]);
+    } else {
+      s[i] = (!kMask || lim_a.ok(c)) ? __fmul_rn(s[i], sc) : -CUDART_INF_F;
+      mx_a = fmaxf(mx_a, s[i]);
+    }
+  }
+  mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
+  mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
+  mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
+  mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
+  const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
+  const float mu_a = mn_a == -CUDART_INF_F ? 0.f : mn_a, mu_b = mn_b == -CUDART_INF_F ? 0.f : mn_b;
+  corr_a = ex2(m_a - mu_a);
+  corr_b = ex2(m_b - mu_b);
+  m_a = mn_a;
+  m_b = mn_b;
+  float rs_a = 0.f, rs_b = 0.f;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    if ((i >> 1) & 1) {
+      s[i] = ex2(s[i] - mu_b);
+      rs_b += s[i];
+    } else {
+      s[i] = ex2(s[i] - mu_a);
+      rs_a += s[i];
+    }
+  }
+  l_a = l_a * corr_a + rs_a;  // per-thread partial row sums (quad-reduced at the end)
+  l_b = l_b * corr_b + rs_b;
+}
+
 __global__ void __launch_bounds__(kThreads, 2)
 attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
                   const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens, int seg1_start,
@@ -74,121 +125,90 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
   uint64_t *q_bar = bars, *full_bar = bars + 1, *empty_bar = bars + 1 + kStages;
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const int n_wg = q0 + 64 < L ? 2 : 1;  // consumer warpgroups with at least one query row
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_qkv);
     mbar_init(q_bar, 1);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 8);  // one arrive per consumer warp
+      mbar_init(&empty_bar[i], 4 * n_wg);  // one arrive per working consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
 
-  if (wg == 2) {
-    if (t == 0) {
-      mbar_expect_tx(q_bar, kQBytes);
-      tma_load_2d(&tmap_qkv, q_bar, sq, h * HD, r0 + q0);
-      tma_load_2d(&tmap_qkv, q_bar, sq + kBoxBytes, h * HD, r0 + q0 + 64);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = 0; it < n_tiles; ++it) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t *dst = ring + stage * kStageBytes;
-        mbar_expect_tx(&full_bar[stage], kStageBytes);
-        tma_load_2d(&tmap_qkv, &full_bar[stage], dst, d + h * HD, r0 + it * BKV);
-        tma_load_2d(&tmap_qkv, &full_bar[stage], dst + kBoxBytes, 2 * d + h * HD, r0 + it * BKV);
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
-      }
-    }
-    return;
+  // TMA of key tile `k` into ring stage k % kStages, once every warp has released the tile kStages before it
+  auto load_tile = [&](int k) {
+    const int stg = k % kStages;
+    mbar_wait(&empty_bar[stg], ((k / kStages) & 1) ^ 1);
+    uint8_t *dst = ring + stg * kStageBytes;
+    mbar_expect_tx(&full_bar[stg], kStageBytes);
+    tma_load_2d(&tmap_qkv, &full_bar[stg], dst, d + h * HD, r0 + k * BKV);
+    tma_load_2d(&tmap_qkv, &full_bar[stg], dst + kBoxBytes, 2 * d + h * HD, r0 + k * BKV);
+  };
+  if (threadIdx.x == 0) {
+    mbar_expect_tx(q_bar, n_wg * kBoxBytes);
+    tma_load_2d(&tmap_qkv, q_bar, sq, h * HD, r0 + q0);
+    if (n_wg == 2) tma_load_2d(&tmap_qkv, q_bar, sq + kBoxBytes, h * HD, r0 + q0 + 64);
+    for (int k = 0; k < min(kStages, n_tiles); ++k) load_tile(k);
   }
+  // no rows, and no key tile of the KV cache to copy (that is tile q0 + 64 >= L)
+  if (wg >= n_wg) return;
 
   // ===== consumers =====
   const int half = wg;
   const int row_a = q0 + half * 64 + wg_row(t, 0), row_b = row_a + 8;  // the two query rows of this thread
   const RowMask lim_a = make_row_mask(mask_mode, row_a, L, S, seg1_start, c1);
   const RowMask lim_b = make_row_mask(mask_mode, row_b, L, S, seg1_start, c1);
-  const float sc = 0.125f * 1.4426950408889634f;  // 1/sqrt(64) * log2(e)
+  // every row of the warpgroup sees keys [0, kfree): lim0 does not decrease with the row in any mask mode, so the
+  // warpgroup's first row has the smallest.  Tiles below it skip the mask tests (they would all pass).
+  const int kfree = make_row_mask(mask_mode, q0 + half * 64, L, S, seg1_start, c1).lim0;
   const uint64_t qdesc = make_smem_desc(smem_u32(sq + half * kBoxBytes));
 
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m_a = -CUDART_INF_F, m_b = -CUDART_INF_F, l_a = 0.f, l_b = 0.f;
+  uint32_t pa[4][4];  // P as bf16 pairs (k-step ks = keys 16 ks .. +16 = s[8 ks .. 8 ks + 7])
 
-  mbar_wait(q_bar, 0);
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int it = 0; it < n_tiles; ++it) {
-    const int j0 = it * BKV;
-    mbar_wait(&full_bar[stage], phase);
-    uint8_t *sk = ring + stage * kStageBytes, *sv = sk + kBoxBytes;
-    // ---- S = Q K^T (64 query rows x 64 keys per warpgroup) ----
-    float s[32];
+  // S = Q K^T of one tile (64 query rows x 64 keys per warpgroup)
+  auto issue_qk = [&](float (&s)[32], const uint8_t *sk) {
     const uint64_t kdesc = make_smem_desc(smem_u32(sk));
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < HD / WGMMA_K; ++k) wgmma_m64n64k16(s, qdesc + (uint64_t)(k * 2), kdesc + (uint64_t)(k * 2), k != 0);
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-    // ---- the prefill fills the KV cache: warpgroup `half` copies key tile q0 + 64 half (rows < L) ----
-    if (kcache != nullptr && j0 == q0 + half * 64) {
+  };
+  // O += P V of the tile in ring stage `stg` (P from registers, pa)
+  auto issue_pv = [&](int stg) {
+    const uint64_t vdesc = make_smem_desc_mn(smem_u32(ring + stg * kStageBytes + kBoxBytes));
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int idx = t + i * 128;
-        const int r = idx >> 3, c = idx & 7;
-        if (j0 + r < L) {
-          const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + j0 + r) * HD + c * 8;
-          const int so = r * 128 + ((c ^ (r & 7)) << 4);
-          *reinterpret_cast<uint4 *>(kcache + off) = *reinterpret_cast<const uint4 *>(sk + so);
-          *reinterpret_cast<uint4 *>(vcache + off) = *reinterpret_cast<const uint4 *>(sv + so);
-        }
+    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs_tb(o, pa[ks], vdesc + (uint64_t)(ks * (16 * 128 >> 4)));
+    wgmma_commit();
+  };
+  // the prefill fills the KV cache: warpgroup `half` copies key tile q0 + 64 half (rows < L)
+  auto fill_cache = [&](int j0, const uint8_t *sk) {
+    if (kcache == nullptr || j0 != q0 + half * 64) return;
+    const uint8_t *sv = sk + kBoxBytes;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int idx = t + i * 128;
+      const int r = idx >> 3, c = idx & 7;
+      if (j0 + r < L) {
+        const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + j0 + r) * HD + c * 8;
+        const int so = r * 128 + ((c ^ (r & 7)) << 4);
+        *reinterpret_cast<uint4 *>(kcache + off) = *reinterpret_cast<const uint4 *>(sk + so);
+        *reinterpret_cast<uint4 *>(vcache + off) = *reinterpret_cast<const uint4 *>(sv + so);
       }
     }
-    // ---- mask + online softmax on the fragments: register i holds row (i >> 1) & 1 ? b : a, key wg_col(t, i) ----
-    float mx_a = -CUDART_INF_F, mx_b = -CUDART_INF_F;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int c = j0 + wg_col(t, i);
-      if ((i >> 1) & 1) {
-        s[i] = lim_b.ok(c) ? s[i] * sc : -CUDART_INF_F;
-        mx_b = fmaxf(mx_b, s[i]);
-      } else {
-        s[i] = lim_a.ok(c) ? s[i] * sc : -CUDART_INF_F;
-        mx_a = fmaxf(mx_a, s[i]);
-      }
-    }
-    mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 1));
-    mx_a = fmaxf(mx_a, __shfl_xor_sync(0xffffffffu, mx_a, 2));
-    mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 1));
-    mx_b = fmaxf(mx_b, __shfl_xor_sync(0xffffffffu, mx_b, 2));
-    const float mn_a = fmaxf(m_a, mx_a), mn_b = fmaxf(m_b, mx_b);
-    const float mu_a = mn_a == -CUDART_INF_F ? 0.f : mn_a, mu_b = mn_b == -CUDART_INF_F ? 0.f : mn_b;
-    const float corr_a = ex2(m_a - mu_a), corr_b = ex2(m_b - mu_b);
-    m_a = mn_a;
-    m_b = mn_b;
-    float rs_a = 0.f, rs_b = 0.f;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      if ((i >> 1) & 1) {
-        s[i] = ex2(s[i] - mu_b);
-        rs_b += s[i];
-        o[i] *= corr_b;
-      } else {
-        s[i] = ex2(s[i] - mu_a);
-        rs_a += s[i];
-        o[i] *= corr_a;
-      }
-    }
-    l_a = l_a * corr_a + rs_a;  // per-thread partial row sums (quad-reduced at the end)
-    l_b = l_b * corr_b + rs_b;
-    // ---- O += P V: P from registers (k-step ks = keys 16 ks .. +16 = accumulator registers 8 ks .. 8 ks + 7) ----
-    uint32_t pa[4][4];
+  };
+  auto softmax = [&](float (&s)[32], int j0, float &corr_a, float &corr_b) {
+    if (j0 + BKV <= kfree)
+      online_softmax<false>(s, j0, t, lim_a, lim_b, m_a, m_b, l_a, l_b, corr_a, corr_b);
+    else
+      online_softmax<true>(s, j0, t, lim_a, lim_b, m_a, m_b, l_a, l_b, corr_a, corr_b);
+  };
+  auto pack_p = [&](const float (&s)[32]) {
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks) {
       pa[ks][0] = pack_bf16(s[8 * ks + 0], s[8 * ks + 1]);
@@ -196,11 +216,32 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
       pa[ks][2] = pack_bf16(s[8 * ks + 4], s[8 * ks + 5]);
       pa[ks][3] = pack_bf16(s[8 * ks + 6], s[8 * ks + 7]);
     }
-    const uint64_t vdesc = make_smem_desc_mn(smem_u32(sv));
-    wgmma_fence();
+  };
+
+  mbar_wait(q_bar, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int it = 0; it < n_tiles; ++it) {
+    const int j0 = it * BKV;
+    // refill the stage of tile it - 2: a warpgroup running up to a tile behind the other does not stall thread 0
+    if (threadIdx.x == 0 && it >= 2 && it - 2 + kStages < n_tiles) load_tile(it - 2 + kStages);
+    __syncwarp();
+    mbar_wait(&full_bar[stage], phase);
+    uint8_t *sk = ring + stage * kStageBytes;
+    float s[32], corr_a, corr_b;
+    issue_qk(s, sk);
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+    fill_cache(j0, sk);
+    softmax(s, j0, corr_a, corr_b);
+    // o * 1.0f == o: a warp whose row maxima all stayed put skips the rescale
+    if (__any_sync(0xffffffffu, corr_a != 1.f || corr_b != 1.f)) {
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) wgmma_m64n64k16_rs_tb(o, pa[ks], vdesc + (uint64_t)(ks * (16 * 128 >> 4)));
-    wgmma_commit();
+      for (int i = 0; i < 32; ++i) o[i] *= ((i >> 1) & 1) ? corr_b : corr_a;
+    }
+    pack_p(s);
+    wgmma_fence();
+    issue_pv(stage);
     wgmma_wait<0>();
     wgmma_fence_regs(o);
     __syncwarp();
