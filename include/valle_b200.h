@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 4
+#define VB_ABI_VERSION 5
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32. */
@@ -293,6 +293,11 @@ typedef struct vb_ar_state {
   int64_t cache_layer_stride, cache_seq_stride; /* in elements */
   int32_t cache_cap;
   int32_t n_active_out_unused;
+  /* seeded device sampler (vb_ar_head.greedy == 2 only, NULL otherwise), per row so that one captured graph serves
+   * any parameters; see vb_sample_logits for what is drawn */
+  const uint64_t *sample_seed; /* [B] seed of each utterance */
+  const int32_t *top_k;        /* [B] <= 0 or >= n_vocab: no filter; 1: argmax */
+  const float *temperature;    /* [B] finite, > 0 */
 } vb_ar_state;
 
 typedef struct vb_ar_head {
@@ -303,7 +308,9 @@ typedef struct vb_ar_head {
   const float *alpha;         /* ar_audio_position.alpha (device scalar) */
   const float *pe;            /* fp32 [pe_rows, d] sine table */
   int32_t pe_rows;
-  int32_t greedy;             /* 1: argmax + stop rule + append on device; 0: logits only */
+  int32_t greedy;             /* 1: argmax + stop rule + append on device; 0: logits only (the caller draws and
+                                 calls vb_ar_push_tokens); 2: seeded draw on the device from the state's sampler
+                                 arrays (vb_sample_logits), then the stop rule + append as for 1 */
   vb_ln_fold fold;            /* final LayerNorm folded into predict_w (all-NULL: separate LayerNorm launch) */
 } vb_ar_head;
 
@@ -330,6 +337,20 @@ int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st,
  * (valle.py:1040-1057 with torch's own RNG), applying the same stop rule. */
 int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int64_t *sampled, int d,
                       vb_stream_t stream);
+
+/* Seeded top-k / temperature draw (valle.py:1040-1043,1287-1302 with top_p = 1), one row r of logits[r * ld ...]
+ * (ld may be 0: every row reads the same logits) with V <= 1280 entries:
+ *   l'_i = l_i / T (rounded fp32 division, skipped when T == 1); kth = the exact k-th largest l'; kept = { i : l'_i >=
+ *   kth } (ties with the k-th value survive; every i when k <= 0 or k >= V);
+ *   u_i = ((h >> 41) + 0.5) * 2^-23 (exact in fp32, within [2^-24, 1 - 2^-24]) with h = splitmix64 finaliser of seed + step * 0x9E3779B97F4A7C15 +
+ *   i * 0xD1342543DE82EF95 (the dropout hash), g_i = -logf(-logf(u_i));
+ *   out_ids[r] = argmax over kept i of (l'_i + g_i), smallest index on ties (Gumbel-max: a draw from softmax(l') over
+ *   the kept set, up to the 23-bit resolution of u: g_i lies in [-2.81, 16.64], so a token less likely than about
+ *   e^-19.4 relative to the most likely kept one is never drawn).  k == 1 returns argmax(l), the greedy id.
+ * The AR decode tail (vb_ar_head.greedy == 2) runs the same function with step = the utterance's n_gen. */
+int vb_sample_logits(const float *logits, int64_t ld, int64_t n_rows, int n_vocab, const uint64_t *seeds,
+                     const int32_t *steps, const int32_t *top_k, const float *temperature, int64_t *out_ids,
+                     vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * a1  NAR stage tail (valle.py:1128-1134): samples = argmax(logits) over rows, written to

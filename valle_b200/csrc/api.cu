@@ -490,6 +490,7 @@ int tc_head(vb_decoder *dec, const vb_ar_head *head, float *x, vb_ar_state *st, 
 VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
                            void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && head && h && st, "vb_ar_head_step: null argument");
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_head_step: greedy %d not in {0, 1, 2}", head->greedy);
   const vb_decoder_desc &D = dec->desc;
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model;
@@ -517,6 +518,7 @@ VB_API int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int6
 VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st, void *workspace,
                              size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && head && st, "vb_ar_decode_step: null argument");
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_decode_step: greedy %d not in {0, 1, 2}", head->greedy);
   const vb_decoder_desc &D = dec->desc;
   VB_CHECK_ARG(workspace_bytes >= vb_ar_step_workspace(&D, st->B, st->cache_cap),
                "vb_ar_decode_step: workspace too small");

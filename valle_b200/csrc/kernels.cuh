@@ -16,14 +16,19 @@ struct DropCfg {
   float inv_keep;      // 1 / (1 - p)
   int64_t lmax;        // attention only: index = ((b * H + h) * lmax + q) * lmax + k
 };
-__host__ __device__ __forceinline__ bool drop_keep(const DropCfg &c, uint64_t idx) {
-  uint64_t z = c.seed + (uint64_t)c.stream * 0x9E3779B97F4A7C15ull + idx * 0xD1342543DE82EF95ull;
+// Counter-based hash of (seed, stream, index): splitmix64 finaliser over seed + stream * C1 + index * C2.  Shared by
+// the dropout masks and the device sampler (sample.cu); tests restate it in numpy.
+__host__ __device__ __forceinline__ uint64_t mix64(uint64_t seed, uint64_t stream, uint64_t idx) {
+  uint64_t z = seed + stream * 0x9E3779B97F4A7C15ull + idx * 0xD1342543DE82EF95ull;
   z ^= z >> 30;
   z *= 0xBF58476D1CE4E5B9ull;
   z ^= z >> 27;
   z *= 0x94D049BB133111EBull;
   z ^= z >> 31;
-  return (uint32_t)(z >> 32) >= c.thresh;
+  return z;
+}
+__host__ __device__ __forceinline__ bool drop_keep(const DropCfg &c, uint64_t idx) {
+  return (uint32_t)(mix64(c.seed, (uint64_t)c.stream, idx) >> 32) >= c.thresh;
 }
 inline DropCfg make_drop(float p, uint64_t seed, uint32_t stream, int64_t lmax = 0) {
   DropCfg c{};
@@ -217,6 +222,8 @@ int launch_dropout_add(float *x, const float *t, int64_t n, const DropCfg &cfg, 
 int launch_cast_from_f32(const float *in, void *out, int dtype, int64_t n, cudaStream_t s);
 
 // sample.cu
+// head->greedy == 2 (and neither `forced` nor `reduce_only`) launches the seeded device sampler, which reads
+// st->sample_seed / top_k / temperature; every other call the argmax / push / reduce kernel
 int launch_ar_sample(float *logits, int64_t ld_logits, const float *partials, int splits, int ldp,
                      const vb_ar_head *head, vb_ar_state *st, int d, const int64_t *forced, int reduce_only, bool pdl,
                      cudaStream_t s, const LnFoldStats *fold = nullptr);

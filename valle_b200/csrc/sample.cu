@@ -3,6 +3,8 @@
 //     (argmax==EOS or sample==EOS or n_new > 16*S), the append of :1057 and the embedding + sine PE
 //     of the appended token (:1013-1015) so the next decode step needs no host round trip
 //     (the reference syncs to the host once per token).
+//     ar_sample_kernel<true> draws the token with the seeded sampler (sample_row) instead of taking the argmax.
+//   * sample_logits_kernel: the same sampler on caller-given logits (vb_sample_logits).
 //   * nar_argmax_accumulate_kernel: samples = argmax(logits) (:1130) and
 //     y_emb[:, Tp:] += nar_audio_embeddings[i+1](samples) (:1133-1134).
 #include <math_constants.h>
@@ -31,6 +33,103 @@ __device__ __forceinline__ ArgMax warp_argmax(ArgMax a) {
   return a;
 }
 
+// ---- seeded top-k / temperature sampler (include/valle_b200.h vb_sample_logits), one CTA of 256 threads per row, the
+// row held in registers as 5 values per thread (element i = threadIdx.x + 256 j, V <= 1280)
+struct SamplerArgs {
+  const uint64_t *seed;
+  const int32_t *top_k;
+  const float *temperature;
+};
+struct SamplerSmem {
+  unsigned hist[256];
+  unsigned wsum[8];
+  ArgMax wbest[8];
+  int sel_bin, sel_k;
+};
+// order-preserving float <-> uint32 (larger float, larger key)
+__device__ __forceinline__ uint32_t float_key(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_float(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+// the row's maximum (smallest index on ties), returned to every thread
+__device__ __forceinline__ ArgMax block_argmax(ArgMax a, ArgMax *wbest) {
+  a = warp_argmax(a);
+  if ((threadIdx.x & 31) == 0) wbest[threadIdx.x >> 5] = a;
+  __syncthreads();
+  a = wbest[0];
+#pragma unroll
+  for (int w = 1; w < 8; ++w) a = better(a, wbest[w]);
+  return a;
+}
+// exact k-th largest of the n valid values (0 < k < n): radix select over the order-preserving keys, 4 passes of 8
+// bits, each a 256-bin histogram of the keys that match the digits chosen so far plus a suffix scan over the bins
+__device__ float radix_kth(const float (&x)[5], int n, int k, SamplerSmem &sm) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  uint32_t key[5];
+#pragma unroll
+  for (int j = 0; j < 5; ++j) key[j] = float_key(x[j]);
+  uint32_t prefix = 0, mask = 0;
+#pragma unroll 1
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    sm.hist[tid] = 0;
+    __syncthreads();
+#pragma unroll
+    for (int j = 0; j < 5; ++j)
+      if (tid + j * 256 < n && (key[j] & mask) == prefix) atomicAdd(&sm.hist[(key[j] >> shift) & 255u], 1u);
+    __syncthreads();
+    // thread t owns bin 255 - t: the inclusive prefix sum over t is the count of keys whose digit is >= that bin
+    const int bin = 255 - tid;
+    const unsigned c = sm.hist[bin];
+    unsigned s = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const unsigned t = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += t;
+    }
+    if (lane == 31) sm.wsum[warp] = s;
+    __syncthreads();
+    for (int w = 0; w < warp; ++w) s += sm.wsum[w];
+    if (s >= (unsigned)k && s - c < (unsigned)k) {  // exactly one bin holds the k-th key
+      sm.sel_bin = bin;
+      sm.sel_k = k - (int)(s - c);
+    }
+    __syncthreads();
+    prefix |= (uint32_t)sm.sel_bin << shift;
+    mask |= 255u << shift;
+    k = sm.sel_k;
+  }
+  return key_float(prefix);
+}
+// Gumbel-max draw over the top-k set of l / T; `amax` = argmax(l), returned for k == 1.  Called by all 256 threads,
+// returns the id to every thread.
+__device__ int sample_row(const float (&l)[5], int n, int amax, uint64_t seed, int step, int k, float temp,
+                          SamplerSmem &sm) {
+  if (k == 1) return amax;
+  const int tid = threadIdx.x;
+  float x[5];
+#pragma unroll
+  for (int j = 0; j < 5; ++j) x[j] = temp != 1.f ? __fdiv_rn(l[j], temp) : l[j];
+  const float kth = (k > 0 && k < n) ? radix_kth(x, n, k, sm) : -CUDART_INF_F;
+  ArgMax best{-CUDART_INF_F, 0x7fffffff};
+#pragma unroll
+  for (int j = 0; j < 5; ++j) {
+    const int i = tid + j * 256;
+    if (i < n && x[j] >= kth) {
+      const uint64_t h = mix64(seed, (uint64_t)(int64_t)step, (uint64_t)i);
+      // 23 bits: m + 0.5 fits fp32's 24-bit significand, so u is exact, in [2^-24, 1 - 2^-24] and g finite
+      // (a 24-bit m + 0.5 would round 2^24 - 0.5 up to 2^24: u = 1, g = +inf)
+      const float u = ((float)(uint32_t)(h >> 41) + 0.5f) * 1.1920928955078125e-7f;
+      const float g = -logf(-logf(u));
+      best = better(best, ArgMax{__fadd_rn(x[j], g), i});
+    }
+  }
+  return block_argmax(best, sm.wbest).i;
+}
+
+template <bool kSample>
 __global__ void __launch_bounds__(256)
 ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__restrict__ partials, int splits,
                  int ldp, int n_vocab, int eos_id,
@@ -39,7 +138,8 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
                  const int32_t *__restrict__ prompt_len, const int32_t *__restrict__ max_new,
                  int32_t *__restrict__ n_gen, int32_t *__restrict__ finished,
                  int32_t *__restrict__ tokens, int tok_stride, float *__restrict__ x_cur, int d,
-                 const int64_t *__restrict__ forced, int reduce_only, LnFoldStats fold, const float *__restrict__ fold_d) {
+                 const int64_t *__restrict__ forced, int reduce_only, LnFoldStats fold, const float *__restrict__ fold_d,
+                 SamplerArgs sa) {
   __shared__ ArgMax wbest[8];
   __shared__ int s_tok, s_pos;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -57,7 +157,16 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
   // scalars of the stop rule: in flight together with the logits instead of after the argmax
   const int n_new = n_gen[b], p_len = prompt_len[b], cap_new = max_new[b];
   const int forced_tok = forced ? (int)forced[b] : -1;
+  uint64_t seed = 0;
+  int top_k = 0;
+  float temp = 1.f;
+  if constexpr (kSample) {
+    seed = sa.seed[b];
+    top_k = sa.top_k[b];
+    temp = sa.temperature[b];
+  }
   float *row = logits + (int64_t)b * ld_logits;
+  float lv[5];  // kSample: the row in registers, element tid + 256 j
   ArgMax best{-CUDART_INF_F, 0x7fffffff};
   // final LayerNorm folded into ar_predict_layer (gemm_decode_x_kernel): logit = rstd (acc - mean c[i]) + (beta W^T)[i]
   float f_mean = 0.f, f_rstd = 1.f;
@@ -85,6 +194,7 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
         row[i] = a;
         best = better(best, ArgMax{a, i});
       }
+      if constexpr (kSample) lv[j] = i < n_vocab ? a : -CUDART_INF_F;
     }
   } else {
     for (int i = tid; i < n_vocab; i += 256) {
@@ -101,16 +211,29 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
       }
       best = better(best, ArgMax{v, i});
     }
+    if constexpr (kSample) {  // read back this thread's elements of the row (its own writes)
+#pragma unroll
+      for (int j = 0; j < 5; ++j) lv[j] = tid + j * 256 < n_vocab ? row[tid + j * 256] : -CUDART_INF_F;
+    }
   }
-  if (reduce_only) return;
-  best = warp_argmax(best);
-  if (lane == 0) wbest[warp] = best;
-  __syncthreads();
+  if constexpr (!kSample) {
+    if (reduce_only) return;
+  }
+  int draw = -1;
+  if constexpr (kSample) {
+    __shared__ SamplerSmem smp;
+    best = block_argmax(best, wbest);
+    draw = sample_row(lv, n_vocab, best.i, seed, n_new, top_k, temp, smp);
+  } else {
+    best = warp_argmax(best);
+    if (lane == 0) wbest[warp] = best;
+    __syncthreads();
+  }
   if (tid == 0) {
     ArgMax a = wbest[0];
 #pragma unroll
     for (int w = 1; w < 8; ++w) a = better(a, wbest[w]);
-    const int samp = forced ? forced_tok : a.i;
+    const int samp = kSample ? draw : (forced ? forced_tok : a.i);
     const bool stop = (a.i == eos_id) || (samp == eos_id) || (n_new > cap_new) || (n_new >= tok_stride);
     if (stop) {
       finished[b] = (n_new == 0) ? 2 : 1;
@@ -151,13 +274,42 @@ int launch_ar_sample(float *logits, int64_t ld_logits, const float *partials, in
   LnFoldStats f{};
   if (fold) f = *fold;
   const float *fold_d = fold ? head->fold.dvec : nullptr;
-  VB_CUDA(launch_kernel(ar_sample_kernel, dim3(st->B), dim3(256), 0, s, pdl, logits, ld_logits, partials, splits, ldp,
-                        head->n_vocab, head->eos_id, head->audio_emb, head->alpha, head->pe, head->pe_rows,
-                        (const int32_t *)st->text_len, (const int32_t *)st->prompt_len, (const int32_t *)st->max_new,
-                        st->n_gen, st->finished, st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, f,
-                        fold_d));
+  const bool sample = head->greedy == 2 && forced == nullptr && !reduce_only;
+  SamplerArgs sa{};
+  if (sample) {
+    VB_CHECK_ARG(st->sample_seed && st->top_k && st->temperature, "vb_ar_head.greedy == 2: sampler arrays not set");
+    VB_CHECK_ARG(head->n_vocab <= 5 * 256, "device sampler: n_vocab %d > 1280", head->n_vocab);
+    sa = SamplerArgs{st->sample_seed, st->top_k, st->temperature};
+  }
+  VB_CUDA(launch_kernel(sample ? ar_sample_kernel<true> : ar_sample_kernel<false>, dim3(st->B), dim3(256), 0, s, pdl,
+                        logits, ld_logits, partials, splits, ldp, head->n_vocab, head->eos_id, head->audio_emb,
+                        head->alpha, head->pe, head->pe_rows, (const int32_t *)st->text_len,
+                        (const int32_t *)st->prompt_len, (const int32_t *)st->max_new, st->n_gen, st->finished,
+                        st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, f, fold_d, sa));
   count_launch();
   return VB_OK;
+}
+
+__global__ void __launch_bounds__(256)
+sample_logits_kernel(const float *__restrict__ logits, int64_t ld, int n_vocab, const uint64_t *__restrict__ seeds,
+                     const int32_t *__restrict__ steps, const int32_t *__restrict__ top_k,
+                     const float *__restrict__ temperature, int64_t *__restrict__ out_ids) {
+  __shared__ SamplerSmem sm;
+  const int64_t r = blockIdx.x;
+  const int tid = threadIdx.x;
+  const float *row = logits + r * ld;
+  float l[5];
+  ArgMax best{-CUDART_INF_F, 0x7fffffff};
+#pragma unroll
+  for (int j = 0; j < 5; ++j) {
+    const int i = tid + j * 256;
+    l[j] = i < n_vocab ? row[i] : -CUDART_INF_F;
+    if (i < n_vocab) best = better(best, ArgMax{l[j], i});
+  }
+  best = block_argmax(best, sm.wbest);
+  __syncthreads();  // sm.wbest is reused by the draw
+  const int id = sample_row(l, n_vocab, best.i, seeds[r], steps[r], top_k[r], temperature[r], sm);
+  if (tid == 0) out_ids[r] = id;
 }
 
 __global__ void nar_argmax_accumulate_kernel(const float *__restrict__ logits, int64_t n_rows, int n_vocab,
@@ -201,6 +353,19 @@ VB_API int vb_nar_argmax_accumulate(const float *logits, int64_t n_rows, int n_v
   const int wpb = 4;
   nar_argmax_accumulate_kernel<<<(unsigned)((n_rows + wpb - 1) / wpb), wpb * 32, 0, (cudaStream_t)stream>>>(
       logits, n_rows, n_vocab, ld_logits, codes, code_row_stride, next_emb, y_emb, y_row_stride, y_rows, d);
+  VB_LAUNCH_CHECK();
+  return VB_OK;
+}
+
+VB_API int vb_sample_logits(const float *logits, int64_t ld, int64_t n_rows, int n_vocab, const uint64_t *seeds,
+                            const int32_t *steps, const int32_t *top_k, const float *temperature, int64_t *out_ids,
+                            vb_stream_t stream) {
+  VB_CHECK_ARG(n_vocab >= 1 && n_vocab <= 5 * 256, "vb_sample_logits: n_vocab %d not in [1, 1280]", n_vocab);
+  VB_CHECK_ARG(n_rows >= 0 && n_rows < (1ll << 31), "vb_sample_logits: n_rows out of range");
+  if (n_rows == 0) return VB_OK;
+  VB_CHECK_ARG(logits && seeds && steps && top_k && temperature && out_ids, "vb_sample_logits: null argument");
+  sample_logits_kernel<<<(unsigned)n_rows, 256, 0, (cudaStream_t)stream>>>(logits, ld, n_vocab, seeds, steps, top_k,
+                                                                          temperature, out_ids);
   VB_LAUNCH_CHECK();
   return VB_OK;
 }

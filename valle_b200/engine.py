@@ -18,6 +18,7 @@ libvalle_b200.so.  There is no CPU fallback.
 """
 from __future__ import annotations
 
+import math
 import os
 
 import ctypes as C
@@ -85,6 +86,10 @@ class _ArBuffers:
         self.logits = torch.zeros((B, self.ldl), dtype=torch.float32, device=dev)
         self.kcache = torch.zeros((nd.n_layer, B, nd.H, cap, 64), dtype=eng.dtype, device=dev)
         self.vcache = torch.zeros_like(self.kcache)
+        # seeded device sampler, per row (uint64 seeds stored as their int64 bit patterns)
+        self.sample_seed = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.top_k = torch.zeros(B, **i32)
+        self.temperature = torch.ones(B, dtype=torch.float32, device=dev)
         st = L.ArState()
         st.B, st.tok_stride = B, tok_stride
         st.text_len, st.prompt_len, st.max_new = self.text_len.data_ptr(), self.prompt_len.data_ptr(), self.max_new.data_ptr()
@@ -92,11 +97,42 @@ class _ArBuffers:
         st.x_cur, st.logits = self.x_cur.data_ptr(), self.logits.data_ptr()
         st.kcache, st.vcache = self.kcache.data_ptr(), self.vcache.data_ptr()
         st.cache_layer_stride, st.cache_seq_stride, st.cache_cap = self.kcache.stride(0), self.kcache.stride(1), cap
+        st.sample_seed, st.top_k = self.sample_seed.data_ptr(), self.top_k.data_ptr()
+        st.temperature = self.temperature.data_ptr()
         self.st = st
         nbytes = eng.lib.vb_ar_step_workspace(C.byref(nd.desc), B, cap)
         self.ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.eng = eng
+
+
+def _is_seq(v) -> bool:
+    return isinstance(v, (list, tuple)) or (isinstance(v, (torch.Tensor, np.ndarray)) and v.ndim > 0)
+
+
+def _sampler_args(B: int, seed, top_k, temperature):
+    """Validated per-utterance (seeds, top_k, temperature) lists of a seeded call: an int seed s stands for s, s+1, ...,
+    s+B-1 (so utterance b decoded alone with seed s+b draws what it draws in the batch); top_k / temperature are one
+    value or a sequence of B."""
+    def per_row(v, what):
+        if _is_seq(v):
+            v = [x.item() if hasattr(x, "item") else x for x in v]
+            if len(v) != B:
+                raise ValueError(f"{what}: {len(v)} values for {B} utterances")
+            return v
+        return [v] * B
+    if _is_seq(seed):
+        seeds = per_row(seed, "seed")
+    else:
+        seeds = [int(seed) + b for b in range(B)]
+    seeds = [int(x) for x in seeds]
+    if any(x < 0 or x >= 1 << 64 for x in seeds):
+        raise ValueError("seed: every utterance's seed must lie in [0, 2**64)")
+    ks = [int(x) for x in per_row(top_k, "top_k")]
+    ts = [float(x) for x in per_row(temperature, "temperature")]
+    if any(not math.isfinite(t) or t <= 0.0 for t in ts):
+        raise ValueError("temperature must be finite and > 0")
+    return seeds, ks, ts
 
 
 def _seg_ranges(starts, lens):
@@ -144,7 +180,8 @@ class ValleEngine:
         self.max_tc_batch = 64
         #: bf16 decode steps run the LayerNorm-folded chain (6 launches per layer instead of 8)
         self.use_decode_fold = os.environ.get("VB_DECODE_FOLD", "1") != "0"
-        #: greedy decode steps captured per CUDA graph (one replay per group; the stop flags are polled every `poll` steps)
+        #: decode steps that draw on the device (greedy or seeded) captured per CUDA graph (one replay per group; the stop
+        #: flags are polled every `poll` steps)
         self.steps_per_graph = 8
         self.replayed_launches = 0   # kernels executed through CUDA-graph replays
         self.captured_launches = 0   # kernels recorded at capture time (counted by the library, not run)
@@ -243,7 +280,7 @@ class ValleEngine:
             self._ada_cache = [self.nar.ada_table(e.weight) for e in self.model.nar_stage_embeddings]
         return self._ada_cache
 
-    def _head(self, pe: torch.Tensor, greedy: bool) -> L.ArHead:
+    def _head(self, pe: torch.Tensor, greedy: int) -> L.ArHead:
         m = self.model
         h = L.ArHead()
         h.predict_w = self.ar_predict_w.data_ptr()
@@ -273,9 +310,15 @@ class ValleEngine:
                  enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1, temperature: float = 1.0,
                  max_new_tokens: Optional[int] = None, poll: int = 32,
                  return_device: bool = False, trace: Optional[dict] = None,
-                 forced: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+                 forced: Optional[Sequence[torch.Tensor]] = None, seed=None) -> List[torch.Tensor]:
         """texts[b]: int64 [S_b] phoneme ids; prompts[b]: int64 [Tp_b, Q] codec ids (host or device).
         Returns codes[b]: int64 [Tgen_b, Q] -- per utterance exactly what VALLE.inference returns.
+
+        seed: None draws top_k != 1 ids with torch's generator (torch.multinomial on the device, or on the host with
+        `sample_on_host`).  An int s, or a sequence of B ints in [0, 2**64), selects the seeded device sampler
+        (vb_sample_logits): utterance b draws from seed s + b (or seed[b]) and its decode step, inside the CUDA-graph
+        decode step, so its codes do not depend on the batch it shares, its slot, or how the call is split.  With a
+        seed, top_k and temperature may be per-utterance sequences; every top_k == 1 is the greedy path.
 
         Test hooks: `trace` collects AR logits (trace["steps"] = set of iterations or "all") and, with
         trace["nar"] = True, the NAR logits / argmax of every stage; `forced[b]` = int64 [T_b, Q] codes the decode is
@@ -285,6 +328,15 @@ class ValleEngine:
         m, dev, d, Q = self.model, self.device, self.d, self.Q
         B = len(texts)
         assert B == len(prompts) and B >= 1
+        sampler = None
+        if seed is not None:
+            if self.sample_on_host:
+                raise ValueError("seed= selects the device sampler; it cannot be combined with sample_on_host = True")
+            sampler = _sampler_args(B, seed, top_k, temperature)
+            if all(k == 1 for k in sampler[1]):
+                sampler, top_k = None, 1          # greedy: the seed draws nothing
+        elif _is_seq(top_k) or _is_seq(temperature):
+            raise ValueError("per-utterance top_k / temperature need seed= (the seeded device sampler)")
         if B > self.max_tc_batch and self.dtype == torch.bfloat16 and trace is None and forced is None:
             # the tensor-core decode projections take up to 64 rows (one UMMA N tile): a larger batch is decoded as
             # consecutive groups of <= 64 utterances instead of falling onto the CUDA-core GEMV path
@@ -293,8 +345,12 @@ class ValleEngine:
             packed = []
             for b0 in range(0, B, self.max_tc_batch):
                 b1 = min(B, b0 + self.max_tc_batch)
+                if sampler is None:
+                    kw = dict(top_k=top_k, temperature=temperature)
+                else:   # by absolute utterance index
+                    kw = dict(seed=sampler[0][b0:b1], top_k=sampler[1][b0:b1], temperature=sampler[2][b0:b1])
                 outs += self.generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
-                                      top_k, temperature, max_new_tokens, poll, return_device, None, None)
+                                      max_new_tokens=max_new_tokens, poll=poll, return_device=return_device, **kw)
                 stats.ar_steps += self.stats.ar_steps
                 stats.ar_ms += self.stats.ar_ms
                 stats.prefill_ms += self.stats.prefill_ms
@@ -317,7 +373,9 @@ class ValleEngine:
             cap_new = [min(c, max_new_tokens - 1) for c in cap_new]
         tok_stride = (max(cap_new) + 2 + 7) // 8 * 8
         cap = (max(S[b] + Tp[b] + cap_new[b] + 2 for b in range(B)) + 63) // 64 * 64
-        greedy = top_k == 1 and forced is None
+        greedy = sampler is None and top_k == 1 and forced is None
+        # seeded draw in the decode step's tail (forced ids replace every draw: that runs the push path below)
+        native = sampler is not None and forced is None
         forced_steps = None
         if forced is not None:  # [steps, B] first-codebook ids, EOS once an utterance's forced ids run out
             n_f = max(int(f.shape[0]) for f in forced) + 1
@@ -365,6 +423,11 @@ class ValleEngine:
         buf.max_new.copy_(capn_d)
         buf.n_gen.zero_()
         buf.finished.zero_()
+        if native:
+            seeds, ks, ts = sampler
+            buf.sample_seed.copy_(torch.tensor([x - (1 << 64) if x >= 1 << 63 else x for x in seeds], dtype=torch.int64))
+            buf.top_k.copy_(torch.tensor(ks, dtype=torch.int32))
+            buf.temperature.copy_(torch.tensor(ts, dtype=torch.float32))
         pe_t = self._pe(m.ar_text_position, max(S))
         pe_a = self._pe(m.ar_audio_position, max(Tp) + max(cap_new) + 2)
         x = torch.empty((M, d), dtype=torch.float32, device=dev)
@@ -376,7 +439,7 @@ class ValleEngine:
             self._embed_pe(prm_all, Q, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, arow_d, apos_d)
         self.ar.forward(x, cu_d, B, max(seq_len), L.VB_MASK_VALLE_AR, S_d, None, buf.kcache, buf.vcache, cap)
         h_last = ops.gather_rows(x, last_d)
-        head = self._head(pe_a, greedy)
+        head = self._head(pe_a, 2 if native else int(greedy))
         self._head_ref = head
         L.check(self.lib.vb_ar_head_step(self.ar.handle, C.byref(head), h_last.data_ptr(), C.byref(buf.st),
                                          buf.ws.data_ptr(), buf.ws.numel(), L.stream_ptr()), "vb_ar_head_step")
@@ -390,7 +453,7 @@ class ValleEngine:
             poll = 1
         if forced_steps is not None:
             poll = 1
-        if not greedy:
+        if not (greedy or native):
             self._sample_push(buf, head, top_k, temperature, None if forced_steps is None else forced_steps[0])
         if any(t.is_cuda for t in list(texts) + list(prompts)):
             ops.check_oob(dev)  # ids that were already on the device are range-checked by the embedding kernels
@@ -401,7 +464,7 @@ class ValleEngine:
         steps = 0
         while steps < max_steps:
             n = min(poll, max_steps - steps)
-            if greedy and self.use_cuda_graph:
+            if (greedy or native) and self.use_cuda_graph:
                 # whole groups of `steps_per_graph` decode steps as one graph replay (no launch gap between the
                 # steps of a group), the remainder one step at a time
                 done = 0
@@ -414,7 +477,7 @@ class ValleEngine:
                     fs = None
                     if forced_steps is not None:
                         fs = forced_steps[min(steps + 1, forced_steps.shape[0] - 1)]
-                    self._decode_step(buf, head, greedy, top_k, temperature, fs)
+                    self._decode_step(buf, head, greedy or native, top_k, temperature, fs)
             steps += n
             if trace is not None and want(steps):  # poll == 1 here: the logits row of iteration `steps`
                 trace["ar_logits"][steps] = buf.logits[:, : self.n_vocab].clone()
@@ -503,8 +566,9 @@ class ValleEngine:
 
     def _decode_step(self, buf: _ArBuffers, head: L.ArHead, greedy: bool, top_k: int, temperature: float,
                      forced_step: Optional[torch.Tensor] = None):
+        """greedy: the step draws on the device (argmax, or the seeded sampler when head.greedy == 2)"""
         if greedy and self.use_cuda_graph:
-            key = (head.pe, head.predict_w, head.audio_emb)
+            key = (head.pe, head.predict_w, head.audio_emb, head.greedy)
             if buf.graph is not None and buf.graph_key != key:
                 buf.graph = None
             if buf.graph is None:
@@ -528,8 +592,9 @@ class ValleEngine:
             self._sample_push(buf, head, top_k, temperature, forced_step)
 
     def _replay_steps(self, buf: _ArBuffers, head: L.ArHead, k: int):
-        """k greedy decode steps as ONE CUDA graph (captured on first use per (buffer, head tables, k))"""
-        key = (head.pe, head.predict_w, head.audio_emb, k)
+        """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
+        draw mode, k))"""
+        key = (head.pe, head.predict_w, head.audio_emb, head.greedy, k)
         graphs = buf.__dict__.setdefault("graphs", {})
         ent = graphs.get(key)
         if ent is None:

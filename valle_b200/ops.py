@@ -210,3 +210,28 @@ def cross_entropy_rows(logits: torch.Tensor, targets: torch.Tensor, ignore_index
     L.check(L.load().vb_cross_entropy(logits.data_ptr(), logits.stride(0), targets.data_ptr(), n, V, ignore_index,
                                       out.data_ptr(), _stream()), "vb_cross_entropy")
     return out
+
+
+@_dev_guard
+def sample_logits(logits: torch.Tensor, top_k, temperature, seeds, steps) -> torch.Tensor:
+    """Seeded top-k / temperature draw per row of fp32 logits [R, V] (V <= 1280; a row stride of 0, e.g. from
+    `expand`, draws R times from one row), vb_sample_logits: top_k / temperature / seeds / steps are one value or one
+    per row; seeds are uint64 values (int64 bit patterns accepted).  Returns int64 ids [R]."""
+    _req_cuda(logits)
+    assert logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
+    R, V = logits.shape
+    dev = logits.device
+
+    def rows(v, dtype):
+        t = v.to(dev, dtype) if isinstance(v, torch.Tensor) else torch.as_tensor(v, dtype=dtype, device=dev)
+        return t.expand(R).contiguous() if t.numel() == 1 else t.reshape(R).contiguous()
+
+    if not isinstance(seeds, torch.Tensor):
+        seeds = [int(x) - (1 << 64) if int(x) >= 1 << 63 else int(x) for x in
+                 (seeds if isinstance(seeds, (list, tuple)) else [seeds])]
+    sd, st = rows(seeds, torch.int64), rows(steps, torch.int32)
+    k, t = rows(top_k, torch.int32), rows(temperature, torch.float32)
+    out = torch.empty(R, dtype=torch.int64, device=dev)
+    L.check(L.load().vb_sample_logits(logits.data_ptr(), logits.stride(0), R, V, sd.data_ptr(), st.data_ptr(),
+                                      k.data_ptr(), t.data_ptr(), out.data_ptr(), _stream()), "vb_sample_logits")
+    return out
