@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 5
+#define VB_ABI_VERSION 6
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32. */
@@ -124,8 +124,8 @@ int vb_attention(const void *qkv, int dtype, int64_t M, int B, int n_head, int h
                  vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Decoder stack handle (transformer.py:337-406 TransformerEncoder of pre-LN
- * TransformerEncoderLayer, transformer.py:178-334).  Stores the caller's pointers only.
+ * Decoder stack handle (transformer.py:337-406 TransformerEncoder of TransformerEncoderLayer,
+ * transformer.py:178-334, pre-LN or post-LN).  Stores the caller's pointers only.
  * ---------------------------------------------------------------------------------------- */
 typedef struct vb_layer_params {
   const void *in_proj_w;   /* [3d, d]  wdtype  self_attn.in_proj_weight */
@@ -144,7 +144,9 @@ typedef struct vb_decoder_desc {
   int32_t d_model, n_head, n_layer, d_ff;
   int32_t wdtype;                /* vb_dtype of the matrices and of activations/KV cache */
   const vb_layer_params *layers; /* host array [n_layer] */
-  const float *final_norm_w, *final_norm_b; /* [d] */
+  const float *final_norm_w, *final_norm_b; /* [d], or both NULL: the stack has no final norm */
+  int32_t norm_first;            /* 1: pre-LN layers, x += SA(norm1(x)); x += FF(norm2(x)) (transformer.py:296-302)
+                                    0: post-LN layers, x = norm1(x + SA(x)); x = norm2(x + FF(x)) (:303-308) */
 } vb_decoder_desc;
 
 typedef struct vb_decoder *vb_decoder_t;
@@ -157,9 +159,10 @@ size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t M);
 
 /* a5/a6  TransformerEncoder.forward WITHOUT the final norm over packed ragged sequences
  *   (prefill of the AR decoder, a NAR pass, the training forward).
- *   x: fp32 [M, d] residual stream, updated in place.
- *   ada_wb: NULL (LayerNorm) or fp32 [(2*n_layer+1), 2d] AdaLN (weight|bias) rows for the
- *   current stage: row 2l = layer l norm1, 2l+1 = layer l norm2, last = final norm.
+ *   x: fp32 [M, d] residual stream, updated in place (post-LN: the output of the last layer's norm2).
+ *   ada_wb: NULL (LayerNorm) or fp32 AdaLN (weight|bias) rows for the current stage, [(2*n_layer+1), 2d] for a
+ *   stack with a final norm, [2*n_layer, 2d] without one: row 2l = layer l norm1, 2l+1 = layer l norm2, row 2*n_layer
+ *   (if present) = final norm (read by the caller's final-norm call, not here).
  *   kcache/vcache: NULL or [n_layer, B, H, cache_cap, hd] caches filled for later decoding. */
 int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
                        const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
@@ -174,7 +177,9 @@ int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32
  *     modules; parameter gradients are fp32 and ACCUMULATED (+=) into caller-zeroed buffers.
  * ---------------------------------------------------------------------------------------- */
 /* bytes of the activation store vb_decoder_forward_train fills for M rows (per layer: layer input, LN1 out, q|k|v,
- * attention out, post-attention residual, LN2 out, FFN hidden; plus one [M, d] scratch row block) */
+ * attention out, post-attention residual, LN2 out, FFN hidden; plus one [M, d] scratch row block).  Post-LN stacks
+ * keep the two fp32 norm inputs r1 = x + drop(SA(x)), r2 = x1 + drop(FF(x1)) in the two fp32 slots and the
+ * storage-dtype copies of the layer input and of x1 = norm1(r1) in the two LN-output slots. */
 size_t vb_decoder_train_save_bytes(const vb_decoder_desc *desc, int64_t M);
 /* vb_decoder_forward (no KV cache) that keeps the activations the backward pass needs in `save`.
  * dropout_p > 0 = training mode of valle/modules/transformer.py:315-334 and of the attention inside
@@ -205,6 +210,7 @@ typedef struct vb_layer_wt { /* the four matrices TRANSPOSED, storage dtype (ope
   const void *lin2_wt;     /* [dff, d] */
 } vb_layer_wt;
 
+/* (post-LN stacks: one fp32 [M, d] more than pre-LN) */
 size_t vb_decoder_backward_workspace(const vb_decoder_desc *desc, int64_t M);
 /* Backward of vb_decoder_forward_train.  dx: fp32 [M, d], gradient w.r.t. the stack output on entry, w.r.t. the
  * stack input on return.  ada_wb / dada_wb: the AdaLN (weight|bias) rows of the forward call and their gradient
@@ -275,7 +281,8 @@ int vb_ln_fold_build(const void *W, int N, int K, const float *gamma, const floa
                      void *wf, float *c, float *dvec, vb_stream_t stream);
 
 /* hands the decoder the folded in_proj (norm1) and linear1 (norm2) of every layer (host arrays [n_layer], copied);
- * NULL, NULL switches the folded decode chain off again.  bf16 decoders only; used by vb_ar_decode_step. */
+ * NULL, NULL switches the folded decode chain off again.  bf16 pre-LN decoders only (the fold is the identity of a
+ * LayerNorm that feeds a projection; post-LN: VB_ERR_ARG); used by vb_ar_decode_step. */
 int vb_decoder_set_decode_fold(vb_decoder_t dec, const vb_ln_fold *qkv, const vb_ln_fold *ffn1);
 
 typedef struct vb_ar_state {
@@ -318,14 +325,17 @@ typedef struct vb_ar_head {
  * concurrently running streams. */
 size_t vb_ar_step_workspace(const vb_decoder_desc *desc, int B, int cache_cap);
 
-/* final LayerNorm + ar_predict_layer on rows h[B,d] (valle.py:1039), then (greedy) the stop
+/* final LayerNorm (none when the stack has none; a pre-LN decoder must have one: VB_ERR_ARG otherwise, here and in
+ * vb_ar_decode_step) + ar_predict_layer on rows h[B,d] (valle.py:1039), then (greedy) the stop
  * rule of valle.py:1044-1048 and the append of valle.py:1057 + next-row embedding
  * (valle.py:1013-1015).  Used after prefill and at the end of every decode step. */
 int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
                     void *workspace, size_t workspace_bytes, vb_stream_t stream);
 
 /* one decode step for all B rows: 12 x (LN -> QKV -> KV append -> single-query attention over
- * the cache -> out-proj -> LN -> FFN), then vb_ar_head_step.  Safe to capture in a CUDA graph
+ * the cache -> out-proj -> LN -> FFN), then vb_ar_head_step.  Post-LN stacks run
+ * 12 x (QKV -> attention -> out-proj -> residual + norm1 -> FFN -> residual + norm2), the same number of launches as
+ * the unfolded pre-LN chain (one cast of x_cur ahead of layer 0 instead of the final norm).  Safe to capture in a CUDA graph
  * (no host reads; launch geometry depends only on B and cache_cap).  bf16 decoders with
  * vb_decoder_set_decode_fold + head->fold run the LayerNorm-folded chain (6 launches per layer; the
  * residual stream is assembled by the split-K projections themselves, the splits of a tile adding up in fixed order
@@ -373,6 +383,9 @@ int vb_cross_entropy(const float *logits, int64_t ld_logits, const int64_t *targ
  * (valle/models/valle.py:97-113,182-204) into one vb_linear over [rows, 5 d] */
 int vb_gather_rows(const float *src, int64_t src_row_stride, const int32_t *rows, int64_t n_rows,
                    int d, float *dst, int64_t dst_row_stride, vb_stream_t stream);
+
+/* out[i] = in[i] rounded to `dtype` (VB_F32: a copy), n fp32 values: the head operand of a stack without a final norm */
+int vb_cast_from_f32(const float *in, void *out, int dtype, int64_t n, vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * a13  AudioTokenizer.encode / .decode (valle/data/tokenizer.py:211-254) -> PyPI `encodec`

@@ -3,7 +3,10 @@ HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / arrive / wait, UTMALDG/UTMAST
 load/store/reduce, UBLKCP = cp.async.bulk, UTMAPF = TMA descriptor prefetch, SYNCS = mbarrier operations,
 HMMA = warp-level mma.sync, LDGSTS = cp.async.
 
-    python tools/sass_summary.py [lib.so]
+    python tools/sass_summary.py [lib.so] [--match REGEX]
+
+--match lists the total instruction count of every kernel whose demangled name matches REGEX instead (e.g.
+`--match "layernorm_kernel|ln_reduce_kernel"` to compare the instantiations of two builds).
 """
 import collections
 import os
@@ -12,7 +15,13 @@ import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "valle_b200", "lib", "libvalle_b200.so")
+args = sys.argv[1:]
+match = None
+if "--match" in args:
+    i = args.index("--match")
+    match = re.compile(args[i + 1])
+    del args[i:i + 2]
+lib = args[0] if args else os.path.join(ROOT, "valle_b200", "lib", "libvalle_b200.so")
 PAT = re.compile(r"\b(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UTMAREDG|UBLKCP|UTMAPF|SYNCS|HMMA|LDGSTS)\b")
 out = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
 cur, tab = None, collections.OrderedDict()
@@ -27,6 +36,12 @@ for line in out.splitlines():
             tab[cur][op] += 1
         tab[cur]["_instr"] += 1 if re.search(r"/\*[0-9a-f]{4}\*/", line) else 0
 dem = subprocess.run(["c++filt"], input="\n".join(tab), capture_output=True, text=True).stdout.splitlines()
+if match is not None:
+    print(f"# {os.path.relpath(lib, ROOT)}: SASS instructions per kernel (cuobjdump -sass, sm_90a)")
+    for (name, cnt), d in sorted(zip(tab.items(), dem), key=lambda t: t[1]):
+        if match.search(d):
+            print(f"{cnt['_instr']:8d}  {d}")
+    sys.exit(0)
 cols = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAREDG", "UBLKCP", "UTMAPF", "SYNCS", "HMMA", "LDGSTS"]
 print(f"# {os.path.relpath(lib, ROOT)}: SASS instruction counts per kernel (cuobjdump -sass, sm_90a)")
 print(f"{'kernel':90s} " + " ".join(f"{c:>8s}" for c in cols))

@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 VB_F32, VB_BF16 = 0, 1
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -34,7 +34,7 @@ class DecoderDesc(C.Structure):
     """vb_decoder_desc"""
     _fields_ = [("d_model", C.c_int32), ("n_head", C.c_int32), ("n_layer", C.c_int32),
                 ("d_ff", C.c_int32), ("wdtype", C.c_int32), ("layers", C.POINTER(LayerParams)),
-                ("final_norm_w", vp), ("final_norm_b", vp)]
+                ("final_norm_w", vp), ("final_norm_b", vp), ("norm_first", C.c_int32)]
 
 
 class ArState(C.Structure):
@@ -139,6 +139,7 @@ PROTOTYPES = {
                                 C.c_int64, C.c_int64, vp]),
     "vb_permute3": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     "vb_gather_rows": (C.c_int, [vp, C.c_int64, vp, C.c_int64, C.c_int, vp, C.c_int64, vp]),
+    "vb_cast_from_f32": (C.c_int, [vp, vp, C.c_int, C.c_int64, vp]),
 }
 
 

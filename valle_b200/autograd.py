@@ -142,6 +142,27 @@ class LayerNormRows(torch.autograd.Function):
         return dx, dg, db, dada, None, None, None
 
 
+class GatherRows(torch.autograd.Function):
+    """the head operand of a stack without a final norm (post-LN): rows x[rows] in out_dtype; the gradient goes back to
+    those rows (zero elsewhere)"""
+
+    @staticmethod
+    def forward(ctx, x, rows, out_dtype):
+        y = ops.gather_rows(x, rows)
+        if out_dtype != torch.float32:
+            y = ops.cast_from_f32(y, out_dtype)
+        ctx.save_for_backward(rows)
+        ctx.n_src = x.shape[0]
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (rows,) = ctx.saved_tensors
+        src = torch.full((ctx.n_src,), -1, dtype=torch.int32, device=rows.device)   # -1: a zero row (vb_gather_rows)
+        src[rows.long()] = torch.arange(rows.numel(), dtype=torch.int32, device=rows.device)
+        return ops.gather_rows(dy.to(torch.float32).contiguous(), src), None, None
+
+
 class Linear(torch.autograd.Function):
     """F.linear without bias for the prediction heads (valle.py:870,929): logits fp32 = a @ w^T, operands in the
     engine dtype"""

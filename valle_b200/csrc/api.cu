@@ -113,6 +113,9 @@ VB_API int vb_decoder_create(const vb_decoder_desc *desc, vb_decoder_t *out) {
                desc->d_model / desc->n_head);
   VB_CHECK_ARG(desc->d_model % 256 == 0 && desc->d_ff % 256 == 0, "vb_decoder_create: d_model and d_ff must be multiples of 256");
   VB_CHECK_ARG(desc->wdtype == VB_F32 || desc->wdtype == VB_BF16, "vb_decoder_create: bad wdtype");
+  VB_CHECK_ARG(desc->norm_first == 0 || desc->norm_first == 1, "vb_decoder_create: norm_first=%d not in {0, 1}",
+               desc->norm_first);
+  VB_CHECK_ARG(!desc->final_norm_w == !desc->final_norm_b, "vb_decoder_create: final_norm_w / final_norm_b: both or neither");
   vb_decoder *d = new (std::nothrow) vb_decoder;
   if (!d) {
     set_error("vb_decoder_create: out of host memory");
@@ -153,6 +156,7 @@ VB_API int vb_decoder_set_decode_fold(vb_decoder_t dec, const vb_ln_fold *qkv, c
   if (!qkv && !ffn1) return VB_OK;
   VB_CHECK_ARG(qkv && ffn1, "vb_decoder_set_decode_fold: both arrays or neither");
   VB_CHECK_ARG(dec->desc.wdtype == VB_BF16, "vb_decoder_set_decode_fold: bf16 decoders only");
+  VB_CHECK_ARG(dec->desc.norm_first, "vb_decoder_set_decode_fold: pre-LN decoders only (post-LN norms do not feed a projection)");
   const int n = dec->desc.n_layer;
   for (int l = 0; l < n; ++l)
     VB_CHECK_ARG(qkv[l].wf && qkv[l].c && qkv[l].dvec && ffn1[l].wf && ffn1[l].c && ffn1[l].dvec,
@@ -201,11 +205,15 @@ VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, cons
   void *qkv = ws;  ws += align_up(Mp * 3 * d * ts, 256);
   void *att = ws;  ws += align_up(Mp * d * ts, 256);
   void *hb = ws;
+  // post-LN (transformer.py:303-308): x = norm1(x + SA(x)); x = norm2(x + FF(x)).  Each post-norm writes the normalised
+  // rows back into x and into the storage-dtype copy xn the next GEMM reads; layer 0 reads a plain cast.
+  const bool post = !D.norm_first;
+  if (post) VB_TRY(launch_cast_from_f32(x, xn, dt, M * d, s));
   for (int l = 0; l < D.n_layer; ++l) {
     const vb_layer_params &P = dec->layers[l];
     const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
     const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-    VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, xn, dt, stream));
+    if (!post) VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, xn, dt, stream));
     VB_TRY(vb_linear(xn, dt, d, P.in_proj_w, dt, P.in_proj_b, qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE,
                      nullptr, 0, stream));
     void *kc = kcache ? (char *)kcache + (size_t)l * cache_layer_stride * ts : nullptr;
@@ -214,11 +222,15 @@ VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, cons
                                    mask_mode, att, kc, vc, cache_seq_stride, cache_cap, nullptr, 0, s));
     VB_TRY(vb_linear(att, dt, d, P.out_proj_w, dt, P.out_proj_b, x, VB_F32, d, M, d, d, VB_EPI_RESIDUAL,
                      nullptr, 0, stream));
-    VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, xn, dt, stream));
+    if (post)
+      VB_TRY(launch_post_norm(x, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, xn, dt, s));
+    else
+      VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, xn, dt, stream));
     VB_TRY(vb_linear(xn, dt, d, P.lin1_w, dt, P.lin1_b, hb, dt, dff, M, dff, d, VB_EPI_RELU, nullptr, 0,
                      stream));
     VB_TRY(vb_linear(hb, dt, dff, P.lin2_w, dt, P.lin2_b, x, VB_F32, d, M, d, dff, VB_EPI_RESIDUAL, nullptr,
                      0, stream));
+    if (post) VB_TRY(launch_post_norm(x, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, xn, dt, s));
   }
   return VB_OK;
 }
@@ -275,13 +287,19 @@ VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B
   const size_t per_layer = layer_save_bytes(D, M);
   const bool drop = dropout_p > 0.f;
   float *sub = (float *)((char *)save + (size_t)D.n_layer * per_layer);   // sub-layer output ahead of its dropout
+  // post-LN: the save slots hold r1 = x + drop(SA(x)) (x_in), r2 = x1 + drop(FF(x1)) (x_mid), and the storage-dtype GEMM
+  // operands x (xn1) and x1 = norm1(r1) (xn2); the post-norm of layer l writes layer l+1's xn1
+  const bool post = !D.norm_first;
+  if (post) VB_TRY(launch_cast_from_f32(x, carve_layer_save(D, M, (char *)save).xn1, dt, (int64_t)M * d, s));
   for (int l = 0; l < D.n_layer; ++l) {
     const vb_layer_params &P = dec->layers[l];
     LayerSave sv = carve_layer_save(D, M, (char *)save + (size_t)l * per_layer);
     const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
     const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-    VB_CUDA(cudaMemcpyAsync(sv.x_in, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
-    VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, sv.xn1, dt, stream));
+    if (!post) {
+      VB_CUDA(cudaMemcpyAsync(sv.x_in, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
+      VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, sv.xn1, dt, stream));
+    }
     VB_TRY(vb_linear(sv.xn1, dt, d, P.in_proj_w, dt, P.in_proj_b, sv.qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE, nullptr, 0,
                      stream));
     // training-mode dropout (p > 0): attention probabilities (activation.py:199 `dropout=`), dropout1 / dropout2 on
@@ -298,8 +316,13 @@ VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B
       VB_TRY(vb_linear(sv.att, dt, d, P.out_proj_w, dt, P.out_proj_b, x, VB_F32, d, M, d, d, VB_EPI_RESIDUAL, nullptr, 0,
                        stream));
     }
-    VB_CUDA(cudaMemcpyAsync(sv.x_mid, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
-    VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, sv.xn2, dt, stream));
+    if (post) {
+      VB_CUDA(cudaMemcpyAsync(sv.x_in, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
+      VB_TRY(launch_post_norm(x, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, sv.xn2, dt, s));
+    } else {
+      VB_CUDA(cudaMemcpyAsync(sv.x_mid, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
+      VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, sv.xn2, dt, stream));
+    }
     VB_TRY(vb_linear(sv.xn2, dt, d, P.lin1_w, dt, P.lin1_b, sv.hb, dt, dff, M, dff, d, VB_EPI_RELU, nullptr, 0, stream));
     if (drop) {
       VB_TRY(launch_dropout(sv.hb, sv.hb, dt, (int64_t)M * dff, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 2u), s));
@@ -307,6 +330,11 @@ VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B
       VB_TRY(launch_dropout_add(x, sub, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 3u), s));
     } else {
       VB_TRY(vb_linear(sv.hb, dt, dff, P.lin2_w, dt, P.lin2_b, x, VB_F32, d, M, d, dff, VB_EPI_RESIDUAL, nullptr, 0, stream));
+    }
+    if (post) {
+      VB_CUDA(cudaMemcpyAsync(sv.x_mid, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
+      void *next_xn1 = l + 1 < D.n_layer ? carve_layer_save(D, M, (char *)save + (size_t)(l + 1) * per_layer).xn1 : nullptr;
+      VB_TRY(launch_post_norm(x, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, next_xn1, dt, s));
     }
   }
   return VB_OK;
@@ -323,6 +351,7 @@ VB_API size_t vb_decoder_backward_workspace(const vb_decoder_desc *desc, int64_t
   n += align_up(Mp * 3 * d * ts, 256);    // dqkv
   n += align_up(vb_attention_backward_workspace(M, desc->n_head), 256);
   n += align_up(vb_linear_backward_workspace(desc->wdtype, M, (int)std::max(dff, 3 * d), (int)std::max(dff, d)), 256);
+  if (!desc->norm_first) n += align_up(Mp * d * 4, 256);   // post-LN: the gradient between the two post-norms
   return n + 256;
 }
 
@@ -359,6 +388,51 @@ VB_API int vb_decoder_backward(vb_decoder_t dec, float *dx, int64_t M, int B, co
   const size_t lin_ws_bytes = vb_linear_backward_workspace(dt, M, std::max(dff, 3 * d), std::max(dff, d));
   void *lin_ws = take(lin_ws_bytes);
   const size_t per_layer = layer_save_bytes(D, M);
+  if (!D.norm_first) {
+    // post-LN, per layer from the top: y = norm2(r2), r2 = x1 + drop(FF(x1)), x1 = norm1(r1), r1 = x + drop(SA(x)).
+    // dx holds dy on entry; dr = norm2^T(dy) replaces it, the FFN input gradient is added to dr (= dx1),
+    // dx = norm1^T(dx1), the attention input gradient is added to dx (= the layer input's gradient).
+    float *dr = (float *)take(Mp * d * 4);
+    for (int l = D.n_layer - 1; l >= 0; --l) {
+      const vb_layer_params &P = dec->layers[l];
+      const vb_layer_grads &G = grads[l];
+      const vb_layer_wt &T = wt[l];
+      LayerSave sv = carve_layer_save(D, M, (char *)const_cast<void *>(save) + (size_t)l * per_layer);
+      const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
+      const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
+      float *dada1 = dada_wb ? dada_wb + (size_t)(2 * l) * 2 * d : nullptr;
+      float *dada2 = dada_wb ? dada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
+      VB_CUDA(cudaMemsetAsync(dr, 0, (size_t)M * d * 4, s));
+      VB_TRY(vb_layernorm_backward(sv.x_mid, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, dx, d, dr, d, dx_dt, dt,
+                                   G.norm2_w, G.norm2_b, dada2, stream));
+      const void *dy2 = dx_dt;
+      if (drop) {
+        VB_TRY(launch_dropout(dx_dt, dy, dt, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 3u), s));
+        dy2 = dy;
+      }
+      VB_TRY(vb_linear_backward(sv.hb, dt, dff, T.lin2_wt, dy2, d, dh, dt, dff, VB_EPI_NONE, G.lin2_w, G.lin2_b, M, d, dff,
+                                lin_ws, lin_ws_bytes, stream));
+      VB_TRY(launch_relu_bwd(dh, sv.hb, dt, (int64_t)M * dff, inv_keep, s));
+      VB_TRY(vb_linear_backward(sv.xn2, dt, d, T.lin1_wt, dh, dff, dr, VB_F32, d, VB_EPI_RESIDUAL, G.lin1_w, G.lin1_b, M,
+                                dff, d, lin_ws, lin_ws_bytes, stream));
+      VB_CUDA(cudaMemsetAsync(dx, 0, (size_t)M * d * 4, s));
+      VB_TRY(vb_layernorm_backward(sv.x_in, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, dr, d, dx, d, dx_dt, dt,
+                                   G.norm1_w, G.norm1_b, dada1, stream));
+      const void *dy1 = dx_dt;
+      if (drop) {
+        VB_TRY(launch_dropout(dx_dt, dy, dt, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 1u), s));
+        dy1 = dy;
+      }
+      VB_TRY(vb_linear_backward(sv.att, dt, d, T.out_proj_wt, dy1, d, dO, dt, d, VB_EPI_NONE, G.out_proj_w, G.out_proj_b, M,
+                                d, d, lin_ws, lin_ws_bytes, stream));
+      const DropCfg dc_attn = make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 0u);
+      VB_TRY(attention_backward(sv.qkv, sv.att, dO, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
+                                seg1_start, max_seqlen, mask_mode, dqkv, attn_ws, attn_ws_bytes, &dc_attn, s));
+      VB_TRY(vb_linear_backward(sv.xn1, dt, d, T.in_proj_wt, dqkv, 3 * d, dx, VB_F32, d, VB_EPI_RESIDUAL, G.in_proj_w,
+                                G.in_proj_b, M, 3 * d, d, lin_ws, lin_ws_bytes, stream));
+    }
+    return VB_OK;
+  }
   VB_TRY(launch_cast_from_f32(dx, dx_dt, dt, (int64_t)M * d, s));
   for (int l = D.n_layer - 1; l >= 0; --l) {
     const vb_layer_params &P = dec->layers[l];
@@ -456,9 +530,10 @@ struct Pending {  // split-K partials of a projection whose bias/residual the ne
 };
 bool use_pdl() { return getenv("VB_NO_PDL") == nullptr; }
 
-// final LayerNorm + ar_predict_layer + sampler on the tensor-core path
+// final LayerNorm + ar_predict_layer + sampler on the tensor-core path.  A stack without a final norm (post-LN) feeds
+// the head the bf16 rows of x: w.xn16 as the decode chain's last post-norm left it (xn_ready), else a cast of x.
 int tc_head(vb_decoder *dec, const vb_ar_head *head, float *x, vb_ar_state *st, const StepWs &w, const Pending &pend,
-            cudaStream_t s) {
+            cudaStream_t s, bool xn_ready = false) {
   const vb_decoder_desc &D = dec->desc;
   const int d = D.d_model, B = st->B;
   const int ldl = (head->n_vocab + 3) & ~3;
@@ -472,8 +547,11 @@ int tc_head(vb_decoder *dec, const vb_ar_head *head, float *x, vb_ar_state *st, 
     return launch_ar_sample(st->logits, ldl, (const float *)w.gemm_ws, sp, ldp, head, st, d, nullptr,
                             head->greedy ? 0 : 1, pdl, s, &fs);
   }
-  VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, D.final_norm_w, D.final_norm_b,
-                          1e-5f, w.xn16, pdl, s));
+  if (D.final_norm_w)
+    VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, D.final_norm_w, D.final_norm_b,
+                            1e-5f, w.xn16, pdl, s));
+  else if (!xn_ready)
+    VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));
   int sp = 1, ldp = 0;
   VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)head->predict_w, head->n_vocab, d, 0, nullptr, DG_F32,
                             st->logits, nullptr, ldl, nullptr, (float *)w.gemm_ws, w.gemm_ws_bytes, &sp, &ldp, nullptr, pdl,
@@ -492,6 +570,7 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
   VB_CHECK_ARG(dec && head && h && st, "vb_ar_head_step: null argument");
   VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_head_step: greedy %d not in {0, 1, 2}", head->greedy);
   const vb_decoder_desc &D = dec->desc;
+  VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_head_step: a pre-LN decoder needs its final norm");
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model;
   const int ldl = (head->n_vocab + 3) & ~3;
@@ -502,10 +581,16 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
     return tc_head(dec, head, const_cast<float *>(h), st, w, Pending{}, s);
   }
   LnParams ln{D.final_norm_w, D.final_norm_b, nullptr, 1e-5f};
-  VB_TRY(launch_gemv(h, d, st->B, head->predict_w, D.wdtype, nullptr, head->n_vocab, d, st->logits, ldl, &ln, 0,
-                     nullptr, s));
+  VB_TRY(launch_gemv(h, d, st->B, head->predict_w, D.wdtype, nullptr, head->n_vocab, d, st->logits, ldl,
+                     D.final_norm_w ? &ln : nullptr, 0, nullptr, s));
   if (head->greedy) VB_TRY(launch_ar_sample(st->logits, ldl, nullptr, 0, 0, head, st, d, nullptr, 0, false, s));
   return VB_OK;
+}
+
+VB_API int vb_cast_from_f32(const float *in, void *out, int dtype, int64_t n, vb_stream_t stream) {
+  VB_CHECK_ARG(dtype == VB_F32 || dtype == VB_BF16, "vb_cast_from_f32: bad dtype %d", dtype);
+  VB_CHECK_ARG(n >= 0 && (n == 0 || (in && out)), "vb_cast_from_f32: null argument / bad size");
+  return launch_cast_from_f32(in, out, dtype, n, (cudaStream_t)stream);
 }
 
 VB_API int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int64_t *sampled, int d,
@@ -520,6 +605,8 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   VB_CHECK_ARG(dec && head && st, "vb_ar_decode_step: null argument");
   VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_decode_step: greedy %d not in {0, 1, 2}", head->greedy);
   const vb_decoder_desc &D = dec->desc;
+  // the pre-LN chain leaves the last FFN2's partial sums to the final norm's reduce: without one they would be lost
+  VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_decode_step: a pre-LN decoder needs its final norm");
   VB_CHECK_ARG(workspace_bytes >= vb_ar_step_workspace(&D, st->B, st->cache_cap),
                "vb_ar_decode_step: workspace too small");
   cudaStream_t s = (cudaStream_t)stream;
@@ -527,6 +614,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   const size_t ts = elem_size(dt);
   StepWs w = carve_step_ws(D, B, st->cache_cap, workspace);
   float *x = st->x_cur;
+  const bool post = !D.norm_first;
   if (use_tc_decode(D, B)) {
     // bf16 tensor-core path: LayerNorm(+pending residual) -> swap-AB split-K wgmma projections whose
     // partial sums are consumed by the next kernel in the chain (7 launches per layer, PDL-chained)
@@ -600,6 +688,11 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
       }
       return tc_head(dec, head, x, st, w, Pending{}, s);
     }
+    // Unfolded chain, 8 launches per layer.  Pre-LN: ln_reduce(+ the previous FFN2's partials, norm1) -> QKV ->
+    // attention -> out-proj -> ln_reduce(norm2) -> FFN1 -> ReLU reduce -> FFN2.  Post-LN (transformer.py:303-308, one cast
+    // of x ahead of layer 0 and none of the final norm): QKV -> attention -> out-proj -> ln_reduce<post>(norm1) -> FFN1 ->
+    // ReLU reduce -> FFN2 -> ln_reduce<post>(norm2), each post-norm writing the normalised rows into x as well.
+    if (post) VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));
     for (int l = 0; l < D.n_layer; ++l) {
       const vb_layer_params &L = dec->layers[l];
       const KvPrefetch pf_qkv = kv_slice(l, 3), pf_out = kv_slice(l + 1, 0), pf_f1 = kv_slice(l + 1, 1),
@@ -608,8 +701,9 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
       void *vc = (char *)st->vcache + (size_t)l * st->cache_layer_stride * ts;
       QkvScatter sc{d, hd, w.q, kc, vc, st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen,
                     st->finished};
-      VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, L.norm1_w, L.norm1_b, 1e-5f,
-                              w.xn16, pdl, s));
+      if (!post)
+        VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, L.norm1_w, L.norm1_b, 1e-5f,
+                                w.xn16, pdl, s));
       int s1 = 1, ldp1 = 0;
       VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.in_proj_w, 3 * d, d, qkv_splits, L.in_proj_b, DG_QKV, nullptr,
                                 nullptr, d, &sc, P, w.gemm_ws_bytes, &s1, &ldp1, &pf_qkv, pdl, s));
@@ -619,8 +713,8 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
       int s2 = 1, ldp2 = 0;
       VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, out_splits, L.out_proj_b, DG_RESIDUAL, x,
                                 nullptr, d, nullptr, P, w.gemm_ws_bytes, &s2, &ldp2, &pf_out, pdl, s));
-      VB_TRY(launch_ln_reduce(x, d, B, d, s2 > 1 ? P : nullptr, s2, ldp2, L.out_proj_b, L.norm2_w, L.norm2_b, 1e-5f,
-                              w.xn16, pdl, s));
+      VB_TRY(launch_ln_reduce(x, d, B, d, s2 > 1 ? P : nullptr, s2, ldp2, L.out_proj_b, post ? L.norm1_w : L.norm2_w,
+                              post ? L.norm1_b : L.norm2_b, 1e-5f, w.xn16, pdl, s, post));
       int sf = 1, ldpf = 0;
       VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.lin1_w, dff, d, ffn1_splits, L.lin1_b, DG_RELU_BF16, nullptr,
                                 w.hb16, dff, nullptr, P, w.gemm_ws_bytes, &sf, &ldpf, &pf_f1, pdl, s));
@@ -632,9 +726,16 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
       if (s3 > 1) {
         pend.part = P; pend.bias = L.lin2_b; pend.splits = s3; pend.ldp = ldp3;
       }
+      if (post) {
+        VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, L.norm2_w, L.norm2_b, 1e-5f,
+                                w.xn16, pdl, s, true));
+        pend = Pending{};
+      }
     }
-    return tc_head(dec, head, x, st, w, pend, s);
+    return tc_head(dec, head, x, st, w, pend, s, post);
   }
+  // CUDA-core chain: pre-LN GEMVs normalise their input rows on the fly; post-LN GEMVs read x as it is, and each
+  // residual GEMV is followed by the in-place post-norm of x's B rows
   for (int l = 0; l < D.n_layer; ++l) {
     const vb_layer_params &P = dec->layers[l];
     void *kc = (char *)st->kcache + (size_t)l * st->cache_layer_stride * ts;
@@ -642,14 +743,16 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     QkvScatter sc{d, hd, w.q, kc, vc, st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen,
                     st->finished};
     LnParams ln1{P.norm1_w, P.norm1_b, nullptr, 1e-5f};
-    VB_TRY(launch_gemv(x, d, B, P.in_proj_w, dt, P.in_proj_b, 3 * d, d, nullptr, 0, &ln1, 3, &sc, s));
+    VB_TRY(launch_gemv(x, d, B, P.in_proj_w, dt, P.in_proj_b, 3 * d, d, nullptr, 0, post ? nullptr : &ln1, 3, &sc, s));
     VB_TRY(launch_attn_decode(w.q, nullptr, 0, 0, nullptr, B, D.n_head, hd, kc, vc, dt, st->cache_seq_stride,
                               st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished, w.att, nullptr,
                               w.attn_ws, false, s));
     VB_TRY(launch_gemv(w.att, d, B, P.out_proj_w, dt, P.out_proj_b, d, d, x, d, nullptr, 2, nullptr, s));
+    if (post) VB_TRY(launch_post_norm(x, B, d, P.norm1_w, P.norm1_b, nullptr, 1e-5f, nullptr, VB_F32, s));
     LnParams ln2{P.norm2_w, P.norm2_b, nullptr, 1e-5f};
-    VB_TRY(launch_gemv(x, d, B, P.lin1_w, dt, P.lin1_b, dff, d, w.hb, dff, &ln2, 1, nullptr, s));
+    VB_TRY(launch_gemv(x, d, B, P.lin1_w, dt, P.lin1_b, dff, d, w.hb, dff, post ? nullptr : &ln2, 1, nullptr, s));
     VB_TRY(launch_gemv(w.hb, dff, B, P.lin2_w, dt, P.lin2_b, d, dff, x, d, nullptr, 2, nullptr, s));
+    if (post) VB_TRY(launch_post_norm(x, B, d, P.norm2_w, P.norm2_b, nullptr, 1e-5f, nullptr, VB_F32, s));
   }
   return vb_ar_head_step(dec, head, x, st, workspace, workspace_bytes, stream);
 }

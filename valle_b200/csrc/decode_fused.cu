@@ -10,7 +10,9 @@ namespace vb {
 
 // one CTA (256 threads) per row: every thread owns 4 consecutive features per 1024-wide slab, sums the
 // S partials with independent loads in flight, then the block reduces the LayerNorm moments.
-template <int kSlabs>
+// kPost: the post-norm of a post-LN layer (transformer.py:304-308, `x = norm(x + block(x))`): the normalised row
+// replaces x[b,:] as well (with or without partials), not the pre-norm sum.
+template <int kSlabs, bool kPost>
 __global__ void __launch_bounds__(256)
 ln_reduce_kernel(float *__restrict__ x, int64_t ldx, int B, int d, const float *__restrict__ partials, int splits,
                  int ldp, const float *__restrict__ bias, const float *__restrict__ gamma,
@@ -53,7 +55,7 @@ ln_reduce_kernel(float *__restrict__ x, int64_t ldx, int B, int d, const float *
           a.x += bb[i].x; a.y += bb[i].y; a.z += bb[i].z; a.w += bb[i].w;
         }
         v[i].x += a.x; v[i].y += a.y; v[i].z += a.z; v[i].w += a.w;
-        *reinterpret_cast<float4 *>(xr + c) = v[i];
+        if constexpr (!kPost) *reinterpret_cast<float4 *>(xr + c) = v[i];
       }
       s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
     }
@@ -86,10 +88,11 @@ ln_reduce_kernel(float *__restrict__ x, int64_t ldx, int B, int d, const float *
   for (int i = 0; i < kSlabs; ++i) {
     const int c = (i * 256 + tid) * 4;
     if (c < d) {
-      __nv_bfloat162 p0 = __floats2bfloat162_rn((v[i].x - mean) * rstd * g[i].x + be[i].x,
-                                                (v[i].y - mean) * rstd * g[i].y + be[i].y);
-      __nv_bfloat162 p1 = __floats2bfloat162_rn((v[i].z - mean) * rstd * g[i].z + be[i].z,
-                                                (v[i].w - mean) * rstd * g[i].w + be[i].w);
+      const float y0 = (v[i].x - mean) * rstd * g[i].x + be[i].x, y1 = (v[i].y - mean) * rstd * g[i].y + be[i].y;
+      const float y2 = (v[i].z - mean) * rstd * g[i].z + be[i].z, y3 = (v[i].w - mean) * rstd * g[i].w + be[i].w;
+      if constexpr (kPost) *reinterpret_cast<float4 *>(xr + c) = make_float4(y0, y1, y2, y3);
+      __nv_bfloat162 p0 = __floats2bfloat162_rn(y0, y1);
+      __nv_bfloat162 p1 = __floats2bfloat162_rn(y2, y3);
       uint2 pk;
       pk.x = *reinterpret_cast<uint32_t *>(&p0);
       pk.y = *reinterpret_cast<uint32_t *>(&p1);
@@ -158,23 +161,31 @@ int launch_relu_reduce(const float *partials, int splits, int ldp, const float *
   return VB_OK;
 }
 
-int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const float *partials, int splits, int ldp,
-                     const float *bias, const float *gamma, const float *beta, float eps, bf16 *out16,
-                     bool pdl, cudaStream_t s) {
+template <bool kPost>
+static int launch_ln_reduce_t(float *x, int64_t ldx, int B, int d, const float *partials, int splits, int ldp,
+                              const float *bias, const float *gamma, const float *beta, float eps, bf16 *out16,
+                              bool pdl, cudaStream_t s) {
   VB_CHECK_ARG(d % 4 == 0 && ldx % 4 == 0 && d <= 4096, "ln_reduce: bad d=%d", d);
   const dim3 grid(B), block(256);
   const int slabs = (d + 1023) / 1024;
   if (slabs <= 1)
-    VB_CUDA(launch_kernel(ln_reduce_kernel<1>, grid, block, 0, s, pdl, x, ldx, B, d, partials, splits, ldp, bias,
+    VB_CUDA(launch_kernel(ln_reduce_kernel<1, kPost>, grid, block, 0, s, pdl, x, ldx, B, d, partials, splits, ldp, bias,
                           gamma, beta, eps, out16));
   else if (slabs <= 2)
-    VB_CUDA(launch_kernel(ln_reduce_kernel<2>, grid, block, 0, s, pdl, x, ldx, B, d, partials, splits, ldp, bias,
+    VB_CUDA(launch_kernel(ln_reduce_kernel<2, kPost>, grid, block, 0, s, pdl, x, ldx, B, d, partials, splits, ldp, bias,
                           gamma, beta, eps, out16));
   else
-    VB_CUDA(launch_kernel(ln_reduce_kernel<4>, grid, block, 0, s, pdl, x, ldx, B, d, partials, splits, ldp, bias,
+    VB_CUDA(launch_kernel(ln_reduce_kernel<4, kPost>, grid, block, 0, s, pdl, x, ldx, B, d, partials, splits, ldp, bias,
                           gamma, beta, eps, out16));
   count_launch();
   return VB_OK;
+}
+
+int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const float *partials, int splits, int ldp,
+                     const float *bias, const float *gamma, const float *beta, float eps, bf16 *out16,
+                     bool pdl, cudaStream_t s, bool post) {
+  return post ? launch_ln_reduce_t<true>(x, ldx, B, d, partials, splits, ldp, bias, gamma, beta, eps, out16, pdl, s)
+              : launch_ln_reduce_t<false>(x, ldx, B, d, partials, splits, ldp, bias, gamma, beta, eps, out16, pdl, s);
 }
 
 }  // namespace vb

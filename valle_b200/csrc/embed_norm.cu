@@ -86,17 +86,21 @@ __global__ void add_pe_kernel(const float *__restrict__ in, int64_t in_row_strid
 }
 
 // One warp per row; the row lives in registers (d <= 32*4*kMaxVec).  Two-pass moments.
-template <typename TO, int kVecs>
+// kPost: the post-norm of a post-LN layer (transformer.py:304-308, `x = norm(x + block(x))`): the normalised row also
+// replaces the fp32 residual row it was read from (xpost, in place; `x` is unused), and `out` (the next GEMM's
+// operand) may be NULL.
+template <typename TO, int kVecs, bool kPost>
 __global__ void layernorm_kernel(const float *__restrict__ x, int64_t x_row_stride,
                                  const int32_t *__restrict__ rows, int64_t n_rows, int d,
                                  const float *__restrict__ gamma, const float *__restrict__ beta,
-                                 const float *__restrict__ ada_wb, float eps, TO *__restrict__ out) {
+                                 const float *__restrict__ ada_wb, float eps, TO *__restrict__ out,
+                                 float *__restrict__ xpost) {
   const int warps_per_block = blockDim.x >> 5;
   const int64_t r = (int64_t)blockIdx.x * warps_per_block + (threadIdx.x >> 5);
   if (r >= n_rows) return;
   const int lane = threadIdx.x & 31;
   const int64_t src = rows ? (int64_t)rows[r] : r;
-  const float *xr = x + src * x_row_stride;
+  const float *xr = (kPost ? xpost : x) + src * x_row_stride;
   float4 v[kVecs];
   float s = 0.f;
 #pragma unroll
@@ -139,6 +143,10 @@ __global__ void layernorm_kernel(const float *__restrict__ x, int64_t x_row_stri
         y[1] = w.y * y[1] + bb.y;
         y[2] = w.z * y[2] + bb.z;
         y[3] = w.w * y[3] + bb.w;
+      }
+      if constexpr (kPost) {
+        *reinterpret_cast<float4 *>(xpost + src * x_row_stride + c) = make_float4(y[0], y[1], y[2], y[3]);
+        if (out == nullptr) continue;
       }
       if constexpr (sizeof(TO) == 4) {
         *reinterpret_cast<float4 *>(orow + c) = make_float4(y[0], y[1], y[2], y[3]);
@@ -221,16 +229,16 @@ VB_API int vb_add_pe(const float *in, int64_t in_row_stride, const float *pe, in
   return VB_OK;
 }
 
-template <typename TO>
+template <typename TO, bool kPost = false>
 static int launch_ln(const float *x, int64_t x_row_stride, const int32_t *rows, int64_t n_rows, int d,
                      const float *gamma, const float *beta, const float *ada_wb, float eps, TO *out,
-                     cudaStream_t s) {
+                     cudaStream_t s, float *xpost = nullptr) {
   const int wpb = 4;
   const unsigned grid = (unsigned)((n_rows + wpb - 1) / wpb);
   const int vecs = (d + 127) / 128;
-#define VB_LN_CASE(V)                                                                         \
-  layernorm_kernel<TO, V><<<grid, wpb * 32, 0, s>>>(x, x_row_stride, rows, n_rows, d, gamma, beta, \
-                                                    ada_wb, eps, out)
+#define VB_LN_CASE(V)                                                                                  \
+  layernorm_kernel<TO, V, kPost><<<grid, wpb * 32, 0, s>>>(x, x_row_stride, rows, n_rows, d, gamma, beta, \
+                                                           ada_wb, eps, out, xpost)
   if (vecs <= 2) VB_LN_CASE(2);
   else if (vecs <= 4) VB_LN_CASE(4);
   else if (vecs <= 8) VB_LN_CASE(8);
@@ -258,6 +266,17 @@ VB_API int vb_layernorm(const float *x, int64_t x_row_stride, const int32_t *row
   set_error("vb_layernorm: bad out_dtype %d", out_dtype);
   return VB_ERR_ARG;
 }
+
+namespace vb {
+int launch_post_norm(float *x, int64_t n_rows, int d, const float *gamma, const float *beta, const float *ada_wb,
+                     float eps, void *out, int out_dtype, cudaStream_t s) {
+  VB_CHECK_ARG(d % 4 == 0, "post_norm: d %% 4 != 0");
+  if (n_rows == 0) return VB_OK;
+  if (out_dtype == VB_BF16)
+    return launch_ln<bf16, true>(nullptr, d, nullptr, n_rows, d, gamma, beta, ada_wb, eps, (bf16 *)out, s, x);
+  return launch_ln<float, true>(nullptr, d, nullptr, n_rows, d, gamma, beta, ada_wb, eps, (float *)out, s, x);
+}
+}  // namespace vb
 
 VB_API int vb_adaln_project(const float *W, const float *b, const float *emb, int d, float *out,
                                 vb_stream_t stream) {

@@ -203,9 +203,15 @@ int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, in
 // decode_fused.cu
 int launch_relu_reduce(const float *partials, int splits, int ldp, const float *bias, int B, int N, bf16 *out16,
                        int64_t ldo, bool pdl, cudaStream_t s, const LnFoldStats *fold = nullptr);
+// post = true: the post-norm of a post-LN layer, x[b,:] = LayerNorm(x[b,:] + bias + partials) (normalised in place)
 int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const float *partials, int splits, int ldp,
                      const float *bias, const float *gamma, const float *beta, float eps, bf16 *out16,
-                     bool pdl, cudaStream_t s);
+                     bool pdl, cudaStream_t s, bool post = false);
+
+// embed_norm.cu: the post-norm of a post-LN layer over the rows x[n_rows, d] (fp32, dense): x = LayerNorm(x) (AdaLN with
+// ada_wb != NULL) in place, and the same rows in out_dtype into `out` (may be NULL)
+int launch_post_norm(float *x, int64_t n_rows, int d, const float *gamma, const float *beta, const float *ada_wb,
+                     float eps, void *out, int out_dtype, cudaStream_t s);
 
 // backward.cu
 int launch_transpose_pad(const void *in, int dtype, int64_t ld_in, int64_t R, int C, void *out, int64_t ld_out,

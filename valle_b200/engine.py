@@ -178,7 +178,8 @@ class ValleEngine:
         self.last_packed: Optional[torch.Tensor] = None
         #: rows of one tensor-core decode group (gemm_decode.cu: one UMMA N tile); larger bf16 batches are split
         self.max_tc_batch = 64
-        #: bf16 decode steps run the LayerNorm-folded chain (6 launches per layer instead of 8)
+        #: bf16 pre-LN decode steps run the LayerNorm-folded chain (6 launches per layer instead of 8); post-LN stacks
+        #: always run the 8-launch chain
         self.use_decode_fold = os.environ.get("VB_DECODE_FOLD", "1") != "0"
         #: decode steps that draw on the device (greedy or seeded) captured per CUDA graph (one replay per group; the stop
         #: flags are polled every `poll` steps)
@@ -720,7 +721,7 @@ class ValleEngine:
             y_in = self._audio_prenet(y_emb, "nar_audio") if self.pre else y_emb
             ops.add_pe(y_in, pe_a, m.nar_audio_position.alpha.detach(), x, NT, positions=ypos_d, out_rows=yrow_d)
             self.nar.forward(x, cu_d, B, max(Ltot), L.VB_MASK_FULL, None, ada[i])
-            hn = self.nar.final_norm(x, ada[i], rows=tgt_d, out_dtype=self.dtype)
+            hn = self.nar.head_rows(x, ada[i], tgt_d, self.dtype)
             ops.linear(hn, self.nar_predict_w[i], None, L.VB_EPI_NONE, out=logits)
             nxt = emb[i + 1] if i < Q - 2 else None
             if trace is not None:

@@ -101,10 +101,6 @@ class VALLE(nn.Module):
         super().__init__()
         prepend_bos = bool(kwargs.pop("prepend_bos", False))
         num_quantizers = int(kwargs.pop("num_quantizers", 8))
-        if not norm_first:
-            raise NotImplementedError(
-                "valle_b200.VALLE: post-LN (norm_first=False) is not built; add_prenet, prepend_bos and "
-                "nar_scale_factor are (DESIGN.md section 7)")
         self.add_prenet = bool(add_prenet)
         nar_d_model = int(d_model * nar_scale_factor)
         if nar_d_model % 256 != 0 or nar_d_model // max(1, int(nhead * nar_scale_factor)) != 64:

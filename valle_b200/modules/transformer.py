@@ -3,7 +3,9 @@ reference's constructor signatures, parameter names (checkpoint layout) and init
 (valle/modules/transformer.py:17-108,178-406).  Forward = libvalle_b200.so:
 `NativeDecoder` packs the layer pointers into a `vb_decoder_t` and runs
 `vb_decoder_forward` (LN/AdaLN -> QKV GEMM -> ragged attention -> out-proj+residual -> LN ->
-FFN1+ReLU -> FFN2+residual per layer).  Pre-LN only (the VALL-E configuration).
+FFN1+ReLU -> FFN2+residual per layer).  Pre-LN (`norm_first=True`, the VALL-E default) and post-LN
+(`norm_first=False`: QKV GEMM -> attention -> out-proj+residual -> LN -> FFN1+ReLU -> FFN2+residual -> LN,
+no final norm in VALLE) stacks.
 """
 from __future__ import annotations
 
@@ -79,8 +81,9 @@ class AdaptiveLayerNorm(nn.Module):
 
 
 class TransformerEncoderLayer(nn.Module):
-    """valle/modules/transformer.py:178-334, pre-LN only (`norm_first=True`, the VALL-E configuration):
-    x += SA(norm1(x)); x += linear2(relu(linear1(norm2(x)))) (:297-302, _sa_block :315, _ff_block :332); optional
+    """valle/modules/transformer.py:178-334.  Pre-LN (`norm_first=True`, the VALL-E default):
+    x += SA(norm1(x)); x += linear2(relu(linear1(norm2(x)))) (:297-302, _sa_block :315, _ff_block :332); post-LN
+    (`norm_first=False`): x = norm1(x + SA(x)); x = norm2(x + linear2(relu(linear1(x)))) (:303-308); optional
     AdaptiveLayerNorm wrapping (:238-258).  Same sub-module and parameter names as the reference; a standalone
     forward runs the one-layer native stack, a TransformerEncoder drives all layers through one vb_decoder_t."""
     __constants__ = ["batch_first", "norm_first"]
@@ -121,10 +124,19 @@ class TransformerEncoderLayer(nn.Module):
 
     def forward_packed(self, xp: Tensor, cu: Tensor, max_len: int, B: int, mode: int, tl, dense,
                        ada1: Optional[Tensor], ada2: Optional[Tensor]) -> Tensor:
-        """transformer.py:296-302 on packed rows xp [M, d] fp32, in place, operator by operator:
-        x += out_proj(SA(norm1(x))); x += linear2(relu(linear1(norm2(x))))."""
+        """transformer.py:296-308 on packed rows xp [M, d] fp32, operator by operator; returns the output rows.  Pre-LN,
+        in place: x += out_proj(SA(norm1(x))); x += linear2(relu(linear1(norm2(x)))).  Post-LN:
+        x = norm1(x + out_proj(SA(x))); x = norm2(x + linear2(relu(linear1(x))))."""
         n1 = self.norm1.norm if isinstance(self.norm1, AdaptiveLayerNorm) else self.norm1
         n2 = self.norm2.norm if isinstance(self.norm2, AdaptiveLayerNorm) else self.norm2
+        if not self.norm_first:
+            o = self.self_attn.attend_packed(xp, cu, max_len, B, mode, tl, dense)
+            ops.linear(o, self.self_attn.out_proj.weight.detach(), self.self_attn.out_proj.bias.detach(),
+                       epilogue=L.VB_EPI_RESIDUAL, out=xp)
+            xp = ops.layernorm(xp, n1.weight.detach(), n1.bias.detach(), n1.eps, ada1)
+            f = ops.linear(xp, self.linear1.weight.detach(), self.linear1.bias.detach(), epilogue=L.VB_EPI_RELU)
+            ops.linear(f, self.linear2.weight.detach(), self.linear2.bias.detach(), epilogue=L.VB_EPI_RESIDUAL, out=xp)
+            return ops.layernorm(xp, n2.weight.detach(), n2.bias.detach(), n2.eps, ada2)
         h = ops.layernorm(xp, n1.weight.detach(), n1.bias.detach(), n1.eps, ada1)
         o = self.self_attn.attend_packed(h, cu, max_len, B, mode, tl, dense)
         ops.linear(o, self.self_attn.out_proj.weight.detach(), self.self_attn.out_proj.bias.detach(),
@@ -135,7 +147,7 @@ class TransformerEncoderLayer(nn.Module):
         return xp
 
     def forward(self, src, src_mask=None, src_key_padding_mask: Optional[Tensor] = None):
-        """One pre-LN layer (transformer.py:296-302) -- runs a 1-layer native stack."""
+        """One layer (transformer.py:296-308) -- runs a 1-layer native stack."""
         enc = TransformerEncoder.__new__(TransformerEncoder)
         nn.Module.__init__(enc)
         enc.layers = nn.ModuleList([self])
@@ -187,8 +199,6 @@ class TransformerEncoder(nn.Module):
         is recognised and served by the structured kernels, any other pattern by the dense-mask kernel);
         `src_key_padding_mask` a bool [B, L] suffix-padding mask.  `return_layer_states=True` returns
         (layer_states, output) as transformer.py:368-381 does."""
-        if not self.layers[0].norm_first:
-            raise NotImplementedError("valle_b200: post-LN (norm_first=False) is not on the VALL-E hot path")
         if self.training and torch.is_grad_enabled():
             raise NotImplementedError("valle_b200.TransformerEncoder: the module-level forward is inference only "
                                       "(training goes through VALLE.forward); call .eval()")
@@ -221,8 +231,8 @@ class TransformerEncoder(nn.Module):
             # layer by layer through the operator surface (dense masks, per-layer states)
             states = []
             for i, lyr in enumerate(self.layers):
-                lyr.forward_packed(xp, cu, max_len, B, mode, tl, dense,
-                                   None if ada is None else ada[2 * i], None if ada is None else ada[2 * i + 1])
+                xp = lyr.forward_packed(xp, cu, max_len, B, mode, tl, dense,
+                                        None if ada is None else ada[2 * i], None if ada is None else ada[2 * i + 1])
                 if return_layer_states:
                     states.append(unpack(xp))
             if self.norm is not None:
@@ -249,6 +259,7 @@ class NativeDecoder:
         self.dff = l0.linear1.out_features
         self.n_layer = len(enc.layers)
         self.adaptive = isinstance(l0.norm1, AdaptiveLayerNorm)
+        self.norm_first = bool(l0.norm_first)
         dev = l0.linear1.weight.device
         if dev.type != "cuda":
             raise L.VbError("valle_b200: the model must live on a CUDA device (no CPU fallback)")
@@ -292,6 +303,7 @@ class NativeDecoder:
         desc.d_model, desc.n_head, desc.n_layer, desc.d_ff = self.d, self.H, self.n_layer, self.dff
         desc.wdtype = L.VB_BF16 if dtype == torch.bfloat16 else L.VB_F32
         desc.layers = arr
+        desc.norm_first = int(self.norm_first)
         fn = enc.norm
         if fn is not None:
             inner = fn.norm if isinstance(fn, AdaptiveLayerNorm) else fn
@@ -333,8 +345,9 @@ class NativeDecoder:
     def enable_decode_fold(self) -> bool:
         """bf16 AR decode chain without the residual + LayerNorm launches (valle/modules/transformer.py:296-302): norm1
         is folded into in_proj and norm2 into linear1 of every layer (plain LayerNorm only).  Returns False (chain left
-        as it is) for fp32 storage and for AdaptiveLayerNorm stacks."""
-        if self.dtype != torch.bfloat16 or self.adaptive:
+        as it is) for fp32 storage, for AdaptiveLayerNorm stacks and for post-LN stacks (their norms follow the
+        residual add instead of feeding a projection)."""
+        if self.dtype != torch.bfloat16 or self.adaptive or not self.norm_first:
             return False
         qkv = (L.LnFold * self.n_layer)()
         ffn1 = (L.LnFold * self.n_layer)()
@@ -352,11 +365,11 @@ class NativeDecoder:
     def stale(self) -> bool:
         return self._sig != self._signature()
 
-    # ---- AdaLN (weight|bias) rows for one stage embedding: [(2L+1), 2d] fp32 --------------
+    # ---- AdaLN (weight|bias) rows for one stage embedding: [(2L+1), 2d] fp32 (2L rows without a final norm) ----
     def ada_table(self, stage_emb: Tensor) -> Tensor:
         assert self.adaptive
         e = stage_emb.detach().reshape(-1).contiguous()
-        rows = 2 * self.n_layer + 1
+        rows = 2 * self.n_layer + int(self.enc.norm is not None)
         tab = torch.empty((rows, 2 * self.d), dtype=torch.float32, device=self.device)
         r = 0
         for lyr in self.enc.layers:
@@ -408,3 +421,11 @@ class NativeDecoder:
                    out_dtype: torch.dtype = torch.float32) -> Tensor:
         wb = ada[2 * self.n_layer] if ada is not None else None
         return ops.layernorm(x, self.final_w, self.final_b, self.final_eps, wb, rows, out_dtype)
+
+    def head_rows(self, x: Tensor, ada: Optional[Tensor], rows: Tensor, out_dtype: torch.dtype) -> Tensor:
+        """the prediction head's operand: the stack output rows x[rows], through the final norm if the stack has one
+        (valle.py:1128), else as they are (post-LN, valle.py:242-246: no final norm), in out_dtype"""
+        if self.enc.norm is not None:
+            return self.final_norm(x, ada, rows, out_dtype)
+        h = ops.gather_rows(x, rows)
+        return h if out_dtype == torch.float32 else ops.cast_from_f32(h, out_dtype)

@@ -187,6 +187,17 @@ def gather_rows(src: torch.Tensor, rows: torch.Tensor, out: Optional[torch.Tenso
 
 
 @_dev_guard
+def cast_from_f32(x: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+    """x (contiguous fp32) rounded to `dtype` (a copy for fp32), vb_cast_from_f32"""
+    _req_cuda(x)
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    out = torch.empty(x.shape, dtype=dtype, device=x.device)
+    L.check(L.load().vb_cast_from_f32(x.data_ptr(), out.data_ptr(), _DT[dtype], x.numel(), _stream()),
+            "vb_cast_from_f32")
+    return out
+
+
+@_dev_guard
 def nar_argmax_accumulate(logits: torch.Tensor, codes: torch.Tensor, code_row_stride: int,
                           next_emb: Optional[torch.Tensor], y_emb: Optional[torch.Tensor],
                           y_rows: Optional[torch.Tensor] = None) -> None:

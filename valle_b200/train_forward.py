@@ -131,8 +131,10 @@ def _valle_forward(model, x: torch.Tensor, x_lens: torch.Tensor, y, y_lens, redu
         return rows
 
     def final_norm(nd, rows, ada, sel):
-        wb = ada[2 * nd.n_layer] if ada is not None else None
         fn = nd.enc.norm
+        if fn is None:   # post-LN stacks have no final norm (valle.py:151,242-246)
+            return AG.GatherRows.apply(rows, sel, dtype)
+        wb = ada[2 * nd.n_layer] if ada is not None else None
         inner = fn.norm if ada is not None else fn
         return AG.LayerNormRows.apply(rows, inner.weight, inner.bias, wb, sel, inner.eps, dtype)
 
@@ -143,7 +145,8 @@ def _valle_forward(model, x: torch.Tensor, x_lens: torch.Tensor, y, y_lens, redu
         for lyr in enc.layers:
             for nm in (lyr.norm1, lyr.norm2):
                 wb += [nm.project_layer.weight, nm.project_layer.bias]
-        wb += [enc.norm.project_layer.weight, enc.norm.project_layer.bias]
+        if enc.norm is not None:
+            wb += [enc.norm.project_layer.weight, enc.norm.project_layer.bias]
         return AG.AdaTable.apply(stage_weight, *wb)
 
     # ---- AR decoder (valle.py:828-881) ----
