@@ -177,11 +177,179 @@ VB_API int vb_decoder_set_decode_fold(vb_decoder_t dec, const vb_ln_fold *qkv, c
 
 static size_t elem_size(int dtype) { return dtype == VB_BF16 ? 2 : 4; }
 
+// ------------------------------------------------------------------------------------------
+// Decoder stack: the forward of inference and training, and the backward pass
+// ------------------------------------------------------------------------------------------
+namespace {
+// Bump allocator: 256-byte aligned slots in the order they are taken.  Carved from a null base it hands out null slots
+// and only adds up the layout, so every workspace size below is its own layout carved from nullptr.
+struct Carve {
+  char *base;
+  size_t used = 0;
+  explicit Carve(const void *b) : base((char *)b) {}
+  template <class T = void>
+  T *take(size_t n) {
+    T *r = base ? (T *)(base + used) : nullptr;
+    used += align_up(n, 256);
+    return r;
+  }
+};
+// bytes of a buffer laid out by layout(c, a...): the layout carved from a null base
+template <class Layout, class... A>
+size_t carved_bytes(Layout layout, const A &...a) {
+  Carve c(nullptr);
+  layout(c, a...);
+  return c.used + 256;
+}
+
+// One layer's activations.  x_in / x_mid: fp32 [M, d] copies of the residual stream as norm1 / norm2 read it, what
+// the LayerNorm backward needs (null: not kept).  Storage dtype: xn1 (the QKV operand), q|k|v, attention out, xn2 (the
+// FFN1 operand), FFN hidden (post-ReLU, post-dropout).
+struct LayerSave {
+  float *x_in, *x_mid;
+  void *xn1, *qkv, *att, *xn2, *hb;
+};
+// the scratch of vb_decoder_forward: one set of slots that every layer reuses, no fp32 copies
+LayerSave carve_forward_ws(Carve &c, const vb_decoder_desc &D, int64_t M) {
+  const size_t ts = elem_size(D.wdtype), d = D.d_model, Mp = align_up((size_t)M, 128);
+  LayerSave s{};
+  s.xn1 = s.xn2 = c.take(Mp * d * ts);
+  s.qkv = c.take(Mp * 3 * d * ts);
+  s.att = c.take(Mp * d * ts);
+  s.hb = c.take(Mp * D.d_ff * ts);
+  return s;
+}
+LayerSave carve_layer_save(Carve &c, const vb_decoder_desc &D, int64_t M) {
+  const size_t ts = elem_size(D.wdtype), d = D.d_model, Mp = align_up((size_t)M, 128);
+  LayerSave s;
+  s.x_in = c.take<float>(Mp * d * 4);
+  s.x_mid = c.take<float>(Mp * d * 4);
+  s.xn1 = c.take(Mp * d * ts);
+  s.att = c.take(Mp * d * ts);
+  s.xn2 = c.take(Mp * d * ts);
+  s.qkv = c.take(Mp * 3 * d * ts);
+  s.hb = c.take(Mp * D.d_ff * ts);
+  return s;
+}
+// The training save buffer: one LayerSave block per layer, then an fp32 [M, d] scratch for the sub-layer output that
+// dropout scales ahead of the residual add (returned).
+float *carve_train_save(Carve &c, const vb_decoder_desc &D, int64_t M) {
+  for (int l = 0; l < D.n_layer; ++l) carve_layer_save(c, D, M);
+  return c.take<float>((size_t)M * D.d_model * 4);
+}
+// layer l's block of the training save buffer
+LayerSave layer_save(const vb_decoder_desc &D, int64_t M, const void *save, int l) {
+  Carve block(nullptr);
+  carve_layer_save(block, D, M);
+  Carve c((const char *)save + (size_t)l * block.used);
+  return carve_layer_save(c, D, M);
+}
+
+// norm k (1 or 2) of layer l: its row of an AdaLN (weight|bias) table [*, 2d] or of the table's gradient (null: LayerNorm)
+template <class T>
+T *ada_row(T *wb, int l, int k, int d) {
+  return wb ? wb + (size_t)(2 * l + k - 1) * 2 * d : nullptr;
+}
+// training-mode dropout of layer l (transformer.py:329,333-334, activation.py:199 `dropout=`) at site 0 (attention
+// probabilities), 1 (attention output), 2 (FFN hidden) or 3 (FFN output): the stateless hash of kernels.cuh on stream
+// (l << 2) | site, regenerated by the backward
+DropCfg layer_drop(float p, uint64_t seed, int l, int site) { return make_drop(p, seed, (uint32_t)(l << 2) | (uint32_t)site); }
+
+// The layer loop of vb_decoder_forward and vb_decoder_forward_train.  slots(l): layer l's activation slots; kcache /
+// vcache: null or the caches the attention fills; sub: the fp32 [M, d] scratch of the sub-layer outputs when
+// dropout_p > 0.  Pre-LN (transformer.py:297-302): x += SA(norm1(x)); x += FF(norm2(x)).  Post-LN (:303-308):
+// x = norm1(x + SA(x)); x = norm2(x + FF(x)); a post-norm writes the normalised rows back into x and into the
+// storage-dtype operand of the next GEMM, and layer 0 reads a plain cast.
+template <class Slots>
+int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32_t *cu_seqlens, const int32_t *text_lens,
+                  const int32_t *seg1_lens, int seg1_start, int max_seqlen, int mask_mode, const float *ada_wb,
+                  Slots slots, void *kcache, void *vcache, int64_t cache_layer_stride, int64_t cache_seq_stride,
+                  int cache_cap, float *sub, float dropout_p, uint64_t dropout_seed, cudaStream_t s) {
+  const vb_decoder_desc &D = dec->desc;
+  const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
+  const size_t ts = elem_size(dt);
+  const vb_stream_t stream = (vb_stream_t)s;
+  if (!D.norm_first) VB_TRY(launch_cast_from_f32(x, slots(0).xn1, dt, M * d, s));
+  for (int l = 0; l < D.n_layer; ++l) {
+    const vb_layer_params &P = dec->layers[l];
+    const LayerSave sv = slots(l);
+    // norm k reads x, copied first into the layer's fp32 slot if it has one, and writes the operand `out`
+    auto norm = [&](int k, void *out) -> int {
+      float *keep = k == 1 ? sv.x_in : sv.x_mid;
+      if (keep) VB_CUDA(cudaMemcpyAsync(keep, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
+      const float *w = k == 1 ? P.norm1_w : P.norm2_w, *b = k == 1 ? P.norm1_b : P.norm2_b;
+      if (D.norm_first) return vb_layernorm(x, d, nullptr, M, d, w, b, ada_row(ada_wb, l, k, d), 1e-5f, out, dt, stream);
+      return launch_post_norm(x, M, d, w, b, ada_row(ada_wb, l, k, d), 1e-5f, out, dt, s);
+    };
+    // x += in W^T + b, the sum ahead of the add through the dropout at `site`
+    auto residual = [&](const void *in, int K, const void *W, const float *b, int site) -> int {
+      if (dropout_p > 0.f) {
+        VB_TRY(vb_linear(in, dt, K, W, dt, b, sub, VB_F32, d, M, d, K, VB_EPI_NONE, nullptr, 0, stream));
+        return launch_dropout_add(x, sub, M * d, layer_drop(dropout_p, dropout_seed, l, site), s);
+      }
+      return vb_linear(in, dt, K, W, dt, b, x, VB_F32, d, M, d, K, VB_EPI_RESIDUAL, nullptr, 0, stream);
+    };
+    auto attn = [&]() -> int {
+      VB_TRY(vb_linear(sv.xn1, dt, d, P.in_proj_w, dt, P.in_proj_b, sv.qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE, nullptr,
+                       0, stream));
+      void *kc = kcache ? (char *)kcache + (size_t)l * cache_layer_stride * ts : nullptr;
+      void *vc = vcache ? (char *)vcache + (size_t)l * cache_layer_stride * ts : nullptr;
+      const DropCfg dc = layer_drop(dropout_p, dropout_seed, l, 0);
+      VB_TRY(launch_attention_varlen(sv.qkv, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
+                                     seg1_start, max_seqlen, mask_mode, sv.att, kc, vc, cache_seq_stride, cache_cap,
+                                     nullptr, 0, s, &dc));
+      return residual(sv.att, d, P.out_proj_w, P.out_proj_b, 1);
+    };
+    auto ffn = [&]() -> int {
+      VB_TRY(vb_linear(sv.xn2, dt, d, P.lin1_w, dt, P.lin1_b, sv.hb, dt, dff, M, dff, d, VB_EPI_RELU, nullptr, 0, stream));
+      if (dropout_p > 0.f)
+        VB_TRY(launch_dropout(sv.hb, sv.hb, dt, M * dff, layer_drop(dropout_p, dropout_seed, l, 2), s));
+      return residual(sv.hb, dff, P.lin2_w, P.lin2_b, 3);
+    };
+    if (D.norm_first) {
+      VB_TRY(norm(1, sv.xn1));
+      VB_TRY(attn());
+      VB_TRY(norm(2, sv.xn2));
+      VB_TRY(ffn());
+    } else {
+      VB_TRY(attn());
+      VB_TRY(norm(1, sv.xn2));
+      VB_TRY(ffn());
+      VB_TRY(norm(2, l + 1 < D.n_layer ? slots(l + 1).xn1 : nullptr));
+    }
+  }
+  return VB_OK;
+}
+
+struct BackwardWs {
+  void *dx_dt;          // dx in the storage dtype
+  void *dy;             // dx through the mask of a sub-layer's output dropout
+  void *dh, *dO, *dqkv;
+  float *dn;            // pre-LN: the gradient of a norm's output
+  float *dr;            // post-LN: the gradient between the two post-norms (null for pre-LN)
+  void *attn_ws, *lin_ws;
+  size_t attn_ws_bytes, lin_ws_bytes;
+};
+BackwardWs carve_backward_ws(Carve &c, const vb_decoder_desc &D, int64_t M) {
+  const size_t ts = elem_size(D.wdtype), d = D.d_model, dff = D.d_ff, Mp = align_up((size_t)M, 128);
+  BackwardWs w{};
+  w.dx_dt = c.take(Mp * d * ts);
+  w.dy = c.take(Mp * d * ts);
+  w.dh = c.take(Mp * dff * ts);
+  w.dn = c.take<float>(Mp * d * 4);
+  w.dO = c.take(Mp * d * ts);
+  w.dqkv = c.take(Mp * 3 * d * ts);
+  w.attn_ws_bytes = vb_attention_backward_workspace(M, D.n_head);
+  w.attn_ws = c.take(w.attn_ws_bytes);
+  w.lin_ws_bytes = vb_linear_backward_workspace(D.wdtype, M, std::max(D.d_ff, 3 * D.d_model), std::max(D.d_ff, D.d_model));
+  w.lin_ws = c.take(w.lin_ws_bytes);
+  if (!D.norm_first) w.dr = c.take<float>(Mp * d * 4);
+  return w;
+}
+}  // namespace
+
 VB_API size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t M) {
-  const size_t ts = elem_size(desc->wdtype);
-  const size_t d = desc->d_model, dff = desc->d_ff;
-  const size_t Mp = align_up((size_t)M, 128);
-  return Mp * (d + 3 * d + d + dff) * ts + 4 * 256;
+  return carved_bytes(carve_forward_ws, *desc, M);
 }
 
 VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
@@ -196,81 +364,15 @@ VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, cons
                "vb_decoder_forward: workspace too small (%zu < %zu)", workspace_bytes,
                vb_decoder_forward_workspace(&D, M));
   if (M == 0) return VB_OK;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
-  const size_t ts = elem_size(dt);
-  const size_t Mp = align_up((size_t)M, 128);
-  char *ws = (char *)workspace;
-  void *xn = ws;   ws += align_up(Mp * d * ts, 256);
-  void *qkv = ws;  ws += align_up(Mp * 3 * d * ts, 256);
-  void *att = ws;  ws += align_up(Mp * d * ts, 256);
-  void *hb = ws;
-  // post-LN (transformer.py:303-308): x = norm1(x + SA(x)); x = norm2(x + FF(x)).  Each post-norm writes the normalised
-  // rows back into x and into the storage-dtype copy xn the next GEMM reads; layer 0 reads a plain cast.
-  const bool post = !D.norm_first;
-  if (post) VB_TRY(launch_cast_from_f32(x, xn, dt, M * d, s));
-  for (int l = 0; l < D.n_layer; ++l) {
-    const vb_layer_params &P = dec->layers[l];
-    const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
-    const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-    if (!post) VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, xn, dt, stream));
-    VB_TRY(vb_linear(xn, dt, d, P.in_proj_w, dt, P.in_proj_b, qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE,
-                     nullptr, 0, stream));
-    void *kc = kcache ? (char *)kcache + (size_t)l * cache_layer_stride * ts : nullptr;
-    void *vc = vcache ? (char *)vcache + (size_t)l * cache_layer_stride * ts : nullptr;
-    VB_TRY(launch_attention_varlen(qkv, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
-                                   mask_mode, att, kc, vc, cache_seq_stride, cache_cap, nullptr, 0, s));
-    VB_TRY(vb_linear(att, dt, d, P.out_proj_w, dt, P.out_proj_b, x, VB_F32, d, M, d, d, VB_EPI_RESIDUAL,
-                     nullptr, 0, stream));
-    if (post)
-      VB_TRY(launch_post_norm(x, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, xn, dt, s));
-    else
-      VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, xn, dt, stream));
-    VB_TRY(vb_linear(xn, dt, d, P.lin1_w, dt, P.lin1_b, hb, dt, dff, M, dff, d, VB_EPI_RELU, nullptr, 0,
-                     stream));
-    VB_TRY(vb_linear(hb, dt, dff, P.lin2_w, dt, P.lin2_b, x, VB_F32, d, M, d, dff, VB_EPI_RESIDUAL, nullptr,
-                     0, stream));
-    if (post) VB_TRY(launch_post_norm(x, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, xn, dt, s));
-  }
-  return VB_OK;
+  Carve c(workspace);
+  const LayerSave ws = carve_forward_ws(c, D, M);
+  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
+                       [&](int) { return ws; }, kcache, vcache, cache_layer_stride, cache_seq_stride, cache_cap,
+                       nullptr, 0.f, 0, (cudaStream_t)stream);
 }
-
-// ------------------------------------------------------------------------------------------
-// Training: forward that keeps the activations, and the backward pass of the stack
-// ------------------------------------------------------------------------------------------
-namespace {
-struct LayerSave {
-  float *x_in, *x_mid;          // fp32 [M, d] residual stream at the layer input / after the attention block
-  void *xn1, *qkv, *att, *xn2, *hb;  // storage dtype: LN1 out, q|k|v, attention out, LN2 out, FFN hidden (post-ReLU)
-};
-size_t layer_save_bytes(const vb_decoder_desc &D, int64_t M) {
-  const size_t ts = elem_size(D.wdtype), d = D.d_model, dff = D.d_ff, Mp = align_up((size_t)M, 128);
-  return 2 * align_up(Mp * d * 4, 256) + 3 * align_up(Mp * d * ts, 256) + align_up(Mp * 3 * d * ts, 256) +
-         align_up(Mp * dff * ts, 256);
-}
-LayerSave carve_layer_save(const vb_decoder_desc &D, int64_t M, char *base) {
-  const size_t ts = elem_size(D.wdtype), d = D.d_model, dff = D.d_ff, Mp = align_up((size_t)M, 128);
-  LayerSave s{};
-  char *p = base;
-  auto take = [&](size_t n) {
-    char *r = p;
-    p += align_up(n, 256);
-    return r;
-  };
-  s.x_in = (float *)take(Mp * d * 4);
-  s.x_mid = (float *)take(Mp * d * 4);
-  s.xn1 = take(Mp * d * ts);
-  s.att = take(Mp * d * ts);
-  s.xn2 = take(Mp * d * ts);
-  s.qkv = take(Mp * 3 * d * ts);
-  s.hb = take(Mp * dff * ts);
-  return s;
-}
-}  // namespace
 
 VB_API size_t vb_decoder_train_save_bytes(const vb_decoder_desc *desc, int64_t M) {
-  // + one fp32 [M, d] scratch behind the layers: the sub-layer output that dropout scales before the residual add
-  return (size_t)desc->n_layer * layer_save_bytes(*desc, M) + align_up((size_t)M * desc->d_model * 4, 256) + 256;
+  return carved_bytes(carve_train_save, *desc, M);
 }
 
 VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
@@ -282,77 +384,15 @@ VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B
   const vb_decoder_desc &D = dec->desc;
   VB_CHECK_ARG(save_bytes >= vb_decoder_train_save_bytes(&D, M), "vb_decoder_forward_train: save buffer too small");
   if (M == 0) return VB_OK;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
-  const size_t per_layer = layer_save_bytes(D, M);
-  const bool drop = dropout_p > 0.f;
-  float *sub = (float *)((char *)save + (size_t)D.n_layer * per_layer);   // sub-layer output ahead of its dropout
-  // post-LN: the save slots hold r1 = x + drop(SA(x)) (x_in), r2 = x1 + drop(FF(x1)) (x_mid), and the storage-dtype GEMM
-  // operands x (xn1) and x1 = norm1(r1) (xn2); the post-norm of layer l writes layer l+1's xn1
-  const bool post = !D.norm_first;
-  if (post) VB_TRY(launch_cast_from_f32(x, carve_layer_save(D, M, (char *)save).xn1, dt, (int64_t)M * d, s));
-  for (int l = 0; l < D.n_layer; ++l) {
-    const vb_layer_params &P = dec->layers[l];
-    LayerSave sv = carve_layer_save(D, M, (char *)save + (size_t)l * per_layer);
-    const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
-    const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-    if (!post) {
-      VB_CUDA(cudaMemcpyAsync(sv.x_in, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
-      VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, sv.xn1, dt, stream));
-    }
-    VB_TRY(vb_linear(sv.xn1, dt, d, P.in_proj_w, dt, P.in_proj_b, sv.qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE, nullptr, 0,
-                     stream));
-    // training-mode dropout (p > 0): attention probabilities (activation.py:199 `dropout=`), dropout1 / dropout2 on
-    // the sub-layer outputs and `dropout` on the FFN hidden (transformer.py:329,333-334); masks from the stateless
-    // hash of kernels.cuh, site streams (l << 2) | {0, 1, 2, 3}, regenerated by vb_decoder_backward
-    const DropCfg dc_attn = make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 0u);
-    VB_TRY(launch_attention_varlen(sv.qkv, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                   max_seqlen, mask_mode, sv.att, nullptr, nullptr, 0, 0, nullptr, 0, s, &dc_attn));
-    if (drop) {
-      VB_TRY(vb_linear(sv.att, dt, d, P.out_proj_w, dt, P.out_proj_b, sub, VB_F32, d, M, d, d, VB_EPI_NONE, nullptr, 0,
-                       stream));
-      VB_TRY(launch_dropout_add(x, sub, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 1u), s));
-    } else {
-      VB_TRY(vb_linear(sv.att, dt, d, P.out_proj_w, dt, P.out_proj_b, x, VB_F32, d, M, d, d, VB_EPI_RESIDUAL, nullptr, 0,
-                       stream));
-    }
-    if (post) {
-      VB_CUDA(cudaMemcpyAsync(sv.x_in, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
-      VB_TRY(launch_post_norm(x, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, sv.xn2, dt, s));
-    } else {
-      VB_CUDA(cudaMemcpyAsync(sv.x_mid, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
-      VB_TRY(vb_layernorm(x, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, sv.xn2, dt, stream));
-    }
-    VB_TRY(vb_linear(sv.xn2, dt, d, P.lin1_w, dt, P.lin1_b, sv.hb, dt, dff, M, dff, d, VB_EPI_RELU, nullptr, 0, stream));
-    if (drop) {
-      VB_TRY(launch_dropout(sv.hb, sv.hb, dt, (int64_t)M * dff, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 2u), s));
-      VB_TRY(vb_linear(sv.hb, dt, dff, P.lin2_w, dt, P.lin2_b, sub, VB_F32, d, M, d, dff, VB_EPI_NONE, nullptr, 0, stream));
-      VB_TRY(launch_dropout_add(x, sub, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 3u), s));
-    } else {
-      VB_TRY(vb_linear(sv.hb, dt, dff, P.lin2_w, dt, P.lin2_b, x, VB_F32, d, M, d, dff, VB_EPI_RESIDUAL, nullptr, 0, stream));
-    }
-    if (post) {
-      VB_CUDA(cudaMemcpyAsync(sv.x_mid, x, (size_t)M * d * 4, cudaMemcpyDeviceToDevice, s));
-      void *next_xn1 = l + 1 < D.n_layer ? carve_layer_save(D, M, (char *)save + (size_t)(l + 1) * per_layer).xn1 : nullptr;
-      VB_TRY(launch_post_norm(x, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, next_xn1, dt, s));
-    }
-  }
-  return VB_OK;
+  Carve c(save);
+  float *sub = carve_train_save(c, D, M);
+  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
+                       [&](int l) { return layer_save(D, M, save, l); }, nullptr, nullptr, 0, 0, 0, sub, dropout_p,
+                       dropout_seed, (cudaStream_t)stream);
 }
 
 VB_API size_t vb_decoder_backward_workspace(const vb_decoder_desc *desc, int64_t M) {
-  const size_t ts = elem_size(desc->wdtype), d = desc->d_model, dff = desc->d_ff, Mp = align_up((size_t)M, 128);
-  size_t n = 0;
-  n += align_up(Mp * d * ts, 256);        // dx in the storage dtype
-  n += align_up(Mp * d * ts, 256);        // dy: dx through the mask of a sub-layer's output dropout
-  n += align_up(Mp * dff * ts, 256);      // dh
-  n += align_up(Mp * d * 4, 256);         // dc / da (fp32)
-  n += align_up(Mp * d * ts, 256);        // do
-  n += align_up(Mp * 3 * d * ts, 256);    // dqkv
-  n += align_up(vb_attention_backward_workspace(M, desc->n_head), 256);
-  n += align_up(vb_linear_backward_workspace(desc->wdtype, M, (int)std::max(dff, 3 * d), (int)std::max(dff, d)), 256);
-  if (!desc->norm_first) n += align_up(Mp * d * 4, 256);   // post-LN: the gradient between the two post-norms
-  return n + 256;
+  return carved_bytes(carve_backward_ws, *desc, M);
 }
 
 VB_API int vb_decoder_backward(vb_decoder_t dec, float *dx, int64_t M, int B, const int32_t *cu_seqlens,
@@ -368,111 +408,65 @@ VB_API int vb_decoder_backward(vb_decoder_t dec, float *dx, int64_t M, int B, co
   if (M == 0) return VB_OK;
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
-  const size_t ts = elem_size(dt), Mp = align_up((size_t)M, 128);
-  char *p = (char *)workspace;
-  auto take = [&](size_t n) {
-    char *r = p;
-    p += align_up(n, 256);
-    return r;
-  };
-  void *dx_dt = take(Mp * d * ts);
-  void *dy = take(Mp * d * ts);
-  void *dh = take(Mp * dff * ts);
+  Carve c(workspace);
+  const BackwardWs w = carve_backward_ws(c, D, M);
   const bool drop = dropout_p > 0.f;
   const float inv_keep = drop ? 1.f / (1.f - dropout_p) : 1.f;
-  float *dn = (float *)take(Mp * d * 4);
-  void *dO = take(Mp * d * ts);
-  void *dqkv = take(Mp * 3 * d * ts);
-  const size_t attn_ws_bytes = vb_attention_backward_workspace(M, D.n_head);
-  void *attn_ws = take(attn_ws_bytes);
-  const size_t lin_ws_bytes = vb_linear_backward_workspace(dt, M, std::max(dff, 3 * d), std::max(dff, d));
-  void *lin_ws = take(lin_ws_bytes);
-  const size_t per_layer = layer_save_bytes(D, M);
-  if (!D.norm_first) {
-    // post-LN, per layer from the top: y = norm2(r2), r2 = x1 + drop(FF(x1)), x1 = norm1(r1), r1 = x + drop(SA(x)).
-    // dx holds dy on entry; dr = norm2^T(dy) replaces it, the FFN input gradient is added to dr (= dx1),
-    // dx = norm1^T(dx1), the attention input gradient is added to dx (= the layer input's gradient).
-    float *dr = (float *)take(Mp * d * 4);
-    for (int l = D.n_layer - 1; l >= 0; --l) {
-      const vb_layer_params &P = dec->layers[l];
-      const vb_layer_grads &G = grads[l];
-      const vb_layer_wt &T = wt[l];
-      LayerSave sv = carve_layer_save(D, M, (char *)const_cast<void *>(save) + (size_t)l * per_layer);
-      const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
-      const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-      float *dada1 = dada_wb ? dada_wb + (size_t)(2 * l) * 2 * d : nullptr;
-      float *dada2 = dada_wb ? dada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-      VB_CUDA(cudaMemsetAsync(dr, 0, (size_t)M * d * 4, s));
-      VB_TRY(vb_layernorm_backward(sv.x_mid, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, dx, d, dr, d, dx_dt, dt,
-                                   G.norm2_w, G.norm2_b, dada2, stream));
-      const void *dy2 = dx_dt;
-      if (drop) {
-        VB_TRY(launch_dropout(dx_dt, dy, dt, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 3u), s));
-        dy2 = dy;
-      }
-      VB_TRY(vb_linear_backward(sv.hb, dt, dff, T.lin2_wt, dy2, d, dh, dt, dff, VB_EPI_NONE, G.lin2_w, G.lin2_b, M, d, dff,
-                                lin_ws, lin_ws_bytes, stream));
-      VB_TRY(launch_relu_bwd(dh, sv.hb, dt, (int64_t)M * dff, inv_keep, s));
-      VB_TRY(vb_linear_backward(sv.xn2, dt, d, T.lin1_wt, dh, dff, dr, VB_F32, d, VB_EPI_RESIDUAL, G.lin1_w, G.lin1_b, M,
-                                dff, d, lin_ws, lin_ws_bytes, stream));
-      VB_CUDA(cudaMemsetAsync(dx, 0, (size_t)M * d * 4, s));
-      VB_TRY(vb_layernorm_backward(sv.x_in, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, dr, d, dx, d, dx_dt, dt,
-                                   G.norm1_w, G.norm1_b, dada1, stream));
-      const void *dy1 = dx_dt;
-      if (drop) {
-        VB_TRY(launch_dropout(dx_dt, dy, dt, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 1u), s));
-        dy1 = dy;
-      }
-      VB_TRY(vb_linear_backward(sv.att, dt, d, T.out_proj_wt, dy1, d, dO, dt, d, VB_EPI_NONE, G.out_proj_w, G.out_proj_b, M,
-                                d, d, lin_ws, lin_ws_bytes, stream));
-      const DropCfg dc_attn = make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 0u);
-      VB_TRY(attention_backward(sv.qkv, sv.att, dO, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
-                                seg1_start, max_seqlen, mask_mode, dqkv, attn_ws, attn_ws_bytes, &dc_attn, s));
-      VB_TRY(vb_linear_backward(sv.xn1, dt, d, T.in_proj_wt, dqkv, 3 * d, dx, VB_F32, d, VB_EPI_RESIDUAL, G.in_proj_w,
-                                G.in_proj_b, M, 3 * d, d, lin_ws, lin_ws_bytes, stream));
-    }
-    return VB_OK;
-  }
-  VB_TRY(launch_cast_from_f32(dx, dx_dt, dt, (int64_t)M * d, s));
+  // dx holds the gradient of the stack output on entry.  dx_dt, the residual stream's gradient in the storage dtype
+  // (refreshed by each LayerNorm backward), is the gradient of the output of the sub-layer handled next; dy is that
+  // gradient through the mask of the sub-layer's output dropout
+  const void *dy = drop ? w.dy : w.dx_dt;
+  if (D.norm_first) VB_TRY(launch_cast_from_f32(dx, w.dx_dt, dt, M * d, s));
   for (int l = D.n_layer - 1; l >= 0; --l) {
     const vb_layer_params &P = dec->layers[l];
     const vb_layer_grads &G = grads[l];
     const vb_layer_wt &T = wt[l];
-    LayerSave sv = carve_layer_save(D, M, (char *)const_cast<void *>(save) + (size_t)l * per_layer);
-    const float *ada1 = ada_wb ? ada_wb + (size_t)(2 * l) * 2 * d : nullptr;
-    const float *ada2 = ada_wb ? ada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-    float *dada1 = dada_wb ? dada_wb + (size_t)(2 * l) * 2 * d : nullptr;
-    float *dada2 = dada_wb ? dada_wb + (size_t)(2 * l + 1) * 2 * d : nullptr;
-    // ---- FFN: x2 = x1 + relu(LN2(x1) W1^T + b1) W2^T + b2 (transformer.py:332-334) ----
-    // (with dropout: the saved hidden is post-dropout -- zero where dropped -- and dx reaches the sub-layer output
-    //  through the mask of dropout2)
-    const void *dy2 = dx_dt;
-    if (drop) {
-      VB_TRY(launch_dropout(dx_dt, dy, dt, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 3u), s));
-      dy2 = dy;
+    const LayerSave sv = layer_save(D, M, save, l);
+    // norm k: from the gradient dout of its output, the gradient of its input added into dst and copied into dx_dt
+    auto norm = [&](int k, const float *dout, float *dst) -> int {
+      const bool n1 = k == 1;
+      return vb_layernorm_backward(n1 ? sv.x_in : sv.x_mid, d, nullptr, M, d, n1 ? P.norm1_w : P.norm2_w,
+                                   n1 ? P.norm1_b : P.norm2_b, ada_row(ada_wb, l, k, d), 1e-5f, dout, d, dst, d, w.dx_dt,
+                                   dt, n1 ? G.norm1_w : G.norm2_w, n1 ? G.norm1_b : G.norm2_b, ada_row(dada_wb, l, k, d),
+                                   stream);
+    };
+    // FFN block x + linear2(drop(relu(linear1(xn2)))): the input gradient into dst by the epilogue epi (with dropout
+    // the saved hidden is post-dropout, zero where dropped)
+    auto ffn = [&](float *dst, int epi) -> int {
+      if (drop) VB_TRY(launch_dropout(w.dx_dt, w.dy, dt, M * d, layer_drop(dropout_p, dropout_seed, l, 3), s));
+      VB_TRY(vb_linear_backward(sv.hb, dt, dff, T.lin2_wt, dy, d, w.dh, dt, dff, VB_EPI_NONE, G.lin2_w, G.lin2_b, M, d, dff,
+                                w.lin_ws, w.lin_ws_bytes, stream));
+      VB_TRY(launch_relu_bwd(w.dh, sv.hb, dt, M * dff, inv_keep, s));
+      return vb_linear_backward(sv.xn2, dt, d, T.lin1_wt, w.dh, dff, dst, VB_F32, d, epi, G.lin1_w, G.lin1_b, M, dff, d,
+                                w.lin_ws, w.lin_ws_bytes, stream);
+    };
+    // attention block x + out_proj(Attn(in_proj(xn1))): input gradient into dst by the epilogue epi
+    auto attn = [&](float *dst, int epi) -> int {
+      if (drop) VB_TRY(launch_dropout(w.dx_dt, w.dy, dt, M * d, layer_drop(dropout_p, dropout_seed, l, 1), s));
+      VB_TRY(vb_linear_backward(sv.att, dt, d, T.out_proj_wt, dy, d, w.dO, dt, d, VB_EPI_NONE, G.out_proj_w, G.out_proj_b,
+                                M, d, d, w.lin_ws, w.lin_ws_bytes, stream));
+      const DropCfg dc = layer_drop(dropout_p, dropout_seed, l, 0);
+      VB_TRY(attention_backward(sv.qkv, sv.att, w.dO, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
+                                seg1_start, max_seqlen, mask_mode, w.dqkv, w.attn_ws, w.attn_ws_bytes, &dc, s));
+      return vb_linear_backward(sv.xn1, dt, d, T.in_proj_wt, w.dqkv, 3 * d, dst, VB_F32, d, epi, G.in_proj_w,
+                                G.in_proj_b, M, 3 * d, d, w.lin_ws, w.lin_ws_bytes, stream);
+    };
+    if (D.norm_first) {
+      // each block's input gradient goes to dn, and its norm's backward adds it to the residual gradient in dx
+      VB_TRY(ffn(w.dn, VB_EPI_NONE));
+      VB_TRY(norm(2, w.dn, dx));
+      VB_TRY(attn(w.dn, VB_EPI_NONE));
+      VB_TRY(norm(1, w.dn, dx));
+    } else {
+      // y = norm2(r2), r2 = x1 + drop(FF(x1)), x1 = norm1(r1), r1 = x + drop(SA(x)): dr = norm2^T(dy), the FFN input
+      // gradient is added to dr (= dx1), dx = norm1^T(dx1), the attention input gradient is added to dx
+      VB_CUDA(cudaMemsetAsync(w.dr, 0, (size_t)M * d * 4, s));
+      VB_TRY(norm(2, dx, w.dr));
+      VB_TRY(ffn(w.dr, VB_EPI_RESIDUAL));
+      VB_CUDA(cudaMemsetAsync(dx, 0, (size_t)M * d * 4, s));
+      VB_TRY(norm(1, w.dr, dx));
+      VB_TRY(attn(dx, VB_EPI_RESIDUAL));
     }
-    VB_TRY(vb_linear_backward(sv.hb, dt, dff, T.lin2_wt, dy2, d, dh, dt, dff, VB_EPI_NONE, G.lin2_w, G.lin2_b, M, d, dff,
-                              lin_ws, lin_ws_bytes, stream));
-    VB_TRY(launch_relu_bwd(dh, sv.hb, dt, (int64_t)M * dff, inv_keep, s));
-    VB_TRY(vb_linear_backward(sv.xn2, dt, d, T.lin1_wt, dh, dff, dn, VB_F32, d, VB_EPI_NONE, G.lin1_w, G.lin1_b, M, dff, d,
-                              lin_ws, lin_ws_bytes, stream));
-    VB_TRY(vb_layernorm_backward(sv.x_mid, d, nullptr, M, d, P.norm2_w, P.norm2_b, ada2, 1e-5f, dn, d, dx, d, dx_dt, dt,
-                                 G.norm2_w, G.norm2_b, dada2, stream));
-    // ---- attention block: x1 = x + Attn(LN1(x) Win^T + bin) Wo^T + bo (transformer.py:315-330) ----
-    const void *dy1 = dx_dt;
-    if (drop) {
-      VB_TRY(launch_dropout(dx_dt, dy, dt, (int64_t)M * d, make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 1u), s));
-      dy1 = dy;
-    }
-    VB_TRY(vb_linear_backward(sv.att, dt, d, T.out_proj_wt, dy1, d, dO, dt, d, VB_EPI_NONE, G.out_proj_w, G.out_proj_b, M, d,
-                              d, lin_ws, lin_ws_bytes, stream));
-    const DropCfg dc_attn = make_drop(dropout_p, dropout_seed, (uint32_t)(l << 2) | 0u);
-    VB_TRY(attention_backward(sv.qkv, sv.att, dO, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
-                              seg1_start, max_seqlen, mask_mode, dqkv, attn_ws, attn_ws_bytes, &dc_attn, s));
-    VB_TRY(vb_linear_backward(sv.xn1, dt, d, T.in_proj_wt, dqkv, 3 * d, dn, VB_F32, d, VB_EPI_NONE, G.in_proj_w, G.in_proj_b,
-                              M, 3 * d, d, lin_ws, lin_ws_bytes, stream));
-    VB_TRY(vb_layernorm_backward(sv.x_in, d, nullptr, M, d, P.norm1_w, P.norm1_b, ada1, 1e-5f, dn, d, dx, d, dx_dt, dt,
-                                 G.norm1_w, G.norm1_b, dada1, stream));
   }
   return VB_OK;
 }
@@ -488,28 +482,20 @@ struct StepWs {
   void *gemm_ws;
   float *stats;  // moments of the folded-LayerNorm projections: [kMaxForcedSplits][64][2]
   size_t gemm_ws_bytes;
-  size_t total;
 };
-StepWs carve_step_ws(const vb_decoder_desc &D, int B, int cache_cap, void *base) {
+StepWs carve_step_ws(Carve &c, const vb_decoder_desc &D, int B, int cache_cap) {
   const size_t d = D.d_model, dff = D.d_ff;
   StepWs w{};
-  char *p = (char *)base;
-  auto take = [&](size_t n) {
-    char *r = p;
-    p += align_up(n, 256);
-    return r;
-  };
-  w.q = (float *)take((size_t)B * d * 4);
-  w.att = (float *)take((size_t)B * d * 4);
-  w.hb = (float *)take((size_t)B * dff * 4);
-  w.attn_ws = take(attn_decode_workspace(B, D.n_head, (int)(d / D.n_head), cache_cap));
-  w.xn16 = (bf16 *)take((size_t)64 * d * 2);
-  w.att16 = (bf16 *)take((size_t)64 * d * 2);
-  w.hb16 = (bf16 *)take((size_t)64 * dff * 2);
+  w.q = c.take<float>((size_t)B * d * 4);
+  w.att = c.take<float>((size_t)B * d * 4);
+  w.hb = c.take<float>((size_t)B * dff * 4);
+  w.attn_ws = c.take(attn_decode_workspace(B, D.n_head, (int)(d / D.n_head), cache_cap));
+  w.xn16 = c.take<bf16>((size_t)64 * d * 2);
+  w.att16 = c.take<bf16>((size_t)64 * d * 2);
+  w.hb16 = c.take<bf16>((size_t)64 * dff * 2);
   w.gemm_ws_bytes = gemm_decode_workspace((int)d, (int)dff);
-  w.gemm_ws = take(w.gemm_ws_bytes);
-  w.stats = (float *)take((size_t)kLnFoldMaxCopies * kMaxForcedSplits * 64 * 2 * sizeof(float));
-  w.total = (size_t)(p - (char *)base) + 256;
+  w.gemm_ws = c.take(w.gemm_ws_bytes);
+  w.stats = c.take<float>((size_t)kLnFoldMaxCopies * kMaxForcedSplits * 64 * 2 * sizeof(float));
   return w;
 }
 // tensor-core decode path: bf16 storage, up to 64 rows (one UMMA N tile)
@@ -519,7 +505,7 @@ bool use_tc_decode(const vb_decoder_desc &D, int B) {
 }  // namespace
 
 VB_API size_t vb_ar_step_workspace(const vb_decoder_desc *desc, int B, int cache_cap) {
-  return carve_step_ws(*desc, B, cache_cap, nullptr).total;
+  return carved_bytes(carve_step_ws, *desc, B, cache_cap);
 }
 
 namespace {
@@ -577,7 +563,8 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
   if (use_tc_decode(D, st->B)) {
     VB_CHECK_ARG(workspace && workspace_bytes >= vb_ar_step_workspace(&D, st->B, st->cache_cap),
                  "vb_ar_head_step: workspace too small");
-    StepWs w = carve_step_ws(D, st->B, st->cache_cap, workspace);
+    Carve c(workspace);
+    const StepWs w = carve_step_ws(c, D, st->B, st->cache_cap);
     return tc_head(dec, head, const_cast<float *>(h), st, w, Pending{}, s);
   }
   LnParams ln{D.final_norm_w, D.final_norm_b, nullptr, 1e-5f};
@@ -612,7 +599,8 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model, dff = D.d_ff, B = st->B, dt = D.wdtype, hd = d / D.n_head;
   const size_t ts = elem_size(dt);
-  StepWs w = carve_step_ws(D, B, st->cache_cap, workspace);
+  Carve c(workspace);
+  const StepWs w = carve_step_ws(c, D, B, st->cache_cap);
   float *x = st->x_cur;
   const bool post = !D.norm_first;
   if (use_tc_decode(D, B)) {
