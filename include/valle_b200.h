@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 6
+#define VB_ABI_VERSION 7
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32. */
@@ -386,6 +386,102 @@ int vb_gather_rows(const float *src, int64_t src_row_stride, const int32_t *rows
 
 /* out[i] = in[i] rounded to `dtype` (VB_F32: a copy), n fp32 values: the head operand of a stack without a final norm */
 int vb_cast_from_f32(const float *in, void *out, int dtype, int64_t n, vb_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * f3  Optimizer steps of the trainer (bin/trainer.py:923-951, 688): ScaledAdam and Eve of
+ *     valle/modules/optim.py:129-661, 836-985, fp32 parameters, updated in place.
+ *   Every tensor is cut into chunks of VB_OPTIM_CHUNK elements; a tensor's chunk0 is the sum of
+ *   ceil(numel / VB_OPTIM_CHUNK) over the tensors before it in the table.  Each chunk's partial
+ *   sums land in the workspace and are added per tensor in chunk order, so a step is
+ *   deterministic run to run.  Up to VB_OPTIM_MAX_TENSORS gradient pointers travel by value with
+ *   each launch; a longer table is split over several launches.
+ * ---------------------------------------------------------------------------------------- */
+#define VB_OPTIM_CHUNK 16384
+#define VB_OPTIM_MAX_TENSORS 1024
+
+/* One real parameter of a ScaledAdam batch (the parameters of one (dtype, *shape) key, stacked
+ * state of optim.py:265-314).  The state pointers address this parameter's slot of the batch's
+ * stacked state: delta[i], exp_avg_sq[i], param_rms[i], scale_exp_avg_sq[i], scale_grads[0, i]. */
+typedef struct vb_scaled_adam_tensor {
+  float *param;
+  float *delta;
+  float *exp_avg_sq;
+  float *param_rms;        /* NULL for a lone scalar (a stack of k > 1 scalars has one, set once at init) */
+  float *scale_exp_avg_sq; /* NULL for a scalar */
+  float *scale_grads;      /* NULL for a scalar */
+  int64_t numel;
+  int32_t chunk0;
+  int32_t sg_stride; /* floats between scale_grads[k, i] and scale_grads[k + 1, i]: the batch size */
+  int32_t scalar;    /* 1: the _step_scalar update (one element per parameter) */
+  int32_t pad;
+} vb_scaled_adam_tensor;
+
+/* The host-known scalars of one ScaledAdam step of a parameter group. */
+typedef struct vb_scaled_adam_args {
+  int32_t n_tensors;
+  int32_t n_chunks;
+  int32_t step;        /* state["step"] of the group's batches before this step */
+  int32_t zero_step;   /* state["zero_step"], 0 when absent: only the non-scalar bias correction subtracts it */
+  int32_t init;        /* 1: the state was just created: param_rms is set from the parameter first (optim.py:297-304) */
+  int32_t clip_mode;   /* 0: no clipping (step 0, clipping_scale None); 1: record the norm in model_norms only;
+                          2: record it and clip by the device-resident threshold (optim.py:391-412) */
+  int32_t clip_period; /* clipping_update_period */
+  int32_t size_period; /* size_update_period */
+  double clipping_scale, lr, scalar_lr_scale, beta1, beta2, eps, param_min_rms, param_max_rms, scalar_max;
+} vb_scaled_adam_args;
+
+/* Device-resident clipping state of a parameter group (caller-allocated, 32 bytes, zero-initialised). */
+typedef struct vb_clip_state {
+  double threshold;     /* model_norm_threshold = clipping_scale * median of model_norms, set on a period step */
+  float scale;          /* the clip scale of the last step (1 when not clipping) */
+  float min_scale;      /* smallest scale of the current period (1 when none) */
+  float prev_min_scale; /* min_scale of the period the last period step closed */
+  int32_t num_clipped;  /* steps of the current period with scale < 1 */
+  int32_t prev_clipped; /* num_clipped of the period the last period step closed */
+  int32_t has_threshold;
+} vb_clip_state;
+
+size_t vb_scaled_adam_workspace(int n_tensors, int n_chunks);
+/* One ScaledAdam step of a parameter group (optim.py:215-661), three launches per VB_OPTIM_MAX_TENSORS tensors:
+ *   1. per chunk: sum g^2, sum p*g, sum p^2 (p and g read once);
+ *   2. one CTA: per-tensor sums in chunk order; tot_sumsq = sum over tensors of sum g^2 (scalars) or param_rms^2 *
+ *      sum g^2; with clip_mode >= 1 model_norms[step % clip_period] = sqrt(tot_sumsq), and on a period step
+ *      (step % clip_period == 0) threshold = clipping_scale * the element of sorted model_norms at
+ *      min(P - 1, (P / 4) * 2), num_clipped -> prev_clipped, min_scale -> prev_min_scale, both reset; with
+ *      clip_mode == 2 and a threshold, scale = min(1, threshold / (norm + 1e-20)), counted when < 1.  Then
+ *      scale_grads[step % size_period] = scale * sum p*g, and when step % size_period == size_period - 1 param_rms =
+ *      sqrt(sum p^2 / numel) and, if step > 0, the size update of optim.py:531-596, one coefficient per tensor;
+ *   3. per element (16-byte accesses), with the UNCLIPPED g (the reference's _step and _step_scalar read p.grad; the
+ *      clip scale only enters scale_grads): delta *= beta1; [size step: delta += (1 - beta1) * p *
+ *      scale_step]; exp_avg_sq = beta2 * exp_avg_sq + (1 - beta2) g^2; delta += g / (sqrt(exp_avg_sq / bc2) + eps) *
+ *      alpha (alpha = -lr (1 - beta1) max(param_rms, param_min_rms)); p += delta.  Scalars: the same with
+ *      lr * scalar_lr_scale and p clamped to +-scalar_max before p += delta (optim.py:639-661).
+ * tensors: DEVICE array of n_tensors entries; grads: HOST array of n_tensors gradient pointers (NULL = zeros);
+ * chunk0: HOST array of n_tensors + 1 chunk offsets, equal to the table's (the last one is n_chunks). */
+int vb_scaled_adam_step(const vb_scaled_adam_tensor *tensors, const float *const *grads, const int32_t *chunk0,
+                        const vb_scaled_adam_args *args, float *model_norms, vb_clip_state *clip, void *workspace,
+                        size_t ws_bytes, vb_stream_t stream);
+
+/* One Eve parameter (optim.py:836-985); the caller passes only parameters that have a gradient. */
+typedef struct vb_eve_tensor {
+  float *param;
+  const float *grad;
+  float *exp_avg;
+  float *exp_avg_sq;
+  int64_t numel;
+  float step_size;  /* lr / (1 - beta1^step), step already incremented */
+  float bc2_rsqrt;  /* (1 - beta2^step)^-0.5 */
+  float norm_limit; /* target_rms * sqrt(numel) */
+  int32_t pad;
+} vb_eve_tensor;
+
+size_t vb_eve_workspace(const vb_eve_tensor *tensors, int n_tensors);
+/* One Eve step over a HOST table of tensors, two launches per VB_OPTIM_EVE_MAX_TENSORS tensors: per-chunk sum p^2,
+ * then per element m = beta1 m + (1 - beta1) g; v = beta2 v + (1 - beta2) g^2; when numel > 1 and ||p|| > norm_limit,
+ * p *= 1 - weight_decay (||p|| of the pre-update p); p += -step_size * m / (sqrt(v) * bc2_rsqrt + eps). */
+#define VB_OPTIM_EVE_MAX_TENSORS 480
+int vb_eve_step(const vb_eve_tensor *tensors, int n_tensors, float beta1, float beta2, float eps, float weight_decay,
+                void *workspace, size_t ws_bytes, vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * a13  AudioTokenizer.encode / .decode (valle/data/tokenizer.py:211-254) -> PyPI `encodec`

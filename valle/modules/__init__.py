@@ -1,2 +1,2 @@
 """valle/modules operator surface."""
-from . import activation, embedding, transformer  # noqa: F401
+from . import activation, embedding, optim, scheduler, transformer  # noqa: F401

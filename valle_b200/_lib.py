@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 VB_F32, VB_BF16 = 0, 1
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -70,6 +70,37 @@ class LayerGrads(C.Structure):
 class LayerWt(C.Structure):
     """vb_layer_wt: transposed matrices of one layer (storage dtype)"""
     _fields_ = [(n, vp) for n in ("in_proj_wt", "out_proj_wt", "lin1_wt", "lin2_wt")]
+
+
+class ScaledAdamTensor(C.Structure):
+    """vb_scaled_adam_tensor: one parameter of a ScaledAdam batch and its slot of the batch's stacked state"""
+    _fields_ = [("param", vp), ("delta", vp), ("exp_avg_sq", vp), ("param_rms", vp), ("scale_exp_avg_sq", vp),
+                ("scale_grads", vp), ("numel", C.c_int64), ("chunk0", C.c_int32), ("sg_stride", C.c_int32),
+                ("scalar", C.c_int32), ("pad", C.c_int32)]
+
+
+class ScaledAdamArgs(C.Structure):
+    """vb_scaled_adam_args: the host-known scalars of one ScaledAdam step of a parameter group"""
+    _fields_ = [(n, C.c_int32) for n in ("n_tensors", "n_chunks", "step", "zero_step", "init", "clip_mode",
+                                         "clip_period", "size_period")] + \
+               [(n, C.c_double) for n in ("clipping_scale", "lr", "scalar_lr_scale", "beta1", "beta2", "eps",
+                                          "param_min_rms", "param_max_rms", "scalar_max")]
+
+
+class ClipState(C.Structure):
+    """vb_clip_state: device-resident clipping state of a ScaledAdam parameter group (32 bytes)"""
+    _fields_ = [("threshold", C.c_double), ("scale", C.c_float), ("min_scale", C.c_float),
+                ("prev_min_scale", C.c_float), ("num_clipped", C.c_int32), ("prev_clipped", C.c_int32),
+                ("has_threshold", C.c_int32)]
+
+
+class EveTensor(C.Structure):
+    """vb_eve_tensor: one Eve parameter with a gradient, and its per-step bias corrections"""
+    _fields_ = [("param", vp), ("grad", vp), ("exp_avg", vp), ("exp_avg_sq", vp), ("numel", C.c_int64),
+                ("step_size", C.c_float), ("bc2_rsqrt", C.c_float), ("norm_limit", C.c_float), ("pad", C.c_int32)]
+
+
+OPTIM_CHUNK = 16384  # VB_OPTIM_CHUNK
 
 
 class VbError(RuntimeError):
@@ -140,6 +171,10 @@ PROTOTYPES = {
     "vb_permute3": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     "vb_gather_rows": (C.c_int, [vp, C.c_int64, vp, C.c_int64, C.c_int, vp, C.c_int64, vp]),
     "vb_cast_from_f32": (C.c_int, [vp, vp, C.c_int, C.c_int64, vp]),
+    "vb_scaled_adam_workspace": (C.c_size_t, [C.c_int, C.c_int]),
+    "vb_scaled_adam_step": (C.c_int, [vp, vp, c_i32p, C.POINTER(ScaledAdamArgs), vp, vp, vp, C.c_size_t, vp]),
+    "vb_eve_workspace": (C.c_size_t, [vp, C.c_int]),
+    "vb_eve_step": (C.c_int, [vp, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, vp, C.c_size_t, vp]),
 }
 
 
