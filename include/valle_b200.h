@@ -339,7 +339,7 @@ int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb
  * (no host reads; launch geometry depends only on B and cache_cap).  bf16 decoders with
  * vb_decoder_set_decode_fold + head->fold run the LayerNorm-folded chain (6 launches per layer; the
  * residual stream is assembled by the split-K projections themselves, the splits of a tile adding up in fixed order
- * inside a thread-block cluster; VB_DECODE_FOLD=0 selects the 8-launch chain).  Both are run-to-run deterministic. */
+ * inside a thread-block cluster); without either fold the 8-launch chain runs.  Both are run-to-run deterministic. */
 int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st, void *workspace,
                       size_t workspace_bytes, vb_stream_t stream);
 

@@ -39,15 +39,16 @@ def test_tcgen05_gemm_matches_fp32_reference(M, N, K, epi):
 
 def test_tcgen05_matches_simt_kernel_bitwise_inputs():
     """same bf16 operands through the CUDA-core kernel (VB_DISABLE_WGMMA is read per call)."""
-    import os
+    from valle_b200 import _lib as L
     from valle_b200 import ops
+    lib = L.load()
     g = torch.Generator().manual_seed(5)
     a = torch.randn(257, 1024, generator=g).bfloat16().to(DEV)
     w = (torch.randn(1024, 1024, generator=g) / 32).bfloat16().to(DEV)
     o1 = ops.linear(a, w, None, out_dtype=torch.float32)
-    os.environ["VB_DISABLE_WGMMA"] = "1"
+    L.check(lib.vb_tune_set(b"VB_DISABLE_WGMMA", 1))
     try:
         o2 = ops.linear(a, w, None, out_dtype=torch.float32)
     finally:
-        del os.environ["VB_DISABLE_WGMMA"]
+        L.check(lib.vb_tune_set(b"VB_DISABLE_WGMMA", 0))
     assert torch.allclose(o1, o2, atol=1e-3, rtol=1e-4), (o1 - o2).abs().max()

@@ -348,8 +348,9 @@ def test_folded_decode_chain_matches_the_unfolded_chain(name):
     projections carrying the rows' moments, residual stream assembled by the projections) against the chain with the
     separate residual + LayerNorm launches on the same weights: per-step logits within 2e-2 (both round to bf16 at
     different points), the same early greedy ids, and the folded chain is what the engine runs by default."""
-    from valle_b200 import _lib as L
-    lib = L.load()
+    from unittest import mock
+
+    from valle_b200.engine import ValleEngine
     g = load_golden(name)
     m = _model(g, torch.bfloat16)
     eng = m.engine()
@@ -362,14 +363,12 @@ def test_folded_decode_chain_matches_the_unfolded_chain(name):
     steps = {0, 1, 2, 7, 15}
     tr_f = {"steps": steps}
     out_f = eng.generate(texts, prompts, top_k=1, trace=tr_f, max_new_tokens=16)
-    L.check(lib.vb_tune_set(b"VB_DECODE_FOLD", 0))
-    try:
-        eng._bufs.clear()
-        tr_u = {"steps": steps}
-        out_u = eng.generate(texts, prompts, top_k=1, trace=tr_u, max_new_tokens=16)
-    finally:
-        L.check(lib.vb_tune_set(b"VB_DECODE_FOLD", 1))
-        eng._bufs.clear()
+    with mock.patch.dict(os.environ, {"VB_DECODE_FOLD": "0"}):   # read when the engine builds its weights
+        eng_u = ValleEngine(m, torch.bfloat16)
+    assert eng_u.ar_head_fold is None
+    eng_u.quiet = eng.quiet
+    tr_u = {"steps": steps}
+    out_u = eng_u.generate(texts, prompts, top_k=1, trace=tr_u, max_new_tokens=16)
     for s in sorted(steps):
         err = (tr_f["ar_logits"][s] - tr_u["ar_logits"][s]).abs().max().item()
         assert err < 2e-2, (s, err)

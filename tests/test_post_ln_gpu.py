@@ -189,11 +189,13 @@ def test_bf16_codes_identical_across_reruns_graphs_and_the_cuda_core_path():
     assert all(torch.equal(p, q) for p, q in zip(a, c))
     tr_tc, tr_simt = {"steps": "all"}, {"steps": "all"}
     eng.generate([x], [y], top_k=1, trace=tr_tc, forced=[a[0]])
-    os.environ["VB_DECODE_SIMT"] = "1"
+    from valle_b200 import _lib as L
+    lib = L.load()
+    L.check(lib.vb_tune_set(b"VB_DECODE_SIMT", 1))
     try:
         eng.generate([x], [y], top_k=1, trace=tr_simt, forced=[a[0]])
     finally:
-        del os.environ["VB_DECODE_SIMT"]
+        L.check(lib.vb_tune_set(b"VB_DECODE_SIMT", 0))
     err = max(float((tr_tc["ar_logits"][k] - tr_simt["ar_logits"][k]).abs().max()) for k in tr_tc["ar_logits"])
     assert err < AR_TOL, err
 

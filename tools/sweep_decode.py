@@ -2,6 +2,9 @@
 re-captured per configuration; prints the AR-phase time of a full decode per configuration.
 
     python tools/sweep_decode.py B FRAMES "K1=v,K2=v" "K1=v" ...      ("" = defaults)
+
+The decode chain is the engine's choice, made once when it builds the weights: VB_DECODE_FOLD=0 in the environment
+of the run sweeps the unfolded chain.
 """
 import json
 import os
@@ -31,7 +34,7 @@ for rep in range(int(os.environ.get("SWEEP_REPS", "2"))):
             lib.vb_tune_set(k.encode(), touched[k])
         kv = dict(x.split("=") for x in c.split(",") if x)
         for k, v in kv.items():
-            touched.setdefault(k, {"VB_KV_PREFETCH_L2_PCT": 60, "VB_DECODE_FOLD": 1}.get(k, 0))
+            touched.setdefault(k, {"VB_KV_PREFETCH_L2_PCT": 60}.get(k, 0))
             lib.vb_tune_set(k.encode(), int(v))
         eng._bufs.clear()
         eng.generate(texts, prompts, top_k=1, max_new_tokens=min(40, frames), return_device=True)   # capture

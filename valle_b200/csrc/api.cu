@@ -500,56 +500,70 @@ StepWs carve_step_ws(Carve &c, const vb_decoder_desc &D, int B, int cache_cap) {
 }
 // tensor-core decode path: bf16 storage, up to 64 rows (one UMMA N tile)
 bool use_tc_decode(const vb_decoder_desc &D, int B) {
-  return D.wdtype == VB_BF16 && B >= 1 && B <= 64 && getenv("VB_DECODE_SIMT") == nullptr;
+  return D.wdtype == VB_BF16 && B >= 1 && B <= 64 && tune("VB_DECODE_SIMT", 0) == 0;
+}
+// the LayerNorm-folded chain: the decoder's norms (vb_decoder_set_decode_fold) and the head's final norm are folded
+bool use_fold(const vb_decoder *dec, const vb_ar_head *head) { return dec->fold_qkv && head->fold.wf; }
+bool use_pdl() { return tune("VB_NO_PDL", 0) == 0; }
+
+// split-K counts of the four decode projections.  Split-K wide enough to fill the SMs (0) is not the optimum for the
+// projections whose partial sums a reduce kernel has to add up again, hence fixed counts (not re-tuned on H100;
+// VB_SPLITS_* override them).  The folded chain has no reduce kernel that pays for more slabs, and with <= 6 k-blocks
+// per CTA its weight ring never wraps.
+struct DecodeSplits {
+  int qkv, out, ffn1, ffn2;
+};
+DecodeSplits decode_splits(const vb_decoder_desc &D, bool fold) {
+  const int kb = D.d_model / 128, fb = D.d_ff / 128;
+  auto upto = [](int n, int cap) { return std::max(1, std::min(cap, n)); };
+  auto knob = [](const char *name, int dflt) {
+    const int v = tune(name, 0);
+    return v > 0 ? v : dflt;
+  };
+  return {knob("VB_SPLITS_QKV", upto(kb, 5)), knob("VB_SPLITS_OUT", fold ? 8 : 0),
+          knob("VB_SPLITS_FFN1", upto(kb, fold ? 4 : 2)), knob("VB_SPLITS_FFN2", upto(fb, fold ? 8 : 9))};
+}
+
+// layer l's caches and the rows' lengths: where the QKV projection leaves q and appends k / v, what the attention
+// reads and what the KV prefetch pulls into L2
+QkvScatter layer_kv(const vb_decoder_desc &D, const vb_ar_state *st, int l, float *q) {
+  const size_t off = (size_t)l * st->cache_layer_stride * elem_size(D.wdtype);
+  return QkvScatter{D.d_model, D.d_model / D.n_head, q, (char *)st->kcache + off, (char *)st->vcache + off,
+                    st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished};
+}
+
+// final LayerNorm (adding the pending partials of the last FFN2) + ar_predict_layer + sampler on the tensor-core
+// path.  fold: the final norm is folded into ar_predict_layer, the projection reads the fp32 rows and the sampler
+// applies the moments.  A stack without a final norm (post-LN) feeds the head the bf16 rows of x: w.xn16 as the
+// decode chain's last post-norm left it (xn_ready), else a cast of x.
+int tc_head(const vb_decoder_desc &D, const vb_ar_head *head, float *x, vb_ar_state *st, const StepWs &w, bool fold,
+            const SplitK &pend, cudaStream_t s, bool xn_ready = false) {
+  const int d = D.d_model, B = st->B;
+  const int ldl = (head->n_vocab + 3) & ~3;
+  const bool pdl = use_pdl();
+  SplitK logits;
+  if (fold) {
+    VB_TRY(launch_gemm_decode_x(x, B, d, head->fold, head->n_vocab, d, 0, (float *)w.gemm_ws, w.gemm_ws_bytes, w.stats,
+                                &logits, nullptr, pdl, s));
+    return launch_ar_sample(st->logits, ldl, logits, head, st, d, nullptr, head->greedy ? 0 : 1, pdl, s);
+  }
+  if (D.final_norm_w)
+    VB_TRY(launch_ln_reduce(x, d, B, d, pend, D.final_norm_w, D.final_norm_b, 1e-5f, w.xn16, pdl, s));
+  else if (!xn_ready)
+    VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));
+  VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)head->predict_w, head->n_vocab, d, 0, nullptr, DG_F32,
+                            st->logits, nullptr, ldl, nullptr, (float *)w.gemm_ws, w.gemm_ws_bytes, &logits, nullptr,
+                            pdl, s));
+  // logits only (host-side sampling follows) and split: just reduce the partials
+  if (head->greedy || logits.part)
+    VB_TRY(launch_ar_sample(st->logits, ldl, logits, head, st, d, nullptr, head->greedy ? 0 : 1, pdl, s));
+  return VB_OK;
 }
 }  // namespace
 
 VB_API size_t vb_ar_step_workspace(const vb_decoder_desc *desc, int B, int cache_cap) {
   return carved_bytes(carve_step_ws, *desc, B, cache_cap);
 }
-
-namespace {
-struct Pending {  // split-K partials of a projection whose bias/residual the next ln_reduce applies
-  const float *part = nullptr;
-  const float *bias = nullptr;
-  int splits = 0, ldp = 0;
-};
-bool use_pdl() { return getenv("VB_NO_PDL") == nullptr; }
-
-// final LayerNorm + ar_predict_layer + sampler on the tensor-core path.  A stack without a final norm (post-LN) feeds
-// the head the bf16 rows of x: w.xn16 as the decode chain's last post-norm left it (xn_ready), else a cast of x.
-int tc_head(vb_decoder *dec, const vb_ar_head *head, float *x, vb_ar_state *st, const StepWs &w, const Pending &pend,
-            cudaStream_t s, bool xn_ready = false) {
-  const vb_decoder_desc &D = dec->desc;
-  const int d = D.d_model, B = st->B;
-  const int ldl = (head->n_vocab + 3) & ~3;
-  const bool pdl = use_pdl();
-  if (head->fold.wf && pend.part == nullptr && tune("VB_DECODE_FOLD", 1) != 0) {
-    // final LayerNorm folded into ar_predict_layer: the projection reads the fp32 rows, the sampler applies the moments
-    int sp = 1, ldp = 0, cp = 1;
-    VB_TRY(launch_gemm_decode_x(x, B, d, (const bf16 *)head->fold.wf, head->n_vocab, d, 0, (float *)w.gemm_ws,
-                                w.gemm_ws_bytes, w.stats, &sp, &ldp, &cp, nullptr, pdl, s));
-    const LnFoldStats fs{w.stats, head->fold.c, sp, d, 1e-5f, cp};
-    return launch_ar_sample(st->logits, ldl, (const float *)w.gemm_ws, sp, ldp, head, st, d, nullptr,
-                            head->greedy ? 0 : 1, pdl, s, &fs);
-  }
-  if (D.final_norm_w)
-    VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, D.final_norm_w, D.final_norm_b,
-                            1e-5f, w.xn16, pdl, s));
-  else if (!xn_ready)
-    VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));
-  int sp = 1, ldp = 0;
-  VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)head->predict_w, head->n_vocab, d, 0, nullptr, DG_F32,
-                            st->logits, nullptr, ldl, nullptr, (float *)w.gemm_ws, w.gemm_ws_bytes, &sp, &ldp, nullptr, pdl,
-                            s));
-  if (head->greedy)
-    VB_TRY(launch_ar_sample(st->logits, ldl, sp > 1 ? (const float *)w.gemm_ws : nullptr, sp, ldp, head, st, d, nullptr,
-                            0, pdl, s));
-  else if (sp > 1)  // logits only (host-side sampling follows): just reduce the partials
-    VB_TRY(launch_ar_sample(st->logits, ldl, (const float *)w.gemm_ws, sp, ldp, head, st, d, nullptr, 1, pdl, s));
-  return VB_OK;
-}
-}  // namespace
 
 VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
                            void *workspace, size_t workspace_bytes, vb_stream_t stream) {
@@ -565,12 +579,12 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
                  "vb_ar_head_step: workspace too small");
     Carve c(workspace);
     const StepWs w = carve_step_ws(c, D, st->B, st->cache_cap);
-    return tc_head(dec, head, const_cast<float *>(h), st, w, Pending{}, s);
+    return tc_head(D, head, const_cast<float *>(h), st, w, use_fold(dec, head), SplitK{}, s);
   }
   LnParams ln{D.final_norm_w, D.final_norm_b, nullptr, 1e-5f};
   VB_TRY(launch_gemv(h, d, st->B, head->predict_w, D.wdtype, nullptr, head->n_vocab, d, st->logits, ldl,
                      D.final_norm_w ? &ln : nullptr, 0, nullptr, s));
-  if (head->greedy) VB_TRY(launch_ar_sample(st->logits, ldl, nullptr, 0, 0, head, st, d, nullptr, 0, false, s));
+  if (head->greedy) VB_TRY(launch_ar_sample(st->logits, ldl, SplitK{}, head, st, d, nullptr, 0, false, s));
   return VB_OK;
 }
 
@@ -584,7 +598,7 @@ VB_API int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int6
                              vb_stream_t stream) {
   VB_CHECK_ARG(head && st && sampled, "vb_ar_push_tokens: null argument");
   const int ldl = (head->n_vocab + 3) & ~3;
-  return launch_ar_sample(st->logits, ldl, nullptr, 0, 0, head, st, d, sampled, 0, false, (cudaStream_t)stream);
+  return launch_ar_sample(st->logits, ldl, SplitK{}, head, st, d, sampled, 0, false, (cudaStream_t)stream);
 }
 
 VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st, void *workspace,
@@ -604,12 +618,21 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   float *x = st->x_cur;
   const bool post = !D.norm_first;
   if (use_tc_decode(D, B)) {
-    // bf16 tensor-core path: LayerNorm(+pending residual) -> swap-AB split-K wgmma projections whose
-    // partial sums are consumed by the next kernel in the chain (7 launches per layer, PDL-chained)
+    // bf16 tensor-core path: swap-AB split-K wgmma projections whose partial sums are consumed by the next kernel in
+    // the chain (PDL-chained).  Three chains share the layer loop:
+    //   folded (6 launches per layer): QKV'(x) -> attention (+ moments, KV append) -> out-proj (+= x) -> FFN1'(x) ->
+    //     ReLU reduce (+ moments) -> FFN2 (+= x).  The projections that consume the residual stream x read its fp32
+    //     rows and carry the LayerNorm in their weights (vb_ln_fold), the rows' moments travel with the partial sums;
+    //     the projections that produce x assemble it in place (the splits of a tile as a cluster, summed over DSMEM
+    //     in fixed order).
+    //   unfolded pre-LN (8): ln_reduce(+ the previous FFN2's partials, norm1) -> QKV -> attention -> out-proj ->
+    //     ln_reduce(norm2) -> FFN1 -> ReLU reduce -> FFN2.
+    //   post-LN (8; transformer.py:303-308, one cast of x ahead of layer 0 and none of the final norm): QKV ->
+    //     attention -> out-proj -> ln_reduce<post>(norm1) -> FFN1 -> ReLU reduce -> FFN2 -> ln_reduce<post>(norm2),
+    //     each post-norm writing the normalised rows into x as well.
     const bool pdl = use_pdl();
-    // Split-K wide enough to fill the SMs is not the optimum for the projections whose partial sums a reduce kernel
-    // has to add up again, hence the fixed split counts below (not re-tuned on H100; VB_SPLITS_* override them).
-    const bool fold_on = dec->fold_qkv && dec->fold_ffn1 && head->fold.wf && tune("VB_DECODE_FOLD", 1) != 0;
+    const bool fold = use_fold(dec, head);
+    const DecodeSplits sp = decode_splits(D, fold);
     // KV prefetch budget: a share of the L2 that one layer's weights, streaming through it at the same time, leave
     // free (VB_KV_PREFETCH_L2_PCT, DESIGN section 7), spread evenly over the B x H streams as their leading rows.
     // Lines evicted before the attention reads them would cost their HBM bytes twice.
@@ -617,124 +640,66 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     const int64_t pf_budget = B >= 16 ? std::max<int64_t>(0, l2_bytes() - layer_w_bytes) *
                                             tune("VB_KV_PREFETCH_L2_PCT", 60) / 100 : 0;
     const int pf_rows = (int)std::min<int64_t>(st->cache_cap, pf_budget / (2 * (int64_t)B * D.n_head * hd * ts));
-    const int qkv_env = tune("VB_SPLITS_QKV", 0);
-    const int out_splits = tune("VB_SPLITS_OUT", 0);   // 0 = fill the SMs
-    const int ffn1_env = tune("VB_SPLITS_FFN1", 0);
-    const int ffn2_env = tune("VB_SPLITS_FFN2", 0);
-    const int qkv_splits = qkv_env > 0 ? qkv_env : std::max(1, std::min(5, d / 128));
-    const int ffn2_splits = ffn2_env > 0 ? ffn2_env : std::max(1, std::min(9, dff / 128));
-    // folded chain: no reduce kernel pays for more slabs, and with <= 6 k-blocks per CTA the weight ring never wraps
-    const int ffn2_fold = ffn2_env > 0 ? ffn2_env : std::max(1, std::min(8, dff / 128));
-    const int ffn1_splits = ffn1_env > 0 ? ffn1_env : std::max(1, std::min(2, d / 128));
     float *P = (float *)w.gemm_ws;
-    Pending pend;
     // the four projections of the chain each prefetch a quarter of the first pf_rows rows of the KV streams that the
     // NEXT attention launch will read (QKV: this layer's, the other three: the following layer's)
     auto kv_slice = [&](int layer, int quarter) {
       KvPrefetch pf{};
       if (pf_rows <= 0) return pf;
-      layer %= D.n_layer;
-      pf.kbase = (char *)st->kcache + (size_t)layer * st->cache_layer_stride * ts;
-      pf.vbase = (char *)st->vcache + (size_t)layer * st->cache_layer_stride * ts;
-      pf.seq_stride_bytes = (int64_t)st->cache_seq_stride * (int64_t)ts;
-      pf.B = B; pf.H = D.n_head; pf.cap = st->cache_cap; pf.row_bytes = (int)(hd * ts);
-      pf.text_len = st->text_len; pf.prompt_len = st->prompt_len; pf.n_gen = st->n_gen;
+      const QkvScatter kv = layer_kv(D, st, layer % D.n_layer, w.q);
+      pf.kbase = kv.kcache; pf.vbase = kv.vcache;
+      pf.seq_stride_bytes = kv.cache_seq_stride * (int64_t)ts;
+      pf.B = B; pf.H = D.n_head; pf.cap = kv.cache_cap; pf.row_bytes = (int)(hd * ts);
+      pf.text_len = kv.text_len; pf.prompt_len = kv.prompt_len; pf.n_gen = kv.n_gen;
       pf.row_lo = pf_rows * quarter / 4; pf.row_hi = pf_rows * (quarter + 1) / 4;
       return pf;
     };
-    if (fold_on) {
-      // Folded chain, 6 launches per layer: the residual stream x is assembled in place by the split-K projections that
-      // produce it (the splits of a tile as a cluster, summed over DSMEM in fixed order), the projections that consume it read the fp32 rows and carry
-      // the LayerNorm in their weights (vb_ln_fold), the rows' moments travel with the partial sums:
-      //   QKV'(x) -> attention (+ moments, KV append) -> out-proj (+= x) -> FFN1'(x) -> ReLU reduce (+ moments) -> FFN2 (+= x)
-      const int qkv_f = qkv_env > 0 ? qkv_env : std::max(1, std::min(5, d / 128));
-      const int ffn1_f = ffn1_env > 0 ? ffn1_env : std::max(1, std::min(4, d / 128));
-      const int out_f = out_splits > 0 ? out_splits : 8;
-      for (int l = 0; l < D.n_layer; ++l) {
-        const vb_layer_params &L = dec->layers[l];
-        const vb_ln_fold &Fq = dec->fold_qkv[l], &Ff = dec->fold_ffn1[l];
-        const KvPrefetch pf_qkv = kv_slice(l, 3), pf_out = kv_slice(l + 1, 0), pf_f1 = kv_slice(l + 1, 1),
-                         pf_f2 = kv_slice(l + 1, 2);
-        void *kc = (char *)st->kcache + (size_t)l * st->cache_layer_stride * ts;
-        void *vc = (char *)st->vcache + (size_t)l * st->cache_layer_stride * ts;
-        int s1 = 1, ldp1 = 0, cp1 = 1;
-        VB_TRY(launch_gemm_decode_x(x, B, d, (const bf16 *)Fq.wf, 3 * d, d, qkv_f, P, w.gemm_ws_bytes, w.stats, &s1, &ldp1,
-                                    &cp1, &pf_qkv, pdl, s));
-        const LnFoldStats fq{w.stats, Fq.c, s1, d, 1e-5f, cp1};
-        VB_TRY(launch_attn_decode(w.q, P, s1, ldp1, Fq.dvec, B, D.n_head, hd, kc, vc, dt, st->cache_seq_stride,
-                                  st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished, w.att, w.att16,
-                                  w.attn_ws, pdl, s, &fq));
-        VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, out_f, L.out_proj_b, DG_RESIDUAL, x,
-                                  nullptr, d, nullptr, nullptr, 0, nullptr, nullptr, &pf_out, pdl, s, true));
-        int sf = 1, ldpf = 0, cpf = 1;
-        VB_TRY(launch_gemm_decode_x(x, B, d, (const bf16 *)Ff.wf, dff, d, ffn1_f, P, w.gemm_ws_bytes, w.stats, &sf, &ldpf,
-                                    &cpf, &pf_f1, pdl, s));
-        const LnFoldStats ff{w.stats, Ff.c, sf, d, 1e-5f, cpf};
-        VB_TRY(launch_relu_reduce(P, sf, ldpf, Ff.dvec, B, dff, w.hb16, dff, pdl, s, &ff));
-        VB_TRY(launch_gemm_decode(w.hb16, B, dff, (const bf16 *)L.lin2_w, d, dff, ffn2_fold, L.lin2_b, DG_RESIDUAL, x,
-                                  nullptr, d, nullptr, nullptr, 0, nullptr, nullptr, &pf_f2, pdl, s, true));
-      }
-      return tc_head(dec, head, x, st, w, Pending{}, s);
-    }
-    // Unfolded chain, 8 launches per layer.  Pre-LN: ln_reduce(+ the previous FFN2's partials, norm1) -> QKV ->
-    // attention -> out-proj -> ln_reduce(norm2) -> FFN1 -> ReLU reduce -> FFN2.  Post-LN (transformer.py:303-308, one cast
-    // of x ahead of layer 0 and none of the final norm): QKV -> attention -> out-proj -> ln_reduce<post>(norm1) -> FFN1 ->
-    // ReLU reduce -> FFN2 -> ln_reduce<post>(norm2), each post-norm writing the normalised rows into x as well.
+    SplitK pend;  // the last FFN2's partial sums, for the next LayerNorm to add
     if (post) VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));
     for (int l = 0; l < D.n_layer; ++l) {
       const vb_layer_params &L = dec->layers[l];
+      const QkvScatter kv = layer_kv(D, st, l, w.q);
       const KvPrefetch pf_qkv = kv_slice(l, 3), pf_out = kv_slice(l + 1, 0), pf_f1 = kv_slice(l + 1, 1),
                        pf_f2 = kv_slice(l + 1, 2);
-      void *kc = (char *)st->kcache + (size_t)l * st->cache_layer_stride * ts;
-      void *vc = (char *)st->vcache + (size_t)l * st->cache_layer_stride * ts;
-      QkvScatter sc{d, hd, w.q, kc, vc, st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen,
-                    st->finished};
-      if (!post)
-        VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, L.norm1_w, L.norm1_b, 1e-5f,
-                                w.xn16, pdl, s));
-      int s1 = 1, ldp1 = 0;
-      VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.in_proj_w, 3 * d, d, qkv_splits, L.in_proj_b, DG_QKV, nullptr,
-                                nullptr, d, &sc, P, w.gemm_ws_bytes, &s1, &ldp1, &pf_qkv, pdl, s));
-      VB_TRY(launch_attn_decode(w.q, s1 > 1 ? P : nullptr, s1, ldp1, L.in_proj_b, B, D.n_head, hd, kc, vc, dt,
-                                st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished,
-                                w.att, w.att16, w.attn_ws, pdl, s));
-      int s2 = 1, ldp2 = 0;
-      VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, out_splits, L.out_proj_b, DG_RESIDUAL, x,
-                                nullptr, d, nullptr, P, w.gemm_ws_bytes, &s2, &ldp2, &pf_out, pdl, s));
-      VB_TRY(launch_ln_reduce(x, d, B, d, s2 > 1 ? P : nullptr, s2, ldp2, L.out_proj_b, post ? L.norm1_w : L.norm2_w,
-                              post ? L.norm1_b : L.norm2_b, 1e-5f, w.xn16, pdl, s, post));
-      int sf = 1, ldpf = 0;
-      VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.lin1_w, dff, d, ffn1_splits, L.lin1_b, DG_RELU_BF16, nullptr,
-                                w.hb16, dff, nullptr, P, w.gemm_ws_bytes, &sf, &ldpf, &pf_f1, pdl, s));
-      if (sf > 1) VB_TRY(launch_relu_reduce(P, sf, ldpf, L.lin1_b, B, dff, w.hb16, dff, pdl, s));
-      int s3 = 1, ldp3 = 0;
-      VB_TRY(launch_gemm_decode(w.hb16, B, dff, (const bf16 *)L.lin2_w, d, dff, ffn2_splits, L.lin2_b, DG_RESIDUAL, x, nullptr,
-                                d, nullptr, P, w.gemm_ws_bytes, &s3, &ldp3, &pf_f2, pdl, s));
-      pend = Pending{};
-      if (s3 > 1) {
-        pend.part = P; pend.bias = L.lin2_b; pend.splits = s3; pend.ldp = ldp3;
+      SplitK qkv, out, ffn1;
+      if (fold) {
+        VB_TRY(launch_gemm_decode_x(x, B, d, dec->fold_qkv[l], 3 * d, d, sp.qkv, P, w.gemm_ws_bytes, w.stats, &qkv,
+                                    &pf_qkv, pdl, s));
+      } else {
+        if (!post) VB_TRY(launch_ln_reduce(x, d, B, d, pend, L.norm1_w, L.norm1_b, 1e-5f, w.xn16, pdl, s));
+        VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.in_proj_w, 3 * d, d, sp.qkv, L.in_proj_b, DG_QKV,
+                                  nullptr, nullptr, d, &kv, P, w.gemm_ws_bytes, &qkv, &pf_qkv, pdl, s));
       }
+      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, dt, w.att, w.att16, w.attn_ws, pdl, s));
+      VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, sp.out, L.out_proj_b, DG_RESIDUAL, x,
+                                nullptr, d, nullptr, P, w.gemm_ws_bytes, &out, &pf_out, pdl, s, fold));
+      if (fold) {
+        VB_TRY(launch_gemm_decode_x(x, B, d, dec->fold_ffn1[l], dff, d, sp.ffn1, P, w.gemm_ws_bytes, w.stats, &ffn1,
+                                    &pf_f1, pdl, s));
+      } else {
+        VB_TRY(launch_ln_reduce(x, d, B, d, out, post ? L.norm1_w : L.norm2_w, post ? L.norm1_b : L.norm2_b, 1e-5f,
+                                w.xn16, pdl, s, post));
+        VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.lin1_w, dff, d, sp.ffn1, L.lin1_b, DG_RELU_BF16,
+                                  nullptr, w.hb16, dff, nullptr, P, w.gemm_ws_bytes, &ffn1, &pf_f1, pdl, s));
+      }
+      if (ffn1.part) VB_TRY(launch_relu_reduce(ffn1, B, dff, w.hb16, dff, pdl, s));
+      VB_TRY(launch_gemm_decode(w.hb16, B, dff, (const bf16 *)L.lin2_w, d, dff, sp.ffn2, L.lin2_b, DG_RESIDUAL, x,
+                                nullptr, d, nullptr, P, w.gemm_ws_bytes, &pend, &pf_f2, pdl, s, fold));
       if (post) {
-        VB_TRY(launch_ln_reduce(x, d, B, d, pend.part, pend.splits, pend.ldp, pend.bias, L.norm2_w, L.norm2_b, 1e-5f,
-                                w.xn16, pdl, s, true));
-        pend = Pending{};
+        VB_TRY(launch_ln_reduce(x, d, B, d, pend, L.norm2_w, L.norm2_b, 1e-5f, w.xn16, pdl, s, true));
+        pend = SplitK{};
       }
     }
-    return tc_head(dec, head, x, st, w, pend, s, post);
+    return tc_head(D, head, x, st, w, fold, pend, s, post);
   }
   // CUDA-core chain: pre-LN GEMVs normalise their input rows on the fly; post-LN GEMVs read x as it is, and each
   // residual GEMV is followed by the in-place post-norm of x's B rows
   for (int l = 0; l < D.n_layer; ++l) {
     const vb_layer_params &P = dec->layers[l];
-    void *kc = (char *)st->kcache + (size_t)l * st->cache_layer_stride * ts;
-    void *vc = (char *)st->vcache + (size_t)l * st->cache_layer_stride * ts;
-    QkvScatter sc{d, hd, w.q, kc, vc, st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen,
-                    st->finished};
+    const QkvScatter kv = layer_kv(D, st, l, w.q);
     LnParams ln1{P.norm1_w, P.norm1_b, nullptr, 1e-5f};
-    VB_TRY(launch_gemv(x, d, B, P.in_proj_w, dt, P.in_proj_b, 3 * d, d, nullptr, 0, post ? nullptr : &ln1, 3, &sc, s));
-    VB_TRY(launch_attn_decode(w.q, nullptr, 0, 0, nullptr, B, D.n_head, hd, kc, vc, dt, st->cache_seq_stride,
-                              st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished, w.att, nullptr,
-                              w.attn_ws, false, s));
+    VB_TRY(launch_gemv(x, d, B, P.in_proj_w, dt, P.in_proj_b, 3 * d, d, nullptr, 0, post ? nullptr : &ln1, 3, &kv, s));
+    VB_TRY(launch_attn_decode(kv, SplitK{}, B, D.n_head, dt, w.att, nullptr, w.attn_ws, false, s));
     VB_TRY(launch_gemv(w.att, d, B, P.out_proj_w, dt, P.out_proj_b, d, d, x, d, nullptr, 2, nullptr, s));
     if (post) VB_TRY(launch_post_norm(x, B, d, P.norm1_w, P.norm1_b, nullptr, 1e-5f, nullptr, VB_F32, s));
     LnParams ln2{P.norm2_w, P.norm2_b, nullptr, 1e-5f};

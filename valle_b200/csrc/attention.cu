@@ -204,7 +204,7 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k<<<grid, 256, smem, s>>>((const float *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, (float *)out,
                               (float *)kcache, (float *)vcache, cache_seq_stride, cache_cap, dense_mask, dense_ld, dc);
-  } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && getenv("VB_ATTN_SIMT") == nullptr) {
+  } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && tune("VB_ATTN_SIMT", 0) == 0) {
     return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
                                   mask_mode, (bf16 *)out, (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, s);
   } else if (dtype == VB_BF16) {
@@ -700,28 +700,25 @@ size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap) {
   return (size_t)B * n_head * ns * (head_dim + 2) * sizeof(float) + 256;
 }
 
-int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, int qkv_ldp, const float *qkv_bias,
-                       int B, int n_head, int head_dim, void *kcache, void *vcache, int dtype,
-                       int64_t cache_seq_stride, int cache_cap, const int32_t *text_len, const int32_t *prompt_len,
-                       const int32_t *n_gen, const int32_t *finished, float *out, void *out16, void *workspace,
-                       bool pdl, cudaStream_t s, const LnFoldStats *fold) {
-  VB_CHECK_ARG(head_dim == HD, "attn_decode: head_dim=%d, only 64 is built", head_dim);
+int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
+                       void *workspace, bool pdl, cudaStream_t s) {
+  VB_CHECK_ARG(kv.head_dim == HD, "attn_decode: head_dim=%d, only 64 is built", kv.head_dim);
+  const int cache_cap = kv.cache_cap;
   const int ns = decode_nsplit(B, n_head, cache_cap);
   VB_CHECK_ARG((cache_cap + ns - 1) / ns + 16 <= kDecMaxChunk, "attn_decode: cache_cap %d too large", cache_cap);
   float *part_o = (float *)workspace;
   float *part_ml = part_o + (size_t)B * n_head * ns * HD;
-  QkvPartials qp{qkv_part, qkv_bias, qkv_splits, qkv_ldp, LnFoldStats{}};
-  if (fold) qp.fold = *fold;
+  const QkvPartials qp{qkv.part, qkv.bias, qkv.splits, qkv.ldp, qkv.fold};
   dim3 grid(n_head, B, ns);
-  if (dtype == VB_F32 || getenv("VB_ATTN_DECODE_1PASS") != nullptr) {  // fp32 parity path / single-pass variant
+  if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
     if (dtype == VB_F32)
-      VB_CUDA(launch_kernel(attn_decode_kernel<float>, grid, dim3(128), 0, s, pdl, q, qp, n_head, (float *)kcache,
-                            (float *)vcache, cache_seq_stride, cache_cap, text_len, prompt_len, n_gen, finished, out,
-                            (bf16 *)out16, part_o, part_ml, ns));
+      VB_CUDA(launch_kernel(attn_decode_kernel<float>, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qp, n_head,
+                            (float *)kv.kcache, (float *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
+                            kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns));
     else
-      VB_CUDA(launch_kernel(attn_decode_kernel<bf16>, grid, dim3(128), 0, s, pdl, q, qp, n_head, (bf16 *)kcache,
-                            (bf16 *)vcache, cache_seq_stride, cache_cap, text_len, prompt_len, n_gen, finished, out,
-                            (bf16 *)out16, part_o, part_ml, ns));
+      VB_CUDA(launch_kernel(attn_decode_kernel<bf16>, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qp, n_head,
+                            (bf16 *)kv.kcache, (bf16 *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
+                            kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns));
   } else {
     // score buffer: the chunk of one split, rounded as the kernel rounds it (+16), in 1 KB steps
     const size_t sc_bytes = align_up((size_t)((cache_cap + ns - 1) / ns + 32) * sizeof(float), 1024);
@@ -743,9 +740,9 @@ int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, in
         VB_CUDA(cudaFuncSetAttribute(attn_decode_2phase_pf_kernel<4>, cudaFuncAttributePreferredSharedMemoryCarveout, want));
       carve_set[dev & 63] = carve;
     }
-    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<4>, grid, dim3(128), sc_bytes, s, pdl, q, qp, n_head,
-                          (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, text_len, prompt_len, n_gen,
-                          finished, out, (bf16 *)out16, part_o, part_ml, ns));
+    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<4>, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q, qp,
+                          n_head, (bf16 *)kv.kcache, (bf16 *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
+                          kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns));
   }
   count_launch();
   if (ns > 1) {

@@ -150,13 +150,10 @@ relu_reduce_kernel(const float *__restrict__ partials, int splits, int ldp, cons
   *reinterpret_cast<uint2 *>(out16 + (int64_t)b * ldo + c) = pk;
 }
 
-int launch_relu_reduce(const float *partials, int splits, int ldp, const float *bias, int B, int N, bf16 *out16,
-                       int64_t ldo, bool pdl, cudaStream_t s, const LnFoldStats *fold) {
+int launch_relu_reduce(const SplitK &in, int B, int N, bf16 *out16, int64_t ldo, bool pdl, cudaStream_t s) {
   VB_CHECK_ARG(N % 4 == 0 && ldo % 4 == 0, "relu_reduce: N %% 4 != 0");
-  LnFoldStats f{};
-  if (fold) f = *fold;
-  VB_CUDA(launch_kernel(relu_reduce_kernel, dim3((N / 4 + 255) / 256, B), dim3(256), 0, s, pdl, partials, splits, ldp,
-                        bias, N, out16, ldo, f));
+  VB_CUDA(launch_kernel(relu_reduce_kernel, dim3((N / 4 + 255) / 256, B), dim3(256), 0, s, pdl, in.part, in.splits,
+                        in.ldp, in.bias, N, out16, ldo, in.fold));
   count_launch();
   return VB_OK;
 }
@@ -181,11 +178,10 @@ static int launch_ln_reduce_t(float *x, int64_t ldx, int B, int d, const float *
   return VB_OK;
 }
 
-int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const float *partials, int splits, int ldp,
-                     const float *bias, const float *gamma, const float *beta, float eps, bf16 *out16,
-                     bool pdl, cudaStream_t s, bool post) {
-  return post ? launch_ln_reduce_t<true>(x, ldx, B, d, partials, splits, ldp, bias, gamma, beta, eps, out16, pdl, s)
-              : launch_ln_reduce_t<false>(x, ldx, B, d, partials, splits, ldp, bias, gamma, beta, eps, out16, pdl, s);
+int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const SplitK &in, const float *gamma, const float *beta,
+                     float eps, bf16 *out16, bool pdl, cudaStream_t s, bool post) {
+  const auto launch = post ? launch_ln_reduce_t<true> : launch_ln_reduce_t<false>;
+  return launch(x, ldx, B, d, in.part, in.splits, in.ldp, in.bias, gamma, beta, eps, out16, pdl, s);
 }
 
 }  // namespace vb

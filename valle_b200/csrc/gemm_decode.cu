@@ -415,7 +415,7 @@ static int pick_splits(int tiles, int num_kb) {
 
 int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, int N, int K, int force_splits,
                        const float *bias, int mode, float *out_f32, bf16 *out_bf16, int64_t ld_out,
-                       const QkvScatter *qkv, float *partials, size_t partial_bytes, int *out_splits, int *out_ldp,
+                       const QkvScatter *qkv, float *partials, size_t partial_bytes, SplitK *out,
                        const KvPrefetch *pf, bool pdl, cudaStream_t s, bool red_add) {
   VB_CHECK_ARG(B >= 1 && B <= dg::TN, "gemm_decode: B=%d not in [1,64]", B);
   VB_CHECK_ARG(!red_add || mode == DG_RESIDUAL, "gemm_decode: red_add needs the residual epilogue");
@@ -429,8 +429,9 @@ int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, in
   if (splits > 1 && !red_add)
     VB_CHECK_ARG(partials && partial_bytes >= (size_t)splits * dg::TN * ldp * sizeof(float),
                  "gemm_decode: partial buffer too small");
-  if (out_splits) *out_splits = red_add ? 1 : splits;  // nothing left for a consumer to add up
-  if (out_ldp) *out_ldp = ldp;
+  // a residual update adds its splits up in the cluster: nothing left for a consumer, and the partials stay unused
+  if (red_add) partials = nullptr;
+  *out = SplitK{splits > 1 ? partials : nullptr, red_add ? 1 : splits, ldp, bias};
   CUtensorMap tw, tx;
   VB_TRY(tc::make_tmap(&tw, W, N, K, K, dg::TM));
   VB_TRY(tc::make_tmap(&tx, act, B, K, ld_act, dg::TN));
@@ -461,9 +462,9 @@ int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, in
 }
 
 // projection of the fp32 rows x[B, K] by LayerNorm-folded weights: fp32 partial tiles + the rows' moments per split
-int launch_gemm_decode_x(const float *x, int B, int64_t ldx, const bf16 *Wf, int N, int K, int force_splits,
-                         float *partials, size_t partial_bytes, float *stats, int *out_splits, int *out_ldp,
-                         int *out_copies, const KvPrefetch *pf, bool pdl, cudaStream_t s) {
+int launch_gemm_decode_x(const float *x, int B, int64_t ldx, const vb_ln_fold &F, int N, int K, int force_splits,
+                         float *partials, size_t partial_bytes, float *stats, SplitK *out, const KvPrefetch *pf,
+                         bool pdl, cudaStream_t s) {
   VB_CHECK_ARG(B >= 1 && B <= dg::TN, "gemm_decode_x: B=%d not in [1,64]", B);
   VB_CHECK_ARG(K % tc::BK == 0 && ldx % 4 == 0, "gemm_decode_x: K %% 64 != 0 or unaligned rows");
   const int tiles = (N + dg::TM - 1) / dg::TM;
@@ -475,11 +476,10 @@ int launch_gemm_decode_x(const float *x, int B, int64_t ldx, const bf16 *Wf, int
   const int ldp = tiles * dg::TM;
   VB_CHECK_ARG(partials && stats && partial_bytes >= (size_t)splits * dg::TN * ldp * sizeof(float),
                "gemm_decode_x: partial buffer too small");
-  if (out_splits) *out_splits = splits;
-  if (out_ldp) *out_ldp = ldp;
-  if (out_copies) *out_copies = std::min(tiles, kLnFoldMaxCopies);
+  *out = SplitK{partials, splits, ldp, F.dvec,
+                LnFoldStats{stats, F.c, splits, K, 1e-5f, std::min(tiles, kLnFoldMaxCopies)}};
   CUtensorMap tw, tx;
-  VB_TRY(tc::make_tmap(&tw, Wf, N, K, K, dg::TM));
+  VB_TRY(tc::make_tmap(&tw, (const bf16 *)F.wf, N, K, K, dg::TM));
   VB_TRY(tc::make_tmap_f32_dense(&tx, x, B, K, ldx, dg::TN, tc::BK));
   static PerDeviceOnce once;
   if (once.first())

@@ -226,7 +226,7 @@ static int launch_t(const CUtensorMap &ta, const CUtensorMap &tb, const CUtensor
 
 bool wgmma_gemm_supported(int64_t M, int N, int K, int64_t lda, int64_t ldc) {
   return M >= 1 && (M + tc::BM - 1) / tc::BM <= 65535 && N % 128 == 0 && K % tc::BK == 0 && K > 0 &&
-         lda % 8 == 0 && ldc % 8 == 0 && getenv("VB_DISABLE_WGMMA") == nullptr;
+         lda % 8 == 0 && ldc % 8 == 0 && tune("VB_DISABLE_WGMMA", 0) == 0;
 }
 
 int launch_gemm_wgmma(const bf16 *A, int64_t lda, const bf16 *W, const float *bias, void *C, int c_dtype,

@@ -139,10 +139,6 @@ int launch_gemm_wgmma(const bf16 *A, int64_t lda, const bf16 *W, const float *bi
 enum { DG_F32 = 0, DG_RESIDUAL = 1, DG_RELU_BF16 = 2, DG_QKV = 3 };
 constexpr int kMaxForcedSplits = 16;  // cap of a caller-chosen split-K count (sizes the partial workspace)
 size_t gemm_decode_workspace(int d_model, int d_ff);
-int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, int N, int K, int force_splits,
-                       const float *bias, int mode, float *out_f32, bf16 *out_bf16, int64_t ld_out,
-                       const QkvScatter *qkv, float *partials, size_t partial_bytes, int *out_splits, int *out_ldp,
-                       const KvPrefetch *pf, bool pdl, cudaStream_t s, bool red_add = false);
 // LayerNorm folded into the projection (decode chain without the residual + LayerNorm launches):
 //   moments of the fp32 rows, stats[split][64][2] = (sum x, sum x^2) over the split's k-range, next to the partials
 struct LnFoldStats {
@@ -176,9 +172,26 @@ __device__ __forceinline__ void ln_fold_moments_finish(const LnFoldStats &f, flo
 __device__ __forceinline__ void ln_fold_moments(const LnFoldStats &f, int b, int which, float &mean, float &rstd) {
   ln_fold_moments_finish(f, ln_fold_moments_load(f, b, which), mean, rstd);
 }
-int launch_gemm_decode_x(const float *x, int B, int64_t ldx, const bf16 *Wf, int N, int K, int force_splits,
-                         float *partials, size_t partial_bytes, float *stats, int *out_splits, int *out_ldp,
-                         int *out_copies, const KvPrefetch *pf, bool pdl, cudaStream_t s);
+// What a decode projection hands to the kernel that consumes it: fp32 partial tiles [splits][64][ldp] for the
+// consumer to add up in fixed order 0..splits-1, then `bias`; with a folded LayerNorm (fold.stats != NULL) the rows'
+// moments as well, and `bias` is the folded bias.  part == NULL: nothing is pending, the projection applied its own
+// epilogue (one split, the QKV scatter, the in-cluster residual update).
+struct SplitK {
+  const float *part = nullptr;
+  int splits = 0, ldp = 0;
+  const float *bias = nullptr;
+  LnFoldStats fold{};
+};
+// out receives the hand-over: the partials when the projection leaves any, and its bias
+int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, int N, int K, int force_splits,
+                       const float *bias, int mode, float *out_f32, bf16 *out_bf16, int64_t ld_out,
+                       const QkvScatter *qkv, float *partials, size_t partial_bytes, SplitK *out,
+                       const KvPrefetch *pf, bool pdl, cudaStream_t s, bool red_add = false);
+// projection of the fp32 rows by the weights of F (vb_ln_fold): out receives the partials, F's c and folded bias, and
+// the moments the kernel leaves in stats
+int launch_gemm_decode_x(const float *x, int B, int64_t ldx, const vb_ln_fold &F, int N, int K, int force_splits,
+                         float *partials, size_t partial_bytes, float *stats, SplitK *out, const KvPrefetch *pf,
+                         bool pdl, cudaStream_t s);
 int launch_ln_fold(const bf16 *W, int N, int K, const float *gamma, const float *beta, const float *bias, bf16 *wf,
                    float *c, float *dvec, cudaStream_t s);
 
@@ -194,19 +207,15 @@ int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const 
                            int mask_mode, bf16 *out, bf16 *kcache, bf16 *vcache, int64_t cache_seq_stride,
                            int cache_cap, cudaStream_t s);
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
-int launch_attn_decode(const float *q, const float *qkv_part, int qkv_splits, int qkv_ldp, const float *qkv_bias,
-                       int B, int n_head, int head_dim, void *kcache, void *vcache, int dtype,
-                       int64_t cache_seq_stride, int cache_cap, const int32_t *text_len, const int32_t *prompt_len,
-                       const int32_t *n_gen, const int32_t *finished, float *out, void *out16, void *workspace,
-                       bool pdl, cudaStream_t s, const LnFoldStats *fold = nullptr);
+// the current token's q, k, v (kv.q, or pending in qkv) against the layer's caches kv.kcache / kv.vcache
+int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
+                       void *workspace, bool pdl, cudaStream_t s);
 
 // decode_fused.cu
-int launch_relu_reduce(const float *partials, int splits, int ldp, const float *bias, int B, int N, bf16 *out16,
-                       int64_t ldo, bool pdl, cudaStream_t s, const LnFoldStats *fold = nullptr);
+int launch_relu_reduce(const SplitK &in, int B, int N, bf16 *out16, int64_t ldo, bool pdl, cudaStream_t s);
 // post = true: the post-norm of a post-LN layer, x[b,:] = LayerNorm(x[b,:] + bias + partials) (normalised in place)
-int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const float *partials, int splits, int ldp,
-                     const float *bias, const float *gamma, const float *beta, float eps, bf16 *out16,
-                     bool pdl, cudaStream_t s, bool post = false);
+int launch_ln_reduce(float *x, int64_t ldx, int B, int d, const SplitK &in, const float *gamma, const float *beta,
+                     float eps, bf16 *out16, bool pdl, cudaStream_t s, bool post = false);
 
 // embed_norm.cu: the post-norm of a post-LN layer over the rows x[n_rows, d] (fp32, dense): x = LayerNorm(x) (AdaLN with
 // ada_wb != NULL) in place, and the same rows in out_dtype into `out` (may be NULL)
@@ -230,8 +239,8 @@ int launch_cast_from_f32(const float *in, void *out, int dtype, int64_t n, cudaS
 // sample.cu
 // head->greedy == 2 (and neither `forced` nor `reduce_only`) launches the seeded device sampler, which reads
 // st->sample_seed / top_k / temperature; every other call the argmax / push / reduce kernel
-int launch_ar_sample(float *logits, int64_t ld_logits, const float *partials, int splits, int ldp,
-                     const vb_ar_head *head, vb_ar_state *st, int d, const int64_t *forced, int reduce_only, bool pdl,
-                     cudaStream_t s, const LnFoldStats *fold = nullptr);
+// in: the head projection's pending partials (in.part == NULL: the logits are complete)
+int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const vb_ar_head *head, vb_ar_state *st,
+                     int d, const int64_t *forced, int reduce_only, bool pdl, cudaStream_t s);
 
 }  // namespace vb

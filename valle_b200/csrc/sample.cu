@@ -268,12 +268,8 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
   }
 }
 
-int launch_ar_sample(float *logits, int64_t ld_logits, const float *partials, int splits, int ldp,
-                     const vb_ar_head *head, vb_ar_state *st, int d, const int64_t *forced, int reduce_only, bool pdl,
-                     cudaStream_t s, const LnFoldStats *fold) {
-  LnFoldStats f{};
-  if (fold) f = *fold;
-  const float *fold_d = fold ? head->fold.dvec : nullptr;
+int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const vb_ar_head *head, vb_ar_state *st,
+                     int d, const int64_t *forced, int reduce_only, bool pdl, cudaStream_t s) {
   const bool sample = head->greedy == 2 && forced == nullptr && !reduce_only;
   SamplerArgs sa{};
   if (sample) {
@@ -282,10 +278,10 @@ int launch_ar_sample(float *logits, int64_t ld_logits, const float *partials, in
     sa = SamplerArgs{st->sample_seed, st->top_k, st->temperature};
   }
   VB_CUDA(launch_kernel(sample ? ar_sample_kernel<true> : ar_sample_kernel<false>, dim3(st->B), dim3(256), 0, s, pdl,
-                        logits, ld_logits, partials, splits, ldp, head->n_vocab, head->eos_id, head->audio_emb,
+                        logits, ld_logits, in.part, in.splits, in.ldp, head->n_vocab, head->eos_id, head->audio_emb,
                         head->alpha, head->pe, head->pe_rows, (const int32_t *)st->text_len,
                         (const int32_t *)st->prompt_len, (const int32_t *)st->max_new, st->n_gen, st->finished,
-                        st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, f, fold_d, sa));
+                        st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, in.fold, in.bias, sa));
   count_launch();
   return VB_OK;
 }

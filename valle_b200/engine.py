@@ -67,8 +67,8 @@ class EngineStats:
 
 
 class _ArBuffers:
-    """Persistent device state for the AR loop at one (B, cache_cap, tok_stride) shape, plus the
-    captured CUDA graph of one decode step."""
+    """Persistent device state for the AR loop at one (B, cache_cap, tok_stride) shape, plus the CUDA graphs of
+    decode steps captured on it."""
 
     def __init__(self, eng: "ValleEngine", B: int, cap: int, tok_stride: int):
         dev, d = eng.device, eng.d
@@ -102,7 +102,8 @@ class _ArBuffers:
         self.st = st
         nbytes = eng.lib.vb_ar_step_workspace(C.byref(nd.desc), B, cap)
         self.ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
-        self.graph: Optional[torch.cuda.CUDAGraph] = None
+        #: (head tables, draw mode, steps) -> (graph of that many decode steps, kernels per replay, head struct)
+        self.graphs: Dict[tuple, Tuple[torch.cuda.CUDAGraph, int, L.ArHead]] = {}
         self.eng = eng
 
 
@@ -178,9 +179,6 @@ class ValleEngine:
         self.last_packed: Optional[torch.Tensor] = None
         #: rows of one tensor-core decode group (gemm_decode.cu: one UMMA N tile); larger bf16 batches are split
         self.max_tc_batch = 64
-        #: bf16 pre-LN decode steps run the LayerNorm-folded chain (6 launches per layer instead of 8); post-LN stacks
-        #: always run the 8-launch chain
-        self.use_decode_fold = os.environ.get("VB_DECODE_FOLD", "1") != "0"
         #: decode steps that draw on the device (greedy or seeded) captured per CUDA graph (one replay per group; the stop
         #: flags are polled every `poll` steps)
         self.steps_per_graph = 8
@@ -206,11 +204,13 @@ class ValleEngine:
         cast = (lambda t: t.detach().to(self.dtype).contiguous()) if self.dtype != torch.float32 \
             else (lambda t: t.detach())
         self.ar_predict_w = cast(m.ar_predict_layer.weight)
-        # bf16 decode chain: LayerNorms folded into the projections that consume them (vb_ln_fold), incl. the final norm
-        # into ar_predict_layer (valle.py:1039)
+        # bf16 pre-LN decode steps run the LayerNorm-folded chain (6 launches per layer instead of 8): the LayerNorms
+        # folded into the projections that consume them (vb_ln_fold), incl. the final norm into ar_predict_layer
+        # (valle.py:1039).  VB_DECODE_FOLD=0 keeps the 8-launch chain, which post-LN stacks always run.
         self.ar_head_fold = None
         fn = m.ar_decoder.norm
-        if self.dtype == torch.bfloat16 and self.use_decode_fold and fn is not None and self.ar.enable_decode_fold():
+        fold = os.environ.get("VB_DECODE_FOLD", "1") != "0"
+        if self.dtype == torch.bfloat16 and fold and fn is not None and self.ar.enable_decode_fold():
             self.ar_head_fold = self.ar.fold_layernorm(self.ar_predict_w, fn.weight.detach(), fn.bias.detach(), None)
         self.nar_predict_w = [cast(l.weight) for l in m.nar_predict_layers] if self.Q > 1 else []
         self._ada_cache = None
@@ -567,27 +567,8 @@ class ValleEngine:
 
     def _decode_step(self, buf: _ArBuffers, head: L.ArHead, greedy: bool, top_k: int, temperature: float,
                      forced_step: Optional[torch.Tensor] = None):
-        """greedy: the step draws on the device (argmax, or the seeded sampler when head.greedy == 2)"""
-        if greedy and self.use_cuda_graph:
-            key = (head.pe, head.predict_w, head.audio_emb, head.greedy)
-            if buf.graph is not None and buf.graph_key != key:
-                buf.graph = None
-            if buf.graph is None:
-                # warm-up launch (also sets function attributes), then capture the same call
-                self._launch_step(buf, head)
-                g = torch.cuda.CUDAGraph()
-                n0 = self.lib.vb_launch_count()
-                with torch.cuda.graph(g):
-                    self._launch_step(buf, head)
-                buf.graph_kernels = self.lib.vb_launch_count() - n0  # kernels inside one replay
-                self.captured_launches += buf.graph_kernels      # recorded, not executed
-                buf.graph = g
-                buf.graph_head = head  # keep the struct alive
-                buf.graph_key = key
-                return  # the warm-up launch was this step
-            buf.graph.replay()
-            self.replayed_launches += buf.graph_kernels
-            return
+        """one decode step without a graph; greedy: the step draws on the device (argmax, or the seeded sampler when
+        head.greedy == 2), else on the host"""
         self._launch_step(buf, head)
         if not greedy:
             self._sample_push(buf, head, top_k, temperature, forced_step)
@@ -596,7 +577,7 @@ class ValleEngine:
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
         draw mode, k))"""
         key = (head.pe, head.predict_w, head.audio_emb, head.greedy, k)
-        graphs = buf.__dict__.setdefault("graphs", {})
+        graphs = buf.graphs
         ent = graphs.get(key)
         if ent is None:
             if any(kk[:3] != key[:3] for kk in graphs):
