@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 7
+#define VB_ABI_VERSION 8
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32. */
@@ -386,6 +386,43 @@ int vb_gather_rows(const float *src, int64_t src_row_stride, const int32_t *rows
 
 /* out[i] = in[i] rounded to `dtype` (VB_F32: a copy), n fp32 values: the head operand of a stack without a final norm */
 int vb_cast_from_f32(const float *in, void *out, int dtype, int64_t n, vb_stream_t stream);
+
+/* a2  Text pre-net training (valle/models/valle.py:96-123,181-213): Conv1d(C, C, 5, "same") -> BatchNorm1d(C) -> ReLU
+ *   -> Dropout, three times, over the padded text batch.  Rows are utterance after utterance, seg_len rows each
+ *   (M = N * seg_len, padding rows included, as the reference convolves them); C a multiple of 32.  A convolution is
+ *   vb_linear over the im2col operand [M, 5C] (column block k = row r + k - 2 of the same utterance, zero outside it)
+ *   with the shift-major weight [Cout, 5 Cin].  Column reductions go through per-block partials in the workspace,
+ *   added in a fixed order: no atomics, the same bits in every run. */
+size_t vb_batchnorm_workspace(int64_t M, int C);
+/* h: the fp32 convolution output [M, C] (bias included).  training = 1: per-channel batch mean and biased variance over
+ *   all M rows, running_mean / running_var updated in place with `momentum` (the variance unbiased, M / (M - 1)); M must
+ *   be > 1.  training = 0: the running statistics.  save_mean / save_rstd [C] receive the statistics used, for
+ *   vb_batchnorm_backward: the mean minus the channel's shift, and 1 / sqrt(var + eps).  The shift is h[0, c] with
+ *   training = 1 (statistics of h - h[0, c] stay exact in fp32 where |mean| >> sigma), 0 with training = 0.  y[r, c] = dropout(relu(gamma (h - mean) rstd + beta)), mask = the stateless hash of
+ *   (dropout_seed, dropout_stream, r * C + c) as vb_dropout (dropout_p = 0: off).  out (out_dtype): taps = 5 the
+ *   im2col [M, 5C] of y for the next convolution, taps = 1 y itself [M, C].  gamma == NULL: y = h (no statistics,
+ *   activation or dropout; the im2col of the first convolution's input). */
+int vb_batchnorm_forward(const float *h, int64_t M, int C, int seg_len, const float *gamma, const float *beta,
+                         float *running_mean, float *running_var, float eps, float momentum, int training,
+                         float *save_mean, float *save_rstd, float dropout_p, uint64_t dropout_seed,
+                         uint32_t dropout_stream, void *out, int out_dtype, int taps, void *workspace,
+                         size_t workspace_bytes, vb_stream_t stream);
+/* Backward of vb_batchnorm_forward.  dy (fp32): the gradient w.r.t. its output, [M, 5C] (taps = 5: the input gradient
+ *   of the next convolution, summed over the five shifts in order k = 0..4) or [M, C] (taps = 1).  The dropout mask
+ *   and the ReLU gate are regenerated from h and the saved statistics; gz = the gradient w.r.t. gamma xhat + beta.
+ *   dh (dh_dtype) = gamma rstd (gz - (sum gz + xhat sum gz xhat) / M) with training = 1, gamma rstd gz with
+ *   training = 0; dgamma = sum gz xhat, dbeta = sum gz, dbias = sum over rows of dh (the convolution bias gradient),
+ *   each written (not accumulated) and each may be NULL.  gamma == NULL: dh = the col2im of dy (the gradient w.r.t.
+ *   the first convolution's input). */
+int vb_batchnorm_backward(const float *dy, int taps, const float *h, int64_t M, int C, int seg_len,
+                          const float *gamma, const float *beta, const float *save_mean, const float *save_rstd,
+                          int training, float dropout_p, uint64_t dropout_seed, uint32_t dropout_stream, void *dh,
+                          int dh_dtype, float *dgamma, float *dbeta, float *dbias, void *workspace,
+                          size_t workspace_bytes, vb_stream_t stream);
+/* Audio pre-net backward of ReLU -> Dropout (valle.py:114-123): dz[i] = dy[i] / (1 - p) where h[i] > 0 (h: the ReLU
+ *   output) and the mask of vb_dropout(seed, stream) keeps i, else 0; dz == dy allowed. */
+int vb_relu_dropout_backward(const void *dy, const void *h, void *dz, int dtype, int64_t n, float dropout_p,
+                             uint64_t dropout_seed, uint32_t dropout_stream, vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * f3  Optimizer steps of the trainer (bin/trainer.py:923-951, 688): ScaledAdam and Eve of

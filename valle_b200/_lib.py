@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 VB_F32, VB_BF16 = 0, 1
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -171,6 +171,13 @@ PROTOTYPES = {
     "vb_permute3": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     "vb_gather_rows": (C.c_int, [vp, C.c_int64, vp, C.c_int64, C.c_int, vp, C.c_int64, vp]),
     "vb_cast_from_f32": (C.c_int, [vp, vp, C.c_int, C.c_int64, vp]),
+    "vb_batchnorm_workspace": (C.c_size_t, [C.c_int64, C.c_int]),
+    "vb_batchnorm_forward": (C.c_int, [vp, C.c_int64, C.c_int, C.c_int, vp, vp, vp, vp, C.c_float, C.c_float, C.c_int,
+                                       vp, vp, C.c_float, C.c_uint64, C.c_uint32, vp, C.c_int, C.c_int, vp, C.c_size_t,
+                                       vp]),
+    "vb_batchnorm_backward": (C.c_int, [vp, C.c_int, vp, C.c_int64, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int,
+                                        C.c_float, C.c_uint64, C.c_uint32, vp, C.c_int, vp, vp, vp, vp, C.c_size_t, vp]),
+    "vb_relu_dropout_backward": (C.c_int, [vp, vp, vp, C.c_int, C.c_int64, C.c_float, C.c_uint64, C.c_uint32, vp]),
     "vb_scaled_adam_workspace": (C.c_size_t, [C.c_int, C.c_int]),
     "vb_scaled_adam_step": (C.c_int, [vp, vp, c_i32p, C.POINTER(ScaledAdamArgs), vp, vp, vp, C.c_size_t, vp]),
     "vb_eve_workspace": (C.c_size_t, [vp, C.c_int]),

@@ -287,6 +287,182 @@ class DecoderStack(torch.autograd.Function):
         return (dx, dada, None, None, *grads)
 
 
+#: dropout site ids of the pre-nets (csrc/kernels.cuh::drop_keep): PRENET_STREAM | site << 4 | dropout index; the
+#: decoder layers use (layer << 2) | k and the positional encodings 0x10000 + k
+PRENET_STREAM = 0x20000
+PRENET_SITES = {"ar_text": 0, "nar_text": 1, "ar_audio": 2, "nar_audio": 3}
+_TEXT_BLOCKS = (1, 5, 9)   # Conv1d indices of the text pre-net Sequential (valle.py:97-113); BatchNorm1d at +1, Dropout +3
+
+
+def text_prenet_params(seq) -> List[torch.Tensor]:
+    """(conv weight, conv bias, BatchNorm weight, BatchNorm bias) of the three blocks, then the Linear's weight, bias"""
+    out = []
+    for i in _TEXT_BLOCKS:
+        out += [seq[i].weight, seq[i].bias, seq[i + 1].weight, seq[i + 1].bias]
+    return out + [seq[14].weight, seq[14].bias]
+
+
+def audio_prenet_params(seq) -> List[torch.Tensor]:
+    return [seq[0].weight, seq[0].bias, seq[3].weight, seq[3].bias, seq[6].weight, seq[6].bias]
+
+
+def _linear_grads(x, w, dy, dx, dw, db):
+    """vb_linear_backward of y = x w^T + b, x / w / dy in one dtype: dx = dy w (None: skipped), dw += dy^T x,
+    db += column sums of dy (None: skipped)"""
+    lib = L.load()
+    M, K = x.shape
+    N = w.shape[0]
+    dt = _DT[x.dtype]
+    wt = w.t().contiguous()
+    nb = lib.vb_linear_backward_workspace(dt, M, N, K)
+    ws = torch.empty(nb, dtype=torch.uint8, device=x.device)
+    L.check(lib.vb_linear_backward(x.data_ptr(), dt, x.stride(0), wt.data_ptr(), dy.data_ptr(), dy.stride(0),
+                                   L.ptr(dx), _DT[dx.dtype] if dx is not None else L.VB_F32,
+                                   dx.stride(0) if dx is not None else K, L.VB_EPI_NONE, dw.data_ptr(), L.ptr(db), M, N,
+                                   K, ws.data_ptr(), nb, _s()), "vb_linear_backward")
+
+
+class TextPrenet(torch.autograd.Function):
+    """The text pre-net (valle.py:96-113) over the embedded, padded text batch e [N * seg_len, C] fp32: three
+    Conv1d(k=5, "same") -> BatchNorm1d -> ReLU -> Dropout blocks and a Linear, GEMM operands in `dtype`.  BatchNorm
+    follows the module's mode: train() normalises by the batch statistics over all rows (padding included) and updates
+    the running statistics in place, eval() uses the running statistics.  Dropout is live in train() with the
+    library's stateless mask.  Backward: the gradients of every pre-net parameter and of e."""
+
+    @staticmethod
+    def forward(ctx, e, seq, seg_len, dtype, drop_seed, site, *params):
+        lib = L.load()
+        dev = e.device
+        e = e.detach().contiguous()
+        M, C_ = e.shape
+        dt = _DT[dtype]
+        training = bool(seq.training)
+        if training and M < 2:
+            raise ValueError(f"Expected more than 1 value per channel when training, got input size [1, {C_}, 1]")
+        if any(seq[j + 1].momentum is None for j in _TEXT_BLOCKS):
+            raise NotImplementedError("valle_b200: BatchNorm1d(momentum=None) is not built")
+        nb = lib.vb_batchnorm_workspace(M, C_)
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        col = torch.empty((M, 5 * C_), dtype=dtype, device=dev)
+        blocks = []
+        with torch.cuda.device(dev):
+            L.check(lib.vb_batchnorm_forward(e.data_ptr(), M, C_, seg_len, 0, 0, 0, 0, 0.0, 0.0, 0, 0, 0, 0.0, 0, 0,
+                                             col.data_ptr(), dt, 5, 0, 0, _s()), "vb_batchnorm_forward")
+            for i, j in enumerate(_TEXT_BLOCKS):
+                conv, bn, drop = seq[j], seq[j + 1], seq[j + 3]
+                w = conv.weight.detach().permute(0, 2, 1).reshape(C_, 5 * C_).to(dtype).contiguous()
+                h = ops.linear(col, w, conv.bias.detach(), out_dtype=torch.float32)
+                mean = torch.empty(C_, dtype=torch.float32, device=dev)
+                rstd = torch.empty_like(mean)
+                taps = 5 if i < 2 else 1
+                nxt = torch.empty((M, taps * C_), dtype=dtype, device=dev)
+                p = float(drop.p) if training else 0.0
+                sid = PRENET_STREAM | (site << 4) | i
+                L.check(lib.vb_batchnorm_forward(h.data_ptr(), M, C_, seg_len, bn.weight.data_ptr(), bn.bias.data_ptr(),
+                                                 bn.running_mean.data_ptr(), bn.running_var.data_ptr(), float(bn.eps),
+                                                 float(bn.momentum), int(training), mean.data_ptr(), rstd.data_ptr(), p,
+                                                 int(drop_seed), sid, nxt.data_ptr(), dt, taps, ws.data_ptr(), nb,
+                                                 _s()), "vb_batchnorm_forward")
+                if training:
+                    # the running statistics changed in place; this bump also moves the engine's weight signature
+                    bn.num_batches_tracked.add_(1)
+                blocks.append((col, w, h, mean, rstd, p, sid))
+                col = nxt
+            wl = seq[14].weight.detach().to(dtype).contiguous()
+            out = ops.linear(col, wl, seq[14].bias.detach(), out_dtype=torch.float32)
+        ctx.blocks, ctx.last = blocks, (col, wl)
+        ctx.cfg = (seq, seg_len, dtype, training, int(drop_seed))
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.load()
+        seq, seg_len, dtype, training, seed = ctx.cfg
+        dev = dout.device
+        col3, wl = ctx.last
+        M, C_ = col3.shape
+        dt = _DT[dtype]
+        nb = lib.vb_batchnorm_workspace(M, C_)
+        ws = torch.empty(nb, dtype=torch.uint8, device=dev)
+        f32 = dict(dtype=torch.float32, device=dev)
+        with torch.cuda.device(dev):
+            dl_w, dl_b = torch.zeros((C_, C_), **f32), torch.zeros(C_, **f32)
+            dy, taps = torch.empty((M, C_), **f32), 1
+            _linear_grads(col3, wl, ops.cast_from_f32(dout.to(torch.float32).contiguous(), dtype), dy, dl_w, dl_b)
+            grads = [None] * 3
+            for i in (2, 1, 0):
+                col, w, h, mean, rstd, p, sid = ctx.blocks[i]
+                bn = seq[_TEXT_BLOCKS[i] + 1]
+                dh = torch.empty((M, C_), dtype=dtype, device=dev)
+                dg, dbeta, dbias = (torch.empty(C_, **f32) for _ in range(3))
+                L.check(lib.vb_batchnorm_backward(dy.data_ptr(), taps, h.data_ptr(), M, C_, seg_len, bn.weight.data_ptr(),
+                                                  bn.bias.data_ptr(), mean.data_ptr(), rstd.data_ptr(), int(training), p,
+                                                  seed, sid, dh.data_ptr(), dt, dg.data_ptr(), dbeta.data_ptr(),
+                                                  dbias.data_ptr(), ws.data_ptr(), nb, _s()), "vb_batchnorm_backward")
+                dcol, dw = torch.empty((M, 5 * C_), **f32), torch.zeros((C_, 5 * C_), **f32)
+                _linear_grads(col, w, dh, dcol, dw, None)   # the conv bias gradient came from the BatchNorm kernel
+                grads[i] = [dw.view(C_, 5, C_).permute(0, 2, 1).contiguous(), dbias, dg, dbeta]
+                dy, taps = dcol, 5
+            de = torch.empty((M, C_), **f32)
+            L.check(lib.vb_batchnorm_backward(dy.data_ptr(), 5, 0, M, C_, seg_len, 0, 0, 0, 0, 0, 0.0, 0, 0,
+                                              de.data_ptr(), L.VB_F32, 0, 0, 0, 0, 0, _s()), "vb_batchnorm_backward")
+        ctx.blocks = ctx.last = None
+        return (de, None, None, None, None, None, *grads[0], *grads[1], *grads[2], dl_w, dl_b)
+
+
+class AudioPrenet(torch.autograd.Function):
+    """The audio pre-net (valle.py:114-123) per row of x [R, C] fp32: Linear(C, 256) -> ReLU -> Dropout ->
+    Linear(256, 256) -> ReLU -> Dropout -> Linear(256, C), GEMM operands in `dtype`, dropout live in train()."""
+
+    @staticmethod
+    def forward(ctx, x, seq, dtype, drop_seed, site, w1, b1, w2, b2, w3, b3):
+        lib = L.load()
+        dev = x.device
+        x = x.detach().contiguous()
+        a = x if dtype == torch.float32 else ops.cast_from_f32(x, dtype)
+        ws_ = [w.detach().to(dtype).contiguous() for w in (w1, w2, w3)]
+        saved = [a]
+        drops = []
+        with torch.cuda.device(dev):
+            for j, (w, b) in enumerate(zip(ws_[:2], (b1, b2))):
+                h = ops.linear(a, w, b.detach(), L.VB_EPI_RELU)
+                p = float(seq[3 * j + 2].p) if seq.training else 0.0
+                sid = PRENET_STREAM | (site << 4) | j
+                a = h
+                if p > 0:
+                    a = torch.empty_like(h)
+                    L.check(lib.vb_dropout(h.data_ptr(), a.data_ptr(), _DT[dtype], h.numel(), p, int(drop_seed), sid,
+                                           _s()), "vb_dropout")
+                saved += [h, a]
+                drops.append((p, sid))
+            out = ops.linear(a, ws_[2], b3.detach(), out_dtype=torch.float32)
+        ctx.saved, ctx.ws, ctx.drops, ctx.seed, ctx.dtype = saved, ws_, drops, int(drop_seed), dtype
+        return out
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = L.load()
+        a0, h1, a1, h2, a2 = ctx.saved
+        dtype, dev = ctx.dtype, dout.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        grads = [None] * 6
+        with torch.cuda.device(dev):
+            dy = ops.cast_from_f32(dout.to(torch.float32).contiguous(), dtype)
+            for j, (x, h) in ((2, (a2, h2)), (1, (a1, h1)), (0, (a0, None))):
+                w = ctx.ws[j]
+                dw, db = torch.zeros(w.shape, **f32), torch.zeros(w.shape[0], **f32)
+                dx = torch.empty((x.shape[0], w.shape[1]), dtype=dtype if j > 0 else torch.float32, device=dev)
+                _linear_grads(x, w, dy, dx, dw, db)
+                grads[2 * j], grads[2 * j + 1] = dw, db
+                if j > 0:
+                    p, sid = ctx.drops[j - 1]
+                    L.check(lib.vb_relu_dropout_backward(dx.data_ptr(), h.data_ptr(), dx.data_ptr(), _DT[dtype],
+                                                         dx.numel(), p, ctx.seed, sid, _s()), "vb_relu_dropout_backward")
+                dy = dx
+        ctx.saved = ctx.ws = None
+        return (dy, None, None, None, None, *grads)
+
+
 class Dropout(torch.autograd.Function):
     """nn.Dropout after the positional encoding (valle/modules/embedding.py:97) on the library's stateless mask:
     vb_dropout forward, the same call on the gradient backward."""

@@ -78,7 +78,7 @@ class Transpose(nn.Identity):
 def _text_prenet(d: int) -> nn.Sequential:
     """valle.py:97-113 / 182-204: 3 x (Conv1d k=5 'same' -> BatchNorm1d -> ReLU -> Dropout(0.5)) between two
     transposes, then Linear.  Parameter container with the reference's state_dict keys (ar_text_prenet.1.weight ...);
-    the arithmetic runs in the engine (ValleEngine._text_prenet)."""
+    the arithmetic runs in the engine (ValleEngine._text_prenet; autograd.TextPrenet in training or with gradients)."""
     layers: List[nn.Module] = [Transpose()]
     for _ in range(3):
         layers += [nn.Conv1d(d, d, kernel_size=5, padding="same"), nn.BatchNorm1d(d), nn.ReLU(), nn.Dropout(0.5)]

@@ -89,22 +89,38 @@ def _valle_forward(model, x: torch.Tensor, x_lens: torch.Tensor, y, y_lens, redu
     total_loss = torch.zeros((), device=dev)
     x_emb_out = None
     eng = None
-    if getattr(model, "add_prenet", False):
-        # valle.py:830,864,898,918: pre-nets between embedding and position.  Evaluation only: BatchNorm1d on its running
-        # statistics (folded into the conv weights by the engine), Dropout = identity
-        if want_grad or model.training:
-            raise NotImplementedError("valle_b200: training with add_prenet=True (BatchNorm batch statistics, pre-net "
-                                      "dropout and their gradients) is not built; evaluation and inference are")
+    # valle.py:830,864,898,918: pre-nets between embedding and position.  Evaluation without gradients runs the engine's
+    # folded pre-nets (BatchNorm1d on its running statistics folded into the conv weights, Dropout = identity); training
+    # mode or gradients run them through autograd.TextPrenet / AudioPrenet (batch statistics in train(), which update
+    # the running statistics in place even under torch.no_grad(), as nn.BatchNorm1d does)
+    prenet = getattr(model, "add_prenet", False)
+    native_prenet = prenet and (want_grad or model.training)
+    if prenet and not native_prenet:
         eng = model.engine()
         eng._refresh()
 
-    def embed_pe(tokens, table, pos_mod, T, text_prenet=None, site=None):
-        """[N, T] ids -> [N, T, d] = dropout(prenet(table[ids]) + alpha * pe[:T])."""
+    def text_prenet(e, name, T):
+        if eng is not None:
+            # the reference convolves the padded batch: pad-token embeddings inside, zeros beyond the longest text
+            return eng._text_prenet(e, [T] * N, name)
+        seq = getattr(model, name + "_prenet")
+        return AG.TextPrenet.apply(e, seq, T, dtype, drop_seed, AG.PRENET_SITES[name], *AG.text_prenet_params(seq))
+
+    def audio_prenet(rows, name):
+        if eng is not None:
+            return eng._audio_prenet(rows, name)
+        seq = getattr(model, name + "_prenet")
+        return AG.AudioPrenet.apply(rows, seq, dtype, drop_seed, AG.PRENET_SITES[name], *AG.audio_prenet_params(seq))
+
+    def embed_pe(tokens, table, pos_mod, T, prenet_name=None, site=None):
+        """[N, T] ids -> [N, T, d] = dropout(prenet(table[ids]) + alpha * pe[:T]); prenet_name: "ar_text" / "nar_text"
+        (the text pre-nets), "ar_audio" (the AR audio pre-net unless `table` already holds it) or None"""
         tok = tokens.reshape(-1).contiguous()
         e = AG.EmbedSum.apply(tok, 1, 0, tok.numel(), table)
-        if eng is not None and text_prenet is not None:
-            # the reference convolves the padded batch: pad-token embeddings inside, zeros beyond the longest text
-            e = eng._text_prenet(e, [T] * N, text_prenet)
+        if prenet and prenet_name in ("ar_text", "nar_text"):
+            e = text_prenet(e, prenet_name, T)
+        elif native_prenet and prenet_name == "ar_audio":
+            e = audio_prenet(e, prenet_name)
         return add_pe(e.view(N, T, table.shape[1]), pos_mod, T, site)
 
     # training mode (model.train(), bin/trainer.py:512): the Dropout modules of the reference are live -- after every
@@ -154,7 +170,7 @@ def _valle_forward(model, x: torch.Tensor, x_lens: torch.Tensor, y, y_lens, redu
         xe = embed_pe(text, model.ar_text_embedding.weight, model.ar_text_position, Smax, "ar_text", "ar_text")
         Ta = yin.shape[1]                     # Tmax, or Tmax + 1 with the prepended <BOS> (valle.py:820-826,833)
         ar_table = eng.ar_audio_table if eng is not None else model.ar_audio_embedding.weight   # pre-net(embedding)
-        ye = embed_pe(yin.contiguous(), ar_table, model.ar_audio_position, Ta, None, "ar_audio")
+        ye = embed_pe(yin.contiguous(), ar_table, model.ar_audio_position, Ta, "ar_audio", "ar_audio")
         rows = torch.cat([xe, ye], dim=1).reshape(N * (Smax + Ta), d).contiguous()
         nd = model.ar_decoder.native(dtype)
         yl_ar = (yl32 + (Ta - Tmax)).contiguous()
@@ -218,8 +234,8 @@ def _valle_forward(model, x: torch.Tensor, x_lens: torch.Tensor, y, y_lens, redu
             seg1 = (yl32 + (Ty - Tmax)).contiguous()   # key mask F.pad(y_mask, (prefix, 0), False) valle.py:908-914
         elif pm == 1:
             tg = tg[:, prefix_len:]
-        if eng is not None:   # valle.py:918
-            y_emb = eng._audio_prenet(y_emb.reshape(N * Ty, -1).contiguous(), "nar_audio").view(N, Ty, -1)
+        if prenet:   # valle.py:918
+            y_emb = audio_prenet(y_emb.reshape(N * Ty, -1).contiguous(), "nar_audio").view(N, Ty, -1)
         y_pos = add_pe(y_emb.contiguous(), model.nar_audio_position, Ty, "nar_audio")
         Lp = Smax + Ty
         rows = torch.cat([xe, y_pos], dim=1).reshape(N * Lp, xe.shape[-1]).contiguous()
