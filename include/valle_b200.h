@@ -25,11 +25,12 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 8
+#define VB_ABI_VERSION 9
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
-/* storage type of the big matrices / activations.  Accumulation is always fp32. */
-enum vb_dtype { VB_F32 = 0, VB_BF16 = 1 };
+/* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
+ * bf16 AR decoding only (vb_decoder_forward_kv8, vb_ar_state.kv_dtype), never a weight or activation type. */
+enum vb_dtype { VB_F32 = 0, VB_BF16 = 1, VB_E4M3 = 2 };
 enum vb_epilogue { VB_EPI_NONE = 0, VB_EPI_RELU = 1, VB_EPI_RESIDUAL = 2 };
 /* attention visibility rule */
 enum vb_mask_mode {
@@ -171,6 +172,28 @@ int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32
                        int64_t cache_seq_stride, int cache_cap, void *workspace,
                        size_t workspace_bytes, vb_stream_t stream);
 
+/* FP8 (e4m3) KV cache, one power-of-two scale per cached row.
+ *   kcache / vcache: uint8 e4m3 [n_layer, B, H, cache_cap, 64] (the bf16 cache's layout with 1-byte elements);
+ *   k_exp / v_exp:   uint8 [n_layer, B, H, cache_cap], the biased exponent e + 127 of each row (element offset / 64
+ *                    of the row's first cache element: the strides are the cache's strides divided by 64).
+ * Row r (64 elements) is the bf16 row the bf16 cache would hold.  a = max|r|; e = the smallest integer with
+ * a <= 448 * 2^e, exactly from frexpf(a) = m * 2^x: e = x - 9 if m <= 0.875, else x - 8; e clamped to [-127, 127], an
+ * all-zero row gets e = -127.  Stored bytes: cvt.rn.satfinite.e4m3(r * 2^-e) (= torch.float8_e4m3fn rounding of the
+ * exactly scaled row); the row reads back as fp8 * 2^e, exact in fp32.
+ * The AR decode step attends to the CURRENT token's k / v as the unquantized bf16 row it has just computed and appends
+ * the quantized row: an FP8-cache step is the bf16 step run on the dequantized cache.  bf16 decoders only, on the
+ * tensor-core decode chains (B <= 64, not VB_DECODE_SIMT, not VB_ATTN_DECODE_1PASS) and the wgmma prefill attention
+ * (not VB_ATTN_SIMT); everything else returns VB_ERR_UNSUPPORTED. */
+/* vb_decoder_forward that fills an FP8 cache (kcache / vcache / k_exp / v_exp all non-NULL; strides in elements of the
+ * [n_layer, B, H, cache_cap, 64] cache).  The FP8 cache requires (here and in vb_ar_decode_step, VB_ERR_ARG otherwise):
+ * cache_layer_stride and cache_seq_stride multiples of 1024, cache_cap a multiple of 16, k_exp / v_exp 16-byte
+ * aligned -- the decode attention reads the exponent rows 16 bytes at a time. */
+int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                           int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
+                           uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
+                           void *workspace, size_t workspace_bytes, vb_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * a2 / f2  Training: VALLE.forward with gradients (valle/models/valle.py:762-959; loss.backward() at
  *     valle/bin/trainer.py:674).  The backward functions produce what torch.autograd produces for the reference's
@@ -305,6 +328,11 @@ typedef struct vb_ar_state {
   const uint64_t *sample_seed; /* [B] seed of each utterance */
   const int32_t *top_k;        /* [B] <= 0 or >= n_vocab: no filter; 1: argmax */
   const float *temperature;    /* [B] finite, > 0 */
+  /* KV cache type (ABI 9): VB_E4M3 selects the FP8 cache (see vb_decoder_forward_kv8) with its exponent arrays
+   * k_exp / v_exp [n_layer, B, H, cache_cap]; any other value (0 in a zero-initialised state) = the decoder's wdtype */
+  int32_t kv_dtype;
+  int32_t kv_pad_unused;
+  uint8_t *k_exp, *v_exp;
 } vb_ar_state;
 
 typedef struct vb_ar_head {

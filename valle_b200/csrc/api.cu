@@ -175,7 +175,7 @@ VB_API int vb_decoder_set_decode_fold(vb_decoder_t dec, const vb_ln_fold *qkv, c
   return VB_OK;
 }
 
-static size_t elem_size(int dtype) { return dtype == VB_BF16 ? 2 : 4; }
+static size_t elem_size(int dtype) { return dtype == VB_E4M3 ? 1 : dtype == VB_BF16 ? 2 : 4; }
 
 // ------------------------------------------------------------------------------------------
 // Decoder stack: the forward of inference and training, and the backward pass
@@ -256,7 +256,7 @@ T *ada_row(T *wb, int l, int k, int d) {
 DropCfg layer_drop(float p, uint64_t seed, int l, int site) { return make_drop(p, seed, (uint32_t)(l << 2) | (uint32_t)site); }
 
 // The layer loop of vb_decoder_forward and vb_decoder_forward_train.  slots(l): layer l's activation slots; kcache /
-// vcache: null or the caches the attention fills; sub: the fp32 [M, d] scratch of the sub-layer outputs when
+// vcache: null or the caches the attention fills (kexp / vexp non-null: the FP8 cache and its exponents); sub: the fp32 [M, d] scratch of the sub-layer outputs when
 // dropout_p > 0.  Pre-LN (transformer.py:297-302): x += SA(norm1(x)); x += FF(norm2(x)).  Post-LN (:303-308):
 // x = norm1(x + SA(x)); x = norm2(x + FF(x)); a post-norm writes the normalised rows back into x and into the
 // storage-dtype operand of the next GEMM, and layer 0 reads a plain cast.
@@ -264,7 +264,8 @@ template <class Slots>
 int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32_t *cu_seqlens, const int32_t *text_lens,
                   const int32_t *seg1_lens, int seg1_start, int max_seqlen, int mask_mode, const float *ada_wb,
                   Slots slots, void *kcache, void *vcache, int64_t cache_layer_stride, int64_t cache_seq_stride,
-                  int cache_cap, float *sub, float dropout_p, uint64_t dropout_seed, cudaStream_t s) {
+                  int cache_cap, float *sub, float dropout_p, uint64_t dropout_seed, cudaStream_t s,
+                  uint8_t *kexp = nullptr, uint8_t *vexp = nullptr) {
   const vb_decoder_desc &D = dec->desc;
   const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
   const size_t ts = elem_size(dt);
@@ -292,12 +293,15 @@ int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32
     auto attn = [&]() -> int {
       VB_TRY(vb_linear(sv.xn1, dt, d, P.in_proj_w, dt, P.in_proj_b, sv.qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE, nullptr,
                        0, stream));
-      void *kc = kcache ? (char *)kcache + (size_t)l * cache_layer_stride * ts : nullptr;
-      void *vc = vcache ? (char *)vcache + (size_t)l * cache_layer_stride * ts : nullptr;
+      const size_t cs = kexp ? 1 : ts;   // cache element size
+      void *kc = kcache ? (char *)kcache + (size_t)l * cache_layer_stride * cs : nullptr;
+      void *vc = vcache ? (char *)vcache + (size_t)l * cache_layer_stride * cs : nullptr;
+      uint8_t *ke = kexp ? kexp + (size_t)l * cache_layer_stride / 64 : nullptr;
+      uint8_t *ve = vexp ? vexp + (size_t)l * cache_layer_stride / 64 : nullptr;
       const DropCfg dc = layer_drop(dropout_p, dropout_seed, l, 0);
       VB_TRY(launch_attention_varlen(sv.qkv, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
                                      seg1_start, max_seqlen, mask_mode, sv.att, kc, vc, cache_seq_stride, cache_cap,
-                                     nullptr, 0, s, &dc));
+                                     nullptr, 0, s, &dc, ke, ve));
       return residual(sv.att, d, P.out_proj_w, P.out_proj_b, 1);
     };
     auto ffn = [&]() -> int {
@@ -369,6 +373,36 @@ VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, cons
   return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
                        [&](int) { return ws; }, kcache, vcache, cache_layer_stride, cache_seq_stride, cache_cap,
                        nullptr, 0.f, 0, (cudaStream_t)stream);
+}
+
+// the FP8 cache's exponent rows are read 16 bytes at a time (cp.async in the decode attention): every (layer, utterance,
+// head) stream of k_exp / v_exp, at offset stride / 64, and every 16-key chunk of it must start 16-byte aligned
+static bool kv8_layout_ok(const void *k_exp, const void *v_exp, int64_t layer_stride, int64_t seq_stride, int cap) {
+  return layer_stride % 1024 == 0 && seq_stride % 1024 == 0 && cap % 16 == 0 &&
+         (reinterpret_cast<uintptr_t>(k_exp) & 15) == 0 && (reinterpret_cast<uintptr_t>(v_exp) & 15) == 0;
+}
+
+VB_API int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                                  const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                                  int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
+                                  uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
+                                  void *workspace, size_t workspace_bytes, vb_stream_t stream) {
+  VB_CHECK_ARG(dec && x && cu_seqlens && kcache && vcache && k_exp && v_exp, "vb_decoder_forward_kv8: null argument");
+  const vb_decoder_desc &D = dec->desc;
+  if (D.wdtype != VB_BF16) {
+    set_error("vb_decoder_forward_kv8: the FP8 KV cache needs a bf16 decoder");
+    return VB_ERR_UNSUPPORTED;
+  }
+  VB_CHECK_ARG(kv8_layout_ok(k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap),
+               "vb_decoder_forward_kv8: FP8 cache: strides must be multiples of 1024, cache_cap a multiple of 16 and "
+               "k_exp / v_exp 16-byte aligned");
+  VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M), "vb_decoder_forward_kv8: workspace too small");
+  if (M == 0) return VB_OK;
+  Carve c(workspace);
+  const LayerSave ws = carve_forward_ws(c, D, M);
+  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
+                       [&](int) { return ws; }, kcache, vcache, cache_layer_stride, cache_seq_stride, cache_cap,
+                       nullptr, 0.f, 0, (cudaStream_t)stream, k_exp, v_exp);
 }
 
 VB_API size_t vb_decoder_train_save_bytes(const vb_decoder_desc *desc, int64_t M) {
@@ -524,12 +558,19 @@ DecodeSplits decode_splits(const vb_decoder_desc &D, bool fold) {
           knob("VB_SPLITS_FFN1", upto(kb, fold ? 4 : 2)), knob("VB_SPLITS_FFN2", upto(fb, fold ? 8 : 9))};
 }
 
+bool kv_fp8(const vb_ar_state *st) { return st->kv_dtype == VB_E4M3; }
 // layer l's caches and the rows' lengths: where the QKV projection leaves q and appends k / v, what the attention
-// reads and what the KV prefetch pulls into L2
+// reads and what the KV prefetch pulls into L2 (FP8 cache: also the layer's exponent arrays)
 QkvScatter layer_kv(const vb_decoder_desc &D, const vb_ar_state *st, int l, float *q) {
-  const size_t off = (size_t)l * st->cache_layer_stride * elem_size(D.wdtype);
-  return QkvScatter{D.d_model, D.d_model / D.n_head, q, (char *)st->kcache + off, (char *)st->vcache + off,
-                    st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished};
+  const bool f8 = kv_fp8(st);
+  const size_t off = (size_t)l * st->cache_layer_stride * (f8 ? 1 : elem_size(D.wdtype));
+  QkvScatter kv{D.d_model, D.d_model / D.n_head, q, (char *)st->kcache + off, (char *)st->vcache + off,
+                st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished};
+  if (f8) {
+    kv.kexp = st->k_exp + (size_t)l * st->cache_layer_stride / 64;
+    kv.vexp = st->v_exp + (size_t)l * st->cache_layer_stride / 64;
+  }
+  return kv;
 }
 
 // final LayerNorm (adding the pending partials of the last FFN2) + ar_predict_layer + sampler on the tensor-core
@@ -610,9 +651,20 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_decode_step: a pre-LN decoder needs its final norm");
   VB_CHECK_ARG(workspace_bytes >= vb_ar_step_workspace(&D, st->B, st->cache_cap),
                "vb_ar_decode_step: workspace too small");
+  const bool f8 = kv_fp8(st);
+  if (f8 && !use_tc_decode(D, st->B)) {
+    set_error("vb_ar_decode_step: the FP8 KV cache runs on the bf16 tensor-core chains only (bf16, B <= 64, not VB_DECODE_SIMT)");
+    return VB_ERR_UNSUPPORTED;
+  }
+  VB_CHECK_ARG(!f8 || (st->k_exp && st->v_exp &&
+                       kv8_layout_ok(st->k_exp, st->v_exp, st->cache_layer_stride, st->cache_seq_stride, st->cache_cap)),
+               "vb_ar_decode_step: FP8 cache: exponent arrays missing, strides not multiples of 1024, cache_cap %% 16 != 0 "
+               "or k_exp / v_exp not 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model, dff = D.d_ff, B = st->B, dt = D.wdtype, hd = d / D.n_head;
   const size_t ts = elem_size(dt);
+  const int kv_dt = f8 ? VB_E4M3 : dt;
+  const size_t kv_row_bytes = f8 ? hd + 1 : hd * ts;   // one cached row of K (or V), with its exponent byte
   Carve c(workspace);
   const StepWs w = carve_step_ws(c, D, B, st->cache_cap);
   float *x = st->x_cur;
@@ -639,7 +691,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     const int64_t layer_w_bytes = (4 * (int64_t)d * d + 2 * (int64_t)d * dff) * (int64_t)ts;
     const int64_t pf_budget = B >= 16 ? std::max<int64_t>(0, l2_bytes() - layer_w_bytes) *
                                             tune("VB_KV_PREFETCH_L2_PCT", 60) / 100 : 0;
-    const int pf_rows = (int)std::min<int64_t>(st->cache_cap, pf_budget / (2 * (int64_t)B * D.n_head * hd * ts));
+    const int pf_rows = (int)std::min<int64_t>(st->cache_cap, pf_budget / (2 * (int64_t)B * D.n_head * kv_row_bytes));
     float *P = (float *)w.gemm_ws;
     // the four projections of the chain each prefetch a quarter of the first pf_rows rows of the KV streams that the
     // NEXT attention launch will read (QKV: this layer's, the other three: the following layer's)
@@ -648,8 +700,10 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
       if (pf_rows <= 0) return pf;
       const QkvScatter kv = layer_kv(D, st, layer % D.n_layer, w.q);
       pf.kbase = kv.kcache; pf.vbase = kv.vcache;
-      pf.seq_stride_bytes = kv.cache_seq_stride * (int64_t)ts;
-      pf.B = B; pf.H = D.n_head; pf.cap = kv.cache_cap; pf.row_bytes = (int)(hd * ts);
+      const int64_t cs = f8 ? 1 : (int64_t)ts;   // cache element size
+      pf.seq_stride_bytes = kv.cache_seq_stride * cs;
+      pf.B = B; pf.H = D.n_head; pf.cap = kv.cache_cap; pf.row_bytes = (int)(hd * cs);
+      pf.kexp = kv.kexp; pf.vexp = kv.vexp;
       pf.text_len = kv.text_len; pf.prompt_len = kv.prompt_len; pf.n_gen = kv.n_gen;
       pf.row_lo = pf_rows * quarter / 4; pf.row_hi = pf_rows * (quarter + 1) / 4;
       return pf;
@@ -667,10 +721,20 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
                                     &pf_qkv, pdl, s));
       } else {
         if (!post) VB_TRY(launch_ln_reduce(x, d, B, d, pend, L.norm1_w, L.norm1_b, 1e-5f, w.xn16, pdl, s));
-        VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.in_proj_w, 3 * d, d, sp.qkv, L.in_proj_b, DG_QKV,
-                                  nullptr, nullptr, d, &kv, P, w.gemm_ws_bytes, &qkv, &pf_qkv, pdl, s));
+        if (f8) {
+          // the FP8 append needs a head's 64 columns together: the projection always hands its product (the raw sums of
+          // one split land as slab 0) to the attention prologue, which adds the bias and quantizes the rows
+          VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.in_proj_w, 3 * d, d, sp.qkv, nullptr, DG_F32, P,
+                                    nullptr, 3 * d, nullptr, P, w.gemm_ws_bytes, &qkv, &pf_qkv, pdl, s));
+          qkv.part = P;
+          qkv.ldp = 3 * d;
+          qkv.bias = L.in_proj_b;
+        } else {
+          VB_TRY(launch_gemm_decode(w.xn16, B, d, (const bf16 *)L.in_proj_w, 3 * d, d, sp.qkv, L.in_proj_b, DG_QKV,
+                                    nullptr, nullptr, d, &kv, P, w.gemm_ws_bytes, &qkv, &pf_qkv, pdl, s));
+        }
       }
-      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, dt, w.att, w.att16, w.attn_ws, pdl, s));
+      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, kv_dt, w.att, w.att16, w.attn_ws, pdl, s));
       VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, sp.out, L.out_proj_b, DG_RESIDUAL, x,
                                 nullptr, d, nullptr, P, w.gemm_ws_bytes, &out, &pf_out, pdl, s, fold));
       if (fold) {

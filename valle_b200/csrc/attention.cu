@@ -10,6 +10,8 @@
 // valle/modules/activation.py:408-427; masks valle/models/valle.py:1010-1033 (AR) / none (NAR).
 #include <math_constants.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "kernels.cuh"
 
@@ -181,7 +183,7 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
                             const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
                             int seg1_start, int max_seqlen, int mask_mode, void *out, void *kcache, void *vcache,
                             int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
-                            cudaStream_t s, const DropCfg *drop) {
+                            cudaStream_t s, const DropCfg *drop, uint8_t *kexp, uint8_t *vexp) {
   VB_CHECK_ARG(head_dim == HD, "attention: head_dim=%d, only 64 is built", head_dim);
   DropCfg dc{};
   if (drop) dc = *drop;
@@ -197,6 +199,16 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
   VB_CHECK_ARG(mask_mode == VB_MASK_FULL || text_lens != nullptr, "attention: this mask mode needs text_lens");
   VB_CHECK_ARG(mask_mode < VB_MASK_PADDED_AR || seg1_lens != nullptr, "attention: padded mask modes need seg1_lens");
   if (M == 0 || B == 0) return VB_OK;
+  if (kexp != nullptr) {   // an FP8 cache is filled by the wgmma kernel only
+    if (dtype != VB_BF16 || dropping || dense_mask != nullptr || tune("VB_ATTN_SIMT", 0) != 0) {
+      set_error("attention: an FP8 KV cache is filled by the bf16 wgmma prefill only (no dropout, no dense mask, not VB_ATTN_SIMT)");
+      return VB_ERR_UNSUPPORTED;
+    }
+    VB_CHECK_ARG(kcache && vcache && vexp, "attention: FP8 cache: kcache, vcache, k_exp and v_exp are all needed");
+    return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start,
+                                  max_seqlen, mask_mode, (bf16 *)out, kcache, vcache, cache_seq_stride, cache_cap, s,
+                                  kexp, vexp);
+  }
   const size_t smem = 4 * 64 * 68 * sizeof(float);
   dim3 grid((max_seqlen + 63) / 64, n_head, B);
   if (dtype == VB_F32) {
@@ -206,7 +218,7 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
                               (float *)kcache, (float *)vcache, cache_seq_stride, cache_cap, dense_mask, dense_ld, dc);
   } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && tune("VB_ATTN_SIMT", 0) == 0) {
     return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
-                                  mask_mode, (bf16 *)out, (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, s);
+                                  mask_mode, (bf16 *)out, kcache, vcache, cache_seq_stride, cache_cap, s);
   } else if (dtype == VB_BF16) {
     auto k = attn_varlen_simt_kernel<bf16>;
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -432,14 +444,35 @@ attn_decode_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, T *_
 // 8 CTAs per SM (<= 64 registers, which holds U = 4 K / V rows per thread without spilling): the 1,024 CTAs of B=64 x
 // 16 heads are then resident at once on the H100's 132 SMs.  At 7 per SM (U = 8, 72 registers) 100 of them waited for
 // the first wave to drain and then streamed their whole K and V alone.
-template <int U>
+// CT = uint8_t: the FP8 cache (e4m3 rows, exponent bytes kexp / vexp; the fused QKV prologue is required).  A lane
+// then loads 8 bytes (its 8 elements) per row, so U = 8 rows keep the same bytes and registers in flight as U = 4 bf16
+// rows.  The exponents of the chunk come into shared memory by cp.async; 2^e is applied once per row: to the score
+// (K) and to p_j ahead of P.V (V).  The current token's k / v are the unquantized bf16 rows, served from shared
+// memory; split 0 appends their quantized rows.
+template <int U, typename CT>
 __global__ void __launch_bounds__(128, 8)
-attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, bf16 *__restrict__ kcache,
-                   bf16 *__restrict__ vcache, int64_t cache_seq_stride, int cache_cap,
+attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, CT *__restrict__ kcache,
+                   CT *__restrict__ vcache, int64_t cache_seq_stride, int cache_cap,
                    const int32_t *__restrict__ text_len, const int32_t *__restrict__ prompt_len,
                    const int32_t *__restrict__ n_gen, const int32_t *__restrict__ finished,
                    float *__restrict__ out, bf16 *__restrict__ out16,
-                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit) {
+                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
+                   uint8_t *__restrict__ kexp, uint8_t *__restrict__ vexp) {
+  constexpr bool kF8 = sizeof(CT) == 1;
+  using Raw = typename std::conditional<kF8, uint2, uint4>::type;
+  auto ld_raw = [](const CT *p) -> Raw {
+    if constexpr (kF8) return ldg_stream8(p);
+    else return ldg_stream16(p);
+  };
+  auto unpack_raw = [](const Raw &r, float (&f)[8]) {
+    if constexpr (kF8) {
+      kv8_unpack(r, f);
+    } else {
+      Vec16<bf16> v;
+      v.raw = r;
+      v.unpack(f);
+    }
+  };
   // score buffer of the chunk: dynamic shared memory sized by the launch (cache_cap / nsplit keys), so that the
   // kernel's footprint -- and with it the shared-memory carve-out the driver picks, i.e. how much L1 is left to land
   // the ~64 KB of K / V loads an SM keeps in flight -- follows the actual context instead of the 4096-key maximum
@@ -456,8 +489,8 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int d = n_head * HD;
   using T = bf16;
-  T *kb = kcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
-  T *vb_ = vcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
+  CT *kb = kcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
+  CT *vb_ = vcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
   const bool has_new = qp.part != nullptr;
   const int g = lane >> 3, j8 = (lane & 7) * 8;
   // The K rows of earlier tokens and the lengths do not depend on the kernels of THIS step that precede the
@@ -465,7 +498,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   // first K batch is requested ahead of the dependency wait; the generated-token count is read again after
   // the wait and the batch re-requested should it have moved (it cannot when steps are separate graph launches).
   int kv_len, pos, c0, c1, n;
-  uint4 kraw[U];
+  Raw kraw[U];
   auto setup = [&](int n_generated) {
     kv_len = max(1, min(text_len[b] + prompt_len[b] + n_generated, cache_cap));
     pos = kv_len - 1;  // cache row of the current token
@@ -476,7 +509,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
     if (n > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        kraw[u] = ldg_stream16(kb + (int64_t)(c0 + min(u * 16 + warp * 4 + g, n - 1)) * HD + j8);
+        kraw[u] = ld_raw(kb + (int64_t)(c0 + min(u * 16 + warp * 4 + g, n - 1)) * HD + j8);
     }
   };
   // (only with the fused QKV prologue: there the current token's row is served from shared memory; without it the
@@ -498,6 +531,22 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   int n_gen_now;
   asm volatile("ld.global.cg.s32 %0, [%1];" : "=r"(n_gen_now) : "l"(n_gen + b) : "memory");
   if (n_gen_now != n_gen_early) setup(n_gen_now);  // uniform over the CTA
+  // FP8: the chunk's exponent bytes -> shared memory (16-byte cp.async: c0 and cache_cap are multiples of 16), behind
+  // the score buffer; read once the scores are in
+  uint8_t *kes = nullptr, *ves = nullptr;
+  if constexpr (kF8) {
+    const int sc_len = ((cache_cap + nsplit - 1) / nsplit + 32 + 15) & ~15;
+    kes = reinterpret_cast<uint8_t *>(sc + sc_len);
+    ves = kes + sc_len;
+    const int64_t e0 = ((int64_t)b * cache_seq_stride) / HD + (int64_t)h * cache_cap + c0;
+    for (int i = tid; i < (n + 15) / 16; i += 128) {
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(kes + 16 * i)),
+                   "l"(kexp + e0 + 16 * i) : "memory");
+      asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(ves + 16 * i)),
+                   "l"(vexp + e0 + 16 * i) : "memory");
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  }
   if (has_new) {
     // q / k / v of the current token = sum of the projection's split-K partial tiles (+ folded LayerNorm, bias).  All 128
     // threads fetch: thread = (column c of the head, parity of the split), <= 3 splits x 3 columns each in ONE round
@@ -535,9 +584,28 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
       const T k16 = from_f32<T>(a[1]), v16 = from_f32<T>(a[2]);
       knew[tid] = to_f32(k16);  // exactly what later steps will read back from the cache
       vnew[tid] = to_f32(v16);
-      if (sp == 0) {
+      if constexpr (kF8) {   // the rows' max |.| over the head's 64 columns (warps 0 and 1)
+        const float ak = warp_max(fabsf(to_f32(k16))), av = warp_max(fabsf(to_f32(v16)));
+        if (lane == 0) {
+          wred[warp] = ak;
+          wred[2 + warp] = av;
+        }
+      } else if (sp == 0) {
         kb[(int64_t)pos * HD + tid] = k16;
         vb_[(int64_t)pos * HD + tid] = v16;
+      }
+    }
+    if constexpr (kF8) {
+      __syncthreads();
+      if (hf == 0 && sp == 0) {   // append the quantized rows and their exponents
+        const int ek = kv8_exp_biased(fmaxf(wred[0], wred[1])), ev = kv8_exp_biased(fmaxf(wred[2], wred[3]));
+        kb[(int64_t)pos * HD + tid] = kv8_quant(knew[tid], ek);
+        vb_[(int64_t)pos * HD + tid] = kv8_quant(vnew[tid], ev);
+        if (tid == 0) {
+          const int64_t e0 = ((int64_t)b * cache_seq_stride) / HD + (int64_t)h * cache_cap + pos;
+          kexp[e0] = (uint8_t)ek;
+          vexp[e0] = (uint8_t)ev;
+        }
       }
     }
   } else if (tid < HD) {
@@ -555,15 +623,13 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
     if (base > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        kraw[u] = ldg_stream16(kb + (int64_t)(c0 + min(base + u * 16 + warp * 4 + g, n - 1)) * HD + j8);
+        kraw[u] = ld_raw(kb + (int64_t)(c0 + min(base + u * 16 + warp * 4 + g, n - 1)) * HD + j8);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int key = base + u * 16 + warp * 4 + g;
-      Vec16<bf16> v;
-      v.raw = kraw[u];
       float kf[8];
-      v.unpack(kf);
+      unpack_raw(kraw[u], kf);
       float dot = 0.f;
 #pragma unroll
       for (int i = 0; i < 8; ++i) dot = fmaf(qf[i], kf[i], dot);
@@ -572,16 +638,16 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
       dot += __shfl_xor_sync(0xffffffffu, dot, 1);
       if ((lane & 7) == 0 && key < n && !(new_here && c0 + key == pos)) {
         sc[key] = dot;
-        lmax = fmaxf(lmax, dot);
+        if constexpr (!kF8) lmax = fmaxf(lmax, dot);
       }
     }
   }
   // first batch of V rows in flight across the block softmax
   const int eg = (tid & 7) * 8, jl = tid >> 3;
-  uint4 vraw[U];
+  Raw vraw[U];
   if (n > 0) {
 #pragma unroll
-    for (int u = 0; u < U; ++u) vraw[u] = ldg_stream16(vb_ + (int64_t)(c0 + min(u * 16 + jl, n - 1)) * HD + eg);
+    for (int u = 0; u < U; ++u) vraw[u] = ld_raw(vb_ + (int64_t)(c0 + min(u * 16 + jl, n - 1)) * HD + eg);
   }
   if (new_here && warp == 0) {  // score of the current token from the shared-memory key (never from the cache)
     float dot = 0.f;
@@ -594,7 +660,17 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
     dot += __shfl_xor_sync(0xffffffffu, dot, 1);
     if (lane == 0) {
       sc[pos - c0] = dot;
-      lmax = fmaxf(lmax, dot);
+      if constexpr (!kF8) lmax = fmaxf(lmax, dot);
+    }
+  }
+  if constexpr (kF8) {   // the scores of the cached keys times 2^e_k (the current token's is exact as it stands)
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    __syncthreads();
+    for (int i = tid; i < n; i += 128) {
+      float sv = sc[i];
+      if (!(new_here && c0 + i == pos)) sv *= kv8_scale(kes[i]);
+      sc[i] = sv;
+      lmax = fmaxf(lmax, sv);
     }
   }
   lmax = warp_max(lmax);
@@ -604,7 +680,8 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   float lsum = 0.f;
   for (int i = tid; i < n; i += 128) {
     const float p = expf(sc[i] - m);
-    sc[i] = p;
+    if constexpr (kF8) sc[i] = (new_here && c0 + i == pos) ? p : p * kv8_scale(ves[i]);   // p_j 2^e_v for P.V
+    else sc[i] = p;
     lsum += p;
   }
   lsum = warp_sum(lsum);
@@ -620,16 +697,14 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
     if (base > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        vraw[u] = ldg_stream16(vb_ + (int64_t)(c0 + min(base + u * 16 + jl, n - 1)) * HD + eg);
+        vraw[u] = ld_raw(vb_ + (int64_t)(c0 + min(base + u * 16 + jl, n - 1)) * HD + eg);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int key = base + u * 16 + jl;
       const float pv = (key < n && !(new_here && c0 + key == pos)) ? sc[min(key, n - 1)] : 0.f;
-      Vec16<bf16> v;
-      v.raw = vraw[u];
       float vf[8];
-      v.unpack(vf);
+      unpack_raw(vraw[u], vf);
 #pragma unroll
       for (int i = 0; i < 8; ++i) acc[i] = fmaf(pv, vf[i], acc[i]);
     }
@@ -710,7 +785,36 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
   float *part_ml = part_o + (size_t)B * n_head * ns * HD;
   const QkvPartials qp{qkv.part, qkv.bias, qkv.splits, qkv.ldp, qkv.fold};
   dim3 grid(n_head, B, ns);
-  if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
+  if (dtype == VB_E4M3) {
+    if (tune("VB_ATTN_DECODE_1PASS", 0) != 0) {
+      set_error("attn_decode: VB_ATTN_DECODE_1PASS has no FP8-cache variant");
+      return VB_ERR_UNSUPPORTED;
+    }
+    VB_CHECK_ARG(qkv.part != nullptr && kv.kexp != nullptr && kv.vexp != nullptr && cache_cap % 16 == 0,
+                 "attn_decode: the FP8 cache needs the fused QKV prologue, exponent arrays and cache_cap %% 16 == 0");
+    // score buffer as for bf16 (rounded to 16 floats), then the chunk's K and V exponent bytes
+    const int sc_len = ((cache_cap + ns - 1) / ns + 32 + 15) & ~15;
+    const size_t smem = align_up((size_t)sc_len * (sizeof(float) + 2), 1024);
+    auto k = attn_decode_2phase_pf_kernel<8, uint8_t>;
+    static int carve_f8[64];
+    static bool carve_f8_init = false;
+    if (!carve_f8_init) {
+      for (int i = 0; i < 64; ++i) carve_f8[i] = -2;
+      carve_f8_init = true;
+    }
+    int dev = 0;
+    cudaGetDevice(&dev);
+    const int carve = tune("VB_ATTN_CARVEOUT", 72);
+    if (carve_f8[dev & 63] != carve) {
+      const int want = carve >= 0 ? carve : (int)cudaSharedmemCarveoutDefault;
+      if (carve >= 0 || carve_f8[dev & 63] != -2)
+        VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, want));
+      carve_f8[dev & 63] = carve;
+    }
+    VB_CUDA(launch_kernel(k, grid, dim3(128), smem, s, pdl, (const float *)kv.q, qp, n_head, (uint8_t *)kv.kcache,
+                          (uint8_t *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len, kv.prompt_len, kv.n_gen,
+                          kv.finished, out, (bf16 *)out16, part_o, part_ml, ns, kv.kexp, kv.vexp));
+  } else if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
     if (dtype == VB_F32)
       VB_CUDA(launch_kernel(attn_decode_kernel<float>, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qp, n_head,
                             (float *)kv.kcache, (float *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
@@ -737,12 +841,13 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
     if (carve_set[dev & 63] != carve) {
       const int want = carve >= 0 ? carve : (int)cudaSharedmemCarveoutDefault;
       if (carve >= 0 || carve_set[dev & 63] != -2)
-        VB_CUDA(cudaFuncSetAttribute(attn_decode_2phase_pf_kernel<4>, cudaFuncAttributePreferredSharedMemoryCarveout, want));
+        VB_CUDA(cudaFuncSetAttribute(attn_decode_2phase_pf_kernel<4, bf16>, cudaFuncAttributePreferredSharedMemoryCarveout, want));
       carve_set[dev & 63] = carve;
     }
-    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<4>, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q, qp,
-                          n_head, (bf16 *)kv.kcache, (bf16 *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
-                          kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns));
+    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<4, bf16>, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q,
+                          qp, n_head, (bf16 *)kv.kcache, (bf16 *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
+                          kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns,
+                          (uint8_t *)nullptr, (uint8_t *)nullptr));
   }
   count_launch();
   if (ns > 1) {

@@ -102,11 +102,14 @@ __device__ __forceinline__ void online_softmax(float (&s)[32], int j0, int t, co
   l_b = l_b * corr_b + rs_b;
 }
 
+// kF8: the KV cache is the FP8 one (include/valle_b200.h, vb_decoder_forward_kv8): kcache / vcache hold e4m3 bytes and
+// kexp / vexp the rows' exponents; the attention itself computes on the bf16 tiles either way
+template <bool kF8>
 __global__ void __launch_bounds__(kThreads, 2)
 attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
                   const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens, int seg1_start,
                   int mask_mode, bf16 *__restrict__ out, bf16 *__restrict__ kcache, bf16 *__restrict__ vcache,
-                  int64_t cache_seq_stride, int cache_cap) {
+                  int64_t cache_seq_stride, int cache_cap, uint8_t *__restrict__ kexp, uint8_t *__restrict__ vexp) {
   const int b = blockIdx.z, h = blockIdx.y;
   const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
   const int q0 = blockIdx.x * BQ;
@@ -190,15 +193,59 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
   auto fill_cache = [&](int j0, const uint8_t *sk) {
     if (kcache == nullptr || j0 != q0 + half * 64) return;
     const uint8_t *sv = sk + kBoxBytes;
+    if constexpr (kF8) {
+      // 8 consecutive lanes hold one row (16 bytes = 8 bf16 each): the row's max |.| is one 8-lane shuffle reduction
+      uint8_t *kc8 = reinterpret_cast<uint8_t *>(kcache), *vc8 = reinterpret_cast<uint8_t *>(vcache);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int idx = t + i * 128;
-      const int r = idx >> 3, c = idx & 7;
-      if (j0 + r < L) {
-        const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + j0 + r) * HD + c * 8;
+      for (int i = 0; i < 4; ++i) {
+        const int idx = t + i * 128;
+        const int r = idx >> 3, c = idx & 7;
         const int so = r * 128 + ((c ^ (r & 7)) << 4);
-        *reinterpret_cast<uint4 *>(kcache + off) = *reinterpret_cast<const uint4 *>(sk + so);
-        *reinterpret_cast<uint4 *>(vcache + off) = *reinterpret_cast<const uint4 *>(sv + so);
+        Vec16<bf16> kv, vv;
+        kv.raw = *reinterpret_cast<const uint4 *>(sk + so);
+        vv.raw = *reinterpret_cast<const uint4 *>(sv + so);
+        float kf[8], vf[8];
+        kv.unpack(kf);
+        vv.unpack(vf);
+        float ak = 0.f, av = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          ak = fmaxf(ak, fabsf(kf[j]));
+          av = fmaxf(av, fabsf(vf[j]));
+        }
+#pragma unroll
+        for (int o = 4; o > 0; o >>= 1) {
+          ak = fmaxf(ak, __shfl_xor_sync(0xffffffffu, ak, o));
+          av = fmaxf(av, __shfl_xor_sync(0xffffffffu, av, o));
+        }
+        if (j0 + r < L) {
+          const int ek = kv8_exp_biased(ak), ev = kv8_exp_biased(av);
+          uint32_t kq[2] = {0u, 0u}, vq[2] = {0u, 0u};
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            kq[j >> 2] |= (uint32_t)kv8_quant(kf[j], ek) << (8 * (j & 3));
+            vq[j >> 2] |= (uint32_t)kv8_quant(vf[j], ev) << (8 * (j & 3));
+          }
+          const int64_t row = (int64_t)b * (cache_seq_stride / HD) + (int64_t)h * cache_cap + j0 + r;
+          *reinterpret_cast<uint2 *>(kc8 + row * HD + c * 8) = make_uint2(kq[0], kq[1]);
+          *reinterpret_cast<uint2 *>(vc8 + row * HD + c * 8) = make_uint2(vq[0], vq[1]);
+          if (c == 0) {
+            kexp[row] = (uint8_t)ek;
+            vexp[row] = (uint8_t)ev;
+          }
+        }
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const int idx = t + i * 128;
+        const int r = idx >> 3, c = idx & 7;
+        if (j0 + r < L) {
+          const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + j0 + r) * HD + c * 8;
+          const int so = r * 128 + ((c ^ (r & 7)) << 4);
+          *reinterpret_cast<uint4 *>(kcache + off) = *reinterpret_cast<const uint4 *>(sk + so);
+          *reinterpret_cast<uint4 *>(vcache + off) = *reinterpret_cast<const uint4 *>(sv + so);
+        }
       }
     }
   };
@@ -271,19 +318,33 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
 
 int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
                            const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, bf16 *out, bf16 *kcache, bf16 *vcache, int64_t cache_seq_stride,
-                           int cache_cap, cudaStream_t s) {
+                           int mask_mode, bf16 *out, void *kcache, void *vcache, int64_t cache_seq_stride,
+                           int cache_cap, cudaStream_t s, uint8_t *kexp, uint8_t *vexp) {
   if (M == 0 || B == 0) return VB_OK;
   VB_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0, "wgmma attention: qkv must be 16-byte aligned");
   CUtensorMap tm;
   VB_TRY(tc::make_tmap(&tm, qkv, M, 3 * n_head * fa3::HD, 3 * (int64_t)n_head * fa3::HD, 64));
+  dim3 grid((max_seqlen + fa3::BQ - 1) / fa3::BQ, n_head, B);
+  if (kexp != nullptr) {
+    static PerDeviceOnce once8;
+    if (once8.first())
+      VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   fa3::kSmemBytes));
+    fa3::attn_wgmma_kernel<true><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(
+        tm, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, out, (bf16 *)kcache, (bf16 *)vcache,
+        cache_seq_stride, cache_cap, kexp, vexp);
+    VB_LAUNCH_CHECK();
+    return VB_OK;
+  }
   static PerDeviceOnce once;
   if (once.first())
-    VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, fa3::kSmemBytes));
-  dim3 grid((max_seqlen + fa3::BQ - 1) / fa3::BQ, n_head, B);
-  fa3::attn_wgmma_kernel<<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(tm, n_head, cu_seqlens, text_lens, seg1_lens,
-                                                                      seg1_start, mask_mode, out, kcache, vcache,
-                                                                      cache_seq_stride, cache_cap);
+    VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 fa3::kSmemBytes));
+  fa3::attn_wgmma_kernel<false><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(tm, n_head, cu_seqlens, text_lens,
+                                                                             seg1_lens, seg1_start, mask_mode, out,
+                                                                             (bf16 *)kcache, (bf16 *)vcache,
+                                                                             cache_seq_stride, cache_cap, nullptr,
+                                                                             nullptr);
   VB_LAUNCH_CHECK();
   return VB_OK;
 }

@@ -1,6 +1,8 @@
 // Shared helpers for the sm_90a kernels of libvalle_b200.so.
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -120,6 +122,44 @@ __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// ---- FP8 (e4m3) KV cache rows, one power-of-two scale per 64-element row (include/valle_b200.h,
+//      vb_decoder_forward_kv8).  Exponents travel biased: eb = e + 127, eb in [0, 254].
+// eb of a row with max |r| = a: the smallest integer e with a <= 448 * 2^e (frexpf: a = m 2^x, m in [0.5, 1); e = x - 9
+// when m <= 0.875 = 448 / 2^9, else x - 8), clamped to [-127, 127]; an all-zero row gets e = -127
+__device__ __forceinline__ int kv8_exp_biased(float a) {
+  if (!(a > 0.f)) return 0;
+  int x;
+  const float m = frexpf(a, &x);
+  const int e = m <= 0.875f ? x - 9 : x - 8;
+  return min(max(e, -127), 127) + 127;
+}
+// 2^(eb - 127) in fp32 (eb = 0: the subnormal 2^-127); 2^-(eb - 127) = kv8_scale(254 - eb)
+__device__ __forceinline__ float kv8_scale(int eb) { return __int_as_float(eb > 0 ? eb << 23 : 0x00400000); }
+// cvt.rn.satfinite.e4m3 of r * 2^-e (the product is exact: a power-of-two scale)
+__device__ __forceinline__ uint8_t kv8_quant(float r, int eb) {
+  return (uint8_t)__nv_cvt_float_to_fp8(r * kv8_scale(254 - eb), __NV_SATFINITE, __NV_E4M3);
+}
+// 8 e4m3 bytes -> 8 floats (exact: e4m3 -> f16 -> f32)
+__device__ __forceinline__ void kv8_unpack(uint2 raw, float (&f)[8]) {
+  const uint32_t w[2] = {raw.x, raw.y};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i] >> (16 * j)), __NV_E4M3);
+      const float2 p = __half22float2(__half2(hr));
+      f[4 * i + 2 * j] = p.x;
+      f[4 * i + 2 * j + 1] = p.y;
+    }
+  }
+}
+// streaming 8-byte global load (half a bf16 row chunk: 8 e4m3 elements)
+__device__ __forceinline__ uint2 ldg_stream8(const void *p) {
+  uint2 r;
+  asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+  return r;
 }
 
 // ---- grid-wide barrier of a cooperative launch (every CTA resident).  `ctr` is a monotonic arrival counter zeroed

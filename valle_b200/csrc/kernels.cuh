@@ -75,6 +75,7 @@ struct KvPrefetch {
   int B, H, cap, row_bytes;   // row_bytes = 64 * element size
   const int32_t *text_len, *prompt_len, *n_gen;
   int row_lo, row_hi;
+  const uint8_t *kexp, *vexp; // FP8 cache: the exponent arrays of the target layer ([B, H, cap]), else nullptr
 };
 // worker = one warp; `n_workers` warps of the grid share the streams.  Lane i of a warp fetches the lengths of the
 // warp's i-th stream up front (the three dependent global loads per stream would otherwise serialise the loop).
@@ -105,6 +106,13 @@ __device__ __forceinline__ void kv_prefetch(const KvPrefetch &pf, int worker, in
                     ((int64_t)h * pf.cap + r_lo) * pf.row_bytes;
     const int lines = ((r_hi - r_lo) * pf.row_bytes) >> 7;  // 128-byte lines
     for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + ((int64_t)l << 7)));
+    if (pf.kexp != nullptr && lane == 0 && r_hi > r_lo) {  // the rows' exponent bytes: one or two lines
+      const char *e = (const char *)((sidx & 1) ? pf.vexp : pf.kexp) + (int64_t)b * (pf.seq_stride_bytes >> 6) +
+                      (int64_t)h * pf.cap;
+      const int64_t l0 = (r_lo + ((int64_t)(uintptr_t)e & 127)) >> 7, l1 = (r_hi - 1 + ((int64_t)(uintptr_t)e & 127)) >> 7;
+      const char *e0 = (const char *)((uintptr_t)e & ~(uintptr_t)127);
+      for (int64_t l = l0; l <= l1; ++l) asm volatile("prefetch.global.L2 [%0];" ::"l"(e0 + (l << 7)));
+    }
   }
 }
 
@@ -121,6 +129,7 @@ struct QkvScatter {
   int cache_cap;
   const int32_t *text_len, *prompt_len, *n_gen;
   const int32_t *finished;  // NULL or [B]: rows that have stopped keep their cache untouched
+  uint8_t *kexp = nullptr, *vexp = nullptr;  // FP8 cache (e4m3 kcache / vcache): this layer's exponent arrays [B, H, cap]
 };
 
 // gemm_simt.cu
@@ -200,14 +209,17 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
                             const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
                             int seg1_start, int max_seqlen, int mask_mode, void *out, void *kcache, void *vcache,
                             int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
-                            cudaStream_t s, const DropCfg *drop = nullptr);
-// attention_wgmma.cu (bf16 flash attention on wgmma / TMA; fills the KV cache when kcache != nullptr)
+                            cudaStream_t s, const DropCfg *drop = nullptr, uint8_t *kexp = nullptr,
+                            uint8_t *vexp = nullptr);
+// attention_wgmma.cu (bf16 flash attention on wgmma / TMA; fills the KV cache when kcache != nullptr: bf16, or with
+// kexp != nullptr the FP8 cache, e4m3 rows + exponent bytes)
 int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
                            const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, bf16 *out, bf16 *kcache, bf16 *vcache, int64_t cache_seq_stride,
-                           int cache_cap, cudaStream_t s);
+                           int mask_mode, bf16 *out, void *kcache, void *vcache, int64_t cache_seq_stride,
+                           int cache_cap, cudaStream_t s, uint8_t *kexp = nullptr, uint8_t *vexp = nullptr);
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
-// the current token's q, k, v (kv.q, or pending in qkv) against the layer's caches kv.kcache / kv.vcache
+// the current token's q, k, v (kv.q, or pending in qkv) against the layer's caches kv.kcache / kv.vcache.  dtype
+// VB_E4M3: the FP8 cache (kv.kexp / kv.vexp); q, k, v must then be pending in qkv
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
                        void *workspace, bool pdl, cudaStream_t s);
 

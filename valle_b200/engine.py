@@ -67,13 +67,14 @@ class EngineStats:
 
 
 class _ArBuffers:
-    """Persistent device state for the AR loop at one (B, cache_cap, tok_stride) shape, plus the CUDA graphs of
-    decode steps captured on it."""
+    """Persistent device state for the AR loop at one (B, cache_cap, tok_stride, cache dtype) shape, plus the CUDA
+    graphs of decode steps captured on it.  kv_dtype torch.float8_e4m3fn: the FP8 cache (e4m3 rows and one exponent
+    byte per cached row, include/valle_b200.h vb_decoder_forward_kv8); None: the engine dtype."""
 
-    def __init__(self, eng: "ValleEngine", B: int, cap: int, tok_stride: int):
+    def __init__(self, eng: "ValleEngine", B: int, cap: int, tok_stride: int, kv_dtype: Optional[torch.dtype] = None):
         dev, d = eng.device, eng.d
         nd = eng.ar
-        self.B, self.cap, self.tok_stride = B, cap, tok_stride
+        self.B, self.cap, self.tok_stride, self.kv_dtype = B, cap, tok_stride, kv_dtype
         i32 = dict(dtype=torch.int32, device=dev)
         self.text_len = torch.zeros(B, **i32)
         self.prompt_len = torch.zeros(B, **i32)
@@ -84,8 +85,12 @@ class _ArBuffers:
         self.x_cur = torch.zeros((B, d), dtype=torch.float32, device=dev)
         self.ldl = (eng.n_vocab + 3) // 4 * 4
         self.logits = torch.zeros((B, self.ldl), dtype=torch.float32, device=dev)
-        self.kcache = torch.zeros((nd.n_layer, B, nd.H, cap, 64), dtype=eng.dtype, device=dev)
+        self.kcache = torch.zeros((nd.n_layer, B, nd.H, cap, 64), dtype=kv_dtype or eng.dtype, device=dev)
         self.vcache = torch.zeros_like(self.kcache)
+        fp8 = kv_dtype == torch.float8_e4m3fn
+        #: FP8 cache: the biased exponent (e + 127) of every cached row, [n_layer, B, H, cap] uint8
+        self.k_exp = torch.zeros((nd.n_layer, B, nd.H, cap), dtype=torch.uint8, device=dev) if fp8 else None
+        self.v_exp = torch.zeros_like(self.k_exp) if fp8 else None
         # seeded device sampler, per row (uint64 seeds stored as their int64 bit patterns)
         self.sample_seed = torch.zeros(B, dtype=torch.int64, device=dev)
         self.top_k = torch.zeros(B, **i32)
@@ -99,6 +104,8 @@ class _ArBuffers:
         st.cache_layer_stride, st.cache_seq_stride, st.cache_cap = self.kcache.stride(0), self.kcache.stride(1), cap
         st.sample_seed, st.top_k = self.sample_seed.data_ptr(), self.top_k.data_ptr()
         st.temperature = self.temperature.data_ptr()
+        if fp8:
+            st.kv_dtype, st.k_exp, st.v_exp = L.VB_E4M3, self.k_exp.data_ptr(), self.v_exp.data_ptr()
         self.st = st
         nbytes = eng.lib.vb_ar_step_workspace(C.byref(nd.desc), B, cap)
         self.ws = torch.zeros(nbytes, dtype=torch.uint8, device=dev)
@@ -294,13 +301,24 @@ class ValleEngine:
             h.fold = self.ar_head_fold
         return h
 
-    def _buffers(self, B: int, cap: int, tok_stride: int) -> _ArBuffers:
-        key = (B, cap, tok_stride)
+    def kv_cache_dtype(self) -> Optional[torch.dtype]:
+        """the model's `kv_cache_dtype` (None: the cache holds the engine dtype), validated against the engine dtype"""
+        kv = getattr(self.model, "kv_cache_dtype", None)
+        if kv is None:
+            return None
+        if kv != torch.float8_e4m3fn:
+            raise ValueError(f"kv_cache_dtype={kv}: only None (the engine dtype) and torch.float8_e4m3fn are supported")
+        if self.dtype != torch.bfloat16:
+            raise ValueError(f"kv_cache_dtype=torch.float8_e4m3fn needs engine_dtype=torch.bfloat16 (got {self.dtype})")
+        return kv
+
+    def _buffers(self, B: int, cap: int, tok_stride: int, kv_dtype: Optional[torch.dtype] = None) -> _ArBuffers:
+        key = (B, cap, tok_stride, kv_dtype)
         b = self._bufs.get(key)
         if b is None:
             if len(self._bufs) > 4:
                 self._bufs.clear()
-            b = _ArBuffers(self, B, cap, tok_stride)
+            b = _ArBuffers(self, B, cap, tok_stride, kv_dtype)
             self._bufs[key] = b
         return b
 
@@ -329,6 +347,7 @@ class ValleEngine:
         m, dev, d, Q = self.model, self.device, self.d, self.Q
         B = len(texts)
         assert B == len(prompts) and B >= 1
+        kv_dtype = self.kv_cache_dtype()
         sampler = None
         if seed is not None:
             if self.sample_on_host:
@@ -418,7 +437,7 @@ class ValleEngine:
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         ev[0].record()
         # ---- AR prefill (valle.py:995-997,1013-1016) ----
-        buf = self._buffers(B, cap, tok_stride)
+        buf = self._buffers(B, cap, tok_stride, kv_dtype)
         buf.text_len.copy_(S_d)
         buf.prompt_len.copy_(Tp_d)
         buf.max_new.copy_(capn_d)
@@ -438,7 +457,8 @@ class ValleEngine:
             self._embed_pe(ar_tok, 1, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, arow_d, apos_d)
         else:
             self._embed_pe(prm_all, Q, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, arow_d, apos_d)
-        self.ar.forward(x, cu_d, B, max(seq_len), L.VB_MASK_VALLE_AR, S_d, None, buf.kcache, buf.vcache, cap)
+        self.ar.forward(x, cu_d, B, max(seq_len), L.VB_MASK_VALLE_AR, S_d, None, buf.kcache, buf.vcache, cap,
+                        k_exp=buf.k_exp, v_exp=buf.v_exp)
         h_last = ops.gather_rows(x, last_d)
         head = self._head(pe_a, 2 if native else int(greedy))
         self._head_ref = head
@@ -576,7 +596,7 @@ class ValleEngine:
     def _replay_steps(self, buf: _ArBuffers, head: L.ArHead, k: int):
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
         draw mode, k))"""
-        key = (head.pe, head.predict_w, head.audio_emb, head.greedy, k)
+        key = (head.pe, head.predict_w, head.audio_emb, head.greedy, buf.kv_dtype, k)
         graphs = buf.graphs
         ent = graphs.get(key)
         if ent is None:

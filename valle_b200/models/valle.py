@@ -149,6 +149,10 @@ class VALLE(nn.Module):
         #: storage/compute type of the engine used by inference(): torch.float32 (bit-exact greedy
         #: parity with the reference) or torch.bfloat16 (tensor-core path)
         self.engine_dtype = torch.float32
+        #: KV cache of the AR decode: None (the engine dtype) or torch.float8_e4m3fn, the opt-in FP8 cache of bf16
+        #: decoding (one power-of-two scale per cached 64-element row; half the cache bytes).  Valid only with
+        #: engine_dtype = torch.bfloat16: generate / inference / inference_batch raise ValueError otherwise.
+        self.kv_cache_dtype: Optional[torch.dtype] = None
 
     # ---- reference helper API (valle.py:294-333) --------------------------------------------
     def stage_parameters(self, stage: int = 1) -> Iterator[nn.Parameter]:
