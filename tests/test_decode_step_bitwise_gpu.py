@@ -5,12 +5,12 @@ clamp) is built through valle_b200.modules.transformer from a torch seed, and ev
 Each case fills vb_ar_state / vb_ar_head directly, runs vb_ar_head_step and then three vb_ar_decode_step calls (with
 greedy = 0 the host's draw is replaced by vb_ar_push_tokens of fixed ids between the calls) and compares with
 tests/golden/decode_step_bits.pt:
-  - SHA-256 of x_cur, logits, tokens, n_gen, finished and both whole KV caches after the last call, and of the logits
-    after every call;
+  - SHA-256 of x_cur, logits, tokens, n_gen, finished and both whole KV caches (with the FP8 cache, both exponent
+    arrays as well) after the last call, and of the logits after every call;
   - the number of library launches of every call.
-The cases cover the LayerNorm-folded, unfolded and post-LN tensor-core chains, the CUDA-core chain (fp32, and bf16
-with VB_DECODE_SIMT), B = 1, 17 and 64 with finished rows, greedy = 0, 1 and 2, and the switches that change what the
-chain launches.  A change to the host-side orchestration that keeps every launch, its arguments and its order passes
+The cases cover the LayerNorm-folded, unfolded and post-LN tensor-core chains on the bf16 and the FP8 cache, the
+CUDA-core chain (fp32, and bf16 with VB_DECODE_SIMT), B = 1, 17 and 64 with finished rows, greedy = 0, 1 and 2, and the
+switches that change what the chain launches.  A change to the host-side orchestration that keeps every launch, its arguments and its order passes
 unchanged.
 
     python tests/test_decode_step_bitwise_gpu.py --record     # rewrite the fixture from the library as built
@@ -28,6 +28,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+import kv_fp8_oracle as K
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -61,6 +63,21 @@ CASES = {
     "simt_b17_g1": ("folded", 17, 1, (6,), (("VB_DECODE_SIMT", 1),)),
     "simt_postln_b64_g2": ("postln", 64, 2, (), (("VB_DECODE_SIMT", 1),)),
 }
+# the FP8 cache (vb_ar_state.kv_dtype = VB_E4M3): the caches start from tests/kv_fp8_oracle.py's quantization of the
+# random bf16 caches, and the exponent arrays are hashed with them
+F8_CASES = {
+    "f8_folded_b1_g1": ("folded", 1, 1, (), ()),
+    "f8_folded_b17_g2": ("folded", 17, 2, (3,), ()),
+    "f8_folded_b64_g0": ("folded", 64, 0, (5, 40), ()),
+    "f8_folded_b64_nopdl": ("folded", 64, 1, (0,), (("VB_NO_PDL", 1),)),
+    "f8_unfolded_b1_g2": ("unfolded", 1, 2, (), ()),
+    "f8_unfolded_b17_g0": ("unfolded", 17, 0, (16,), ()),
+    "f8_unfolded_b64_g1": ("unfolded", 64, 1, (7, 63), ()),
+    "f8_postln_b1_g0": ("postln", 1, 0, (), ()),
+    "f8_postln_b17_g1": ("postln", 17, 1, (2,), ()),
+    "f8_postln_b64_g2": ("postln", 64, 2, (9, 33), ()),
+}
+CASES.update(F8_CASES)
 
 
 def _sha(t):
@@ -135,6 +152,9 @@ def _run(name):
              seed=torch.arange(B, dtype=torch.int64).mul(7919).add(3).to(DEV),
              top_k=torch.randint(1, 60, (B,), generator=g).to(**i32),
              temperature=(0.6 + torch.rand(B, generator=g)).to(DEV))
+    if name in F8_CASES:
+        for c, e in (("kc", "ke"), ("vc", "ve")):
+            t[c], t[e] = (a.to(DEV) for a in K.quantize(t[c].cpu()))
     h_in = torch.randn(B, D, generator=g).to(DEV)
     pushed = torch.randint(0, N_VOCAB - 1, (STEPS + 1, B), generator=g, dtype=torch.int64).to(DEV)
     s = L.ArState()
@@ -144,6 +164,8 @@ def _run(name):
     s.x_cur, s.logits = t["x"].data_ptr(), t["logits"].data_ptr()
     s.kcache, s.vcache = t["kc"].data_ptr(), t["vc"].data_ptr()
     s.cache_layer_stride, s.cache_seq_stride, s.cache_cap = t["kc"].stride(0), t["kc"].stride(1), CAP
+    if name in F8_CASES:
+        s.kv_dtype, s.k_exp, s.v_exp = L.VB_E4M3, t["ke"].data_ptr(), t["ve"].data_ptr()
     s.sample_seed, s.top_k, s.temperature = t["seed"].data_ptr(), t["top_k"].data_ptr(), t["temperature"].data_ptr()
     h = L.ArHead()
     h.predict_w, h.n_vocab, h.eos_id = m["head_w"].data_ptr(), N_VOCAB, EOS
@@ -172,7 +194,7 @@ def _run(name):
                 L.check(lib.vb_ar_push_tokens(C.byref(h), C.byref(s), pushed[step].data_ptr(), D, L.stream_ptr()),
                         "vb_ar_push_tokens")
         torch.cuda.synchronize()
-    for k in ("x", "logits", "tokens", "n_gen", "finished", "kc", "vc"):
+    for k in ("x", "logits", "tokens", "n_gen", "finished", "kc", "vc") + (("ke", "ve") if name in F8_CASES else ()):
         r[k] = _sha(t[k])
     return r
 

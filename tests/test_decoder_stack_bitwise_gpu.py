@@ -3,8 +3,8 @@
 A small stack (d=256, 4 heads, d_ff=1024, 2 layers) is built through valle_b200.modules.transformer from a torch seed,
 and every input is generated on the CPU.  Each case runs the stack through `NativeDecoder.forward` (inference) or
 `autograd.DecoderStack` (training forward + backward) and compares with tests/golden/decoder_stack_bits.pt:
-  - SHA-256 of the stack output, of both whole KV caches (pre-filled with a sentinel), of the input gradient and of
-    the four weight-matrix gradients of every layer;
+  - SHA-256 of the stack output, of both whole KV caches (pre-filled with a sentinel; with the FP8 cache, both
+    exponent arrays as well), of the input gradient and of the four weight-matrix gradients of every layer;
   - the bias, LayerNorm-affine and AdaLN gradients within 1e-5 x the recorded tensor's max-abs: they are summed with
     atomicAdd, so their last bits vary from run to run;
   - the number of library launches of each call.
@@ -66,17 +66,26 @@ def _launches(fn):
 
 
 def _forward(name):
-    """fwd_{pre,post}_{ln_prefill,adaln_nar}_{f32,bf16}: one vb_decoder_forward call"""
+    """fwd_{pre,post}_{ln_prefill,adaln_nar}_{f32,bf16}: one vb_decoder_forward call; fwd_{pre,post}_ln_prefill_f8: one
+    vb_decoder_forward_kv8 call (bf16 stack, FP8 cache)"""
     from valle_b200 import _lib as L
     _, order, norm, shape, dt = name.split("_")
+    f8 = dt == "f8"
     enc, ada = _stack(order == "pre", norm == "adaln", 5)
-    nd = enc.native(DTYPES[dt])
+    nd = enc.native(torch.bfloat16 if f8 else DTYPES[dt])
     g = torch.Generator().manual_seed(6)
     r = {}
+    ke = ve = None
     if shape == "prefill":        # the AR prefill: text + prompt rows per utterance, KV caches filled for decoding
         lens, tl, cap = [40, 23, 61], [9, 5, 17], 64
-        cache = lambda v: torch.full((NL, len(lens), H, cap, D // H), v, dtype=DTYPES[dt], device=DEV)
-        kc, vc = cache(1234.0), cache(-1234.0)
+        rows = (NL, len(lens), H, cap)
+        if f8:                    # sentinel bytes in the e4m3 rows and in the exponent arrays
+            cache = lambda v: torch.full(rows + (D // H,), v, dtype=torch.uint8, device=DEV).view(torch.float8_e4m3fn)
+            kc, vc = cache(0x5A), cache(0xDA)
+            ke, ve = (torch.full(rows, v, dtype=torch.uint8, device=DEV) for v in (0xAB, 0xCD))
+        else:
+            cache = lambda v: torch.full(rows + (D // H,), v, dtype=DTYPES[dt], device=DEV)
+            kc, vc = cache(1234.0), cache(-1234.0)
         mode, tl = L.VB_MASK_VALLE_AR, torch.tensor(tl, dtype=torch.int32, device=DEV)
     else:                         # a NAR pass: whole sequences, AdaLN rows of one stage
         lens, kc, vc, cap = [57, 12, 90], None, None, 0
@@ -84,10 +93,13 @@ def _forward(name):
     x = torch.randn(sum(lens), D, generator=g).to(DEV)
     cu = torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), dtype=torch.int32, device=DEV)
     ada = ada.to(DEV) if ada is not None else None
-    _, r["launches"] = _launches(lambda: nd.forward(x, cu, len(lens), max(lens), mode, tl, ada, kc, vc, cap))
+    _, r["launches"] = _launches(lambda: nd.forward(x, cu, len(lens), max(lens), mode, tl, ada, kc, vc, cap,
+                                                    k_exp=ke, v_exp=ve))
     r["out"] = _sha(x)
     if kc is not None:
         r["kcache"], r["vcache"] = _sha(kc), _sha(vc)
+    if ke is not None:
+        r["k_exp"], r["v_exp"] = _sha(ke), _sha(ve)
     return r
 
 
@@ -130,6 +142,7 @@ def _train(name):
 
 
 CASES = ([f"fwd_{o}_{k}_{dt}" for o in ("pre", "post") for k in ("ln_prefill", "adaln_nar") for dt in DTYPES] +
+         [f"fwd_{o}_ln_prefill_f8" for o in ("pre", "post")] +
          [f"train_{o}_{n}_{dt}_{p}" for o in ("pre", "post") for n in ("ln", "adaln") for dt in DTYPES
           for p in ("p0", "p01")])
 

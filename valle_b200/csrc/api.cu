@@ -175,8 +175,6 @@ VB_API int vb_decoder_set_decode_fold(vb_decoder_t dec, const vb_ln_fold *qkv, c
   return VB_OK;
 }
 
-static size_t elem_size(int dtype) { return dtype == VB_E4M3 ? 1 : dtype == VB_BF16 ? 2 : 4; }
-
 // ------------------------------------------------------------------------------------------
 // Decoder stack: the forward of inference and training, and the backward pass
 // ------------------------------------------------------------------------------------------
@@ -255,20 +253,18 @@ T *ada_row(T *wb, int l, int k, int d) {
 // (l << 2) | site, regenerated by the backward
 DropCfg layer_drop(float p, uint64_t seed, int l, int site) { return make_drop(p, seed, (uint32_t)(l << 2) | (uint32_t)site); }
 
-// The layer loop of vb_decoder_forward and vb_decoder_forward_train.  slots(l): layer l's activation slots; kcache /
-// vcache: null or the caches the attention fills (kexp / vexp non-null: the FP8 cache and its exponents); sub: the fp32 [M, d] scratch of the sub-layer outputs when
-// dropout_p > 0.  Pre-LN (transformer.py:297-302): x += SA(norm1(x)); x += FF(norm2(x)).  Post-LN (:303-308):
+// The layer loop of vb_decoder_forward and vb_decoder_forward_train.  slots(l): layer l's activation slots; cache:
+// the whole KV cache the attention fills (cache.k == nullptr: none); sub: the fp32 [M, d] scratch of the sub-layer
+// outputs when dropout_p > 0.  Pre-LN (transformer.py:297-302): x += SA(norm1(x)); x += FF(norm2(x)).  Post-LN (:303-308):
 // x = norm1(x + SA(x)); x = norm2(x + FF(x)); a post-norm writes the normalised rows back into x and into the
 // storage-dtype operand of the next GEMM, and layer 0 reads a plain cast.
 template <class Slots>
 int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32_t *cu_seqlens, const int32_t *text_lens,
                   const int32_t *seg1_lens, int seg1_start, int max_seqlen, int mask_mode, const float *ada_wb,
-                  Slots slots, void *kcache, void *vcache, int64_t cache_layer_stride, int64_t cache_seq_stride,
-                  int cache_cap, float *sub, float dropout_p, uint64_t dropout_seed, cudaStream_t s,
-                  uint8_t *kexp = nullptr, uint8_t *vexp = nullptr) {
+                  Slots slots, const KvCache &cache, int64_t cache_layer_stride, float *sub, float dropout_p,
+                  uint64_t dropout_seed, cudaStream_t s) {
   const vb_decoder_desc &D = dec->desc;
   const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
-  const size_t ts = elem_size(dt);
   const vb_stream_t stream = (vb_stream_t)s;
   if (!D.norm_first) VB_TRY(launch_cast_from_f32(x, slots(0).xn1, dt, M * d, s));
   for (int l = 0; l < D.n_layer; ++l) {
@@ -293,15 +289,10 @@ int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32
     auto attn = [&]() -> int {
       VB_TRY(vb_linear(sv.xn1, dt, d, P.in_proj_w, dt, P.in_proj_b, sv.qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE, nullptr,
                        0, stream));
-      const size_t cs = kexp ? 1 : ts;   // cache element size
-      void *kc = kcache ? (char *)kcache + (size_t)l * cache_layer_stride * cs : nullptr;
-      void *vc = vcache ? (char *)vcache + (size_t)l * cache_layer_stride * cs : nullptr;
-      uint8_t *ke = kexp ? kexp + (size_t)l * cache_layer_stride / 64 : nullptr;
-      uint8_t *ve = vexp ? vexp + (size_t)l * cache_layer_stride / 64 : nullptr;
       const DropCfg dc = layer_drop(dropout_p, dropout_seed, l, 0);
       VB_TRY(launch_attention_varlen(sv.qkv, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
-                                     seg1_start, max_seqlen, mask_mode, sv.att, kc, vc, cache_seq_stride, cache_cap,
-                                     nullptr, 0, s, &dc, ke, ve));
+                                     seg1_start, max_seqlen, mask_mode, sv.att,
+                                     kv_cache_layer(cache, cache_layer_stride, l), nullptr, 0, s, &dc));
       return residual(sv.att, d, P.out_proj_w, P.out_proj_b, 1);
     };
     auto ffn = [&]() -> int {
@@ -356,6 +347,21 @@ VB_API size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t 
   return carved_bytes(carve_forward_ws, *desc, M);
 }
 
+// the body of vb_decoder_forward and vb_decoder_forward_kv8 (fn: the entry point's name, for the error message)
+static int decoder_forward(const char *fn, vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                           int mask_mode, const float *ada_wb, const KvCache &cache, int64_t cache_layer_stride,
+                           void *workspace, size_t workspace_bytes, vb_stream_t stream) {
+  const vb_decoder_desc &D = dec->desc;
+  VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M), "%s: workspace too small (%zu < %zu)", fn,
+               workspace_bytes, vb_decoder_forward_workspace(&D, M));
+  if (M == 0) return VB_OK;
+  Carve c(workspace);
+  const LayerSave ws = carve_forward_ws(c, D, M);
+  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
+                       [&](int) { return ws; }, cache, cache_layer_stride, nullptr, 0.f, 0, (cudaStream_t)stream);
+}
+
 VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
                                   const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start,
                                   int max_seqlen, int mask_mode,
@@ -363,16 +369,9 @@ VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, cons
                                   int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
                                   void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && x && cu_seqlens, "vb_decoder_forward: null argument");
-  const vb_decoder_desc &D = dec->desc;
-  VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M),
-               "vb_decoder_forward: workspace too small (%zu < %zu)", workspace_bytes,
-               vb_decoder_forward_workspace(&D, M));
-  if (M == 0) return VB_OK;
-  Carve c(workspace);
-  const LayerSave ws = carve_forward_ws(c, D, M);
-  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
-                       [&](int) { return ws; }, kcache, vcache, cache_layer_stride, cache_seq_stride, cache_cap,
-                       nullptr, 0.f, 0, (cudaStream_t)stream);
+  const KvCache cache{kcache, vcache, nullptr, nullptr, cache_seq_stride, cache_cap, (int)elem_size(dec->desc.wdtype)};
+  return decoder_forward("vb_decoder_forward", dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
+                         mask_mode, ada_wb, cache, cache_layer_stride, workspace, workspace_bytes, stream);
 }
 
 // the FP8 cache's exponent rows are read 16 bytes at a time (cp.async in the decode attention): every (layer, utterance,
@@ -388,21 +387,16 @@ VB_API int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, 
                                   uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
                                   void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && x && cu_seqlens && kcache && vcache && k_exp && v_exp, "vb_decoder_forward_kv8: null argument");
-  const vb_decoder_desc &D = dec->desc;
-  if (D.wdtype != VB_BF16) {
+  if (dec->desc.wdtype != VB_BF16) {
     set_error("vb_decoder_forward_kv8: the FP8 KV cache needs a bf16 decoder");
     return VB_ERR_UNSUPPORTED;
   }
   VB_CHECK_ARG(kv8_layout_ok(k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap),
                "vb_decoder_forward_kv8: FP8 cache: strides must be multiples of 1024, cache_cap a multiple of 16 and "
                "k_exp / v_exp 16-byte aligned");
-  VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M), "vb_decoder_forward_kv8: workspace too small");
-  if (M == 0) return VB_OK;
-  Carve c(workspace);
-  const LayerSave ws = carve_forward_ws(c, D, M);
-  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
-                       [&](int) { return ws; }, kcache, vcache, cache_layer_stride, cache_seq_stride, cache_cap,
-                       nullptr, 0.f, 0, (cudaStream_t)stream, k_exp, v_exp);
+  const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap, (int)elem_size(VB_E4M3)};
+  return decoder_forward("vb_decoder_forward_kv8", dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start,
+                         max_seqlen, mask_mode, ada_wb, cache, cache_layer_stride, workspace, workspace_bytes, stream);
 }
 
 VB_API size_t vb_decoder_train_save_bytes(const vb_decoder_desc *desc, int64_t M) {
@@ -421,8 +415,8 @@ VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B
   Carve c(save);
   float *sub = carve_train_save(c, D, M);
   return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
-                       [&](int l) { return layer_save(D, M, save, l); }, nullptr, nullptr, 0, 0, 0, sub, dropout_p,
-                       dropout_seed, (cudaStream_t)stream);
+                       [&](int l) { return layer_save(D, M, save, l); }, KvCache{}, 0, sub, dropout_p, dropout_seed,
+                       (cudaStream_t)stream);
 }
 
 VB_API size_t vb_decoder_backward_workspace(const vb_decoder_desc *desc, int64_t M) {
@@ -559,18 +553,14 @@ DecodeSplits decode_splits(const vb_decoder_desc &D, bool fold) {
 }
 
 bool kv_fp8(const vb_ar_state *st) { return st->kv_dtype == VB_E4M3; }
-// layer l's caches and the rows' lengths: where the QKV projection leaves q and appends k / v, what the attention
-// reads and what the KV prefetch pulls into L2 (FP8 cache: also the layer's exponent arrays)
+// layer l's cache and the rows' lengths: where the QKV projection leaves q and appends k / v, what the attention
+// reads and what the KV prefetch pulls into L2
 QkvScatter layer_kv(const vb_decoder_desc &D, const vb_ar_state *st, int l, float *q) {
   const bool f8 = kv_fp8(st);
-  const size_t off = (size_t)l * st->cache_layer_stride * (f8 ? 1 : elem_size(D.wdtype));
-  QkvScatter kv{D.d_model, D.d_model / D.n_head, q, (char *)st->kcache + off, (char *)st->vcache + off,
-                st->cache_seq_stride, st->cache_cap, st->text_len, st->prompt_len, st->n_gen, st->finished};
-  if (f8) {
-    kv.kexp = st->k_exp + (size_t)l * st->cache_layer_stride / 64;
-    kv.vexp = st->v_exp + (size_t)l * st->cache_layer_stride / 64;
-  }
-  return kv;
+  const KvCache cache{st->kcache, st->vcache, f8 ? st->k_exp : nullptr, f8 ? st->v_exp : nullptr, st->cache_seq_stride,
+                      st->cache_cap, (int)elem_size(f8 ? VB_E4M3 : D.wdtype)};
+  return QkvScatter{D.d_model, D.d_model / D.n_head, q, kv_cache_layer(cache, st->cache_layer_stride, l),
+                    KvRows{st->text_len, st->prompt_len, st->n_gen, st->finished}};
 }
 
 // final LayerNorm (adding the pending partials of the last FFN2) + ar_predict_layer + sampler on the tensor-core
@@ -664,7 +654,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   const int d = D.d_model, dff = D.d_ff, B = st->B, dt = D.wdtype, hd = d / D.n_head;
   const size_t ts = elem_size(dt);
   const int kv_dt = f8 ? VB_E4M3 : dt;
-  const size_t kv_row_bytes = f8 ? hd + 1 : hd * ts;   // one cached row of K (or V), with its exponent byte
+  const size_t kv_row_bytes = hd * elem_size(kv_dt) + (f8 ? 1 : 0);   // one cached row of K (or V), with its exponent byte
   Carve c(workspace);
   const StepWs w = carve_step_ws(c, D, B, st->cache_cap);
   float *x = st->x_cur;
@@ -696,17 +686,9 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     // the four projections of the chain each prefetch a quarter of the first pf_rows rows of the KV streams that the
     // NEXT attention launch will read (QKV: this layer's, the other three: the following layer's)
     auto kv_slice = [&](int layer, int quarter) {
-      KvPrefetch pf{};
-      if (pf_rows <= 0) return pf;
+      if (pf_rows <= 0) return KvPrefetch{};
       const QkvScatter kv = layer_kv(D, st, layer % D.n_layer, w.q);
-      pf.kbase = kv.kcache; pf.vbase = kv.vcache;
-      const int64_t cs = f8 ? 1 : (int64_t)ts;   // cache element size
-      pf.seq_stride_bytes = kv.cache_seq_stride * cs;
-      pf.B = B; pf.H = D.n_head; pf.cap = kv.cache_cap; pf.row_bytes = (int)(hd * cs);
-      pf.kexp = kv.kexp; pf.vexp = kv.vexp;
-      pf.text_len = kv.text_len; pf.prompt_len = kv.prompt_len; pf.n_gen = kv.n_gen;
-      pf.row_lo = pf_rows * quarter / 4; pf.row_hi = pf_rows * (quarter + 1) / 4;
-      return pf;
+      return KvPrefetch{kv.kv, kv.rows, B, D.n_head, pf_rows * quarter / 4, pf_rows * (quarter + 1) / 4};
     };
     SplitK pend;  // the last FFN2's partial sums, for the next LayerNorm to add
     if (post) VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));

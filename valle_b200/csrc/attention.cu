@@ -26,9 +26,8 @@ template <typename T>
 __global__ void __launch_bounds__(256)
 attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
                         const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens,
-                        int seg1_start, int mask_mode, T *__restrict__ out,
-                        T *__restrict__ kcache, T *__restrict__ vcache, int64_t cache_seq_stride,
-                        int cache_cap, const uint8_t *__restrict__ dmask, int64_t dld, DropCfg drop) {
+                        int seg1_start, int mask_mode, T *__restrict__ out, KvCache kv,
+                        const uint8_t *__restrict__ dmask, int64_t dld, DropCfg drop) {
   constexpr int LDT = 68;  // padded leading dim (floats), keeps float4 alignment
   extern __shared__ __align__(16) float smem[];
   float *Qt = smem;             // [64 e][LDT rows]
@@ -87,12 +86,12 @@ attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__
         Kt[(le0 + i) * LDT + lrow] = ok ? to_f32(kraw[i]) : 0.f;
         Vs[lrow * LDT + le0 + i] = ok ? to_f32(vraw[i]) : 0.f;
       }
-      if (kcache != nullptr && j0 == q0 && ok) {  // this CTA owns rows [q0, q0+64) of the cache
-        const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + kr) * HD + le0;
+      if (kv.k != nullptr && j0 == q0 && ok) {  // this CTA owns rows [q0, q0+64) of the cache
+        T *kc = (T *)kv.k + kv.row(b, h, kr) + le0, *vc = (T *)kv.v + kv.row(b, h, kr) + le0;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
-          kcache[off + i] = kraw[i];
-          vcache[off + i] = vraw[i];
+          kc[i] = kraw[i];
+          vc[i] = vraw[i];
         }
       }
     }
@@ -181,9 +180,8 @@ attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__
 
 int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_head, int head_dim,
                             const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
-                            int seg1_start, int max_seqlen, int mask_mode, void *out, void *kcache, void *vcache,
-                            int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
-                            cudaStream_t s, const DropCfg *drop, uint8_t *kexp, uint8_t *vexp) {
+                            int seg1_start, int max_seqlen, int mask_mode, void *out, const KvCache &kv,
+                            const uint8_t *dense_mask, int64_t dense_ld, cudaStream_t s, const DropCfg *drop) {
   VB_CHECK_ARG(head_dim == HD, "attention: head_dim=%d, only 64 is built", head_dim);
   DropCfg dc{};
   if (drop) dc = *drop;
@@ -199,31 +197,30 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_
   VB_CHECK_ARG(mask_mode == VB_MASK_FULL || text_lens != nullptr, "attention: this mask mode needs text_lens");
   VB_CHECK_ARG(mask_mode < VB_MASK_PADDED_AR || seg1_lens != nullptr, "attention: padded mask modes need seg1_lens");
   if (M == 0 || B == 0) return VB_OK;
-  if (kexp != nullptr) {   // an FP8 cache is filled by the wgmma kernel only
+  if (kv.kexp != nullptr) {   // an FP8 cache is filled by the wgmma kernel only
     if (dtype != VB_BF16 || dropping || dense_mask != nullptr || tune("VB_ATTN_SIMT", 0) != 0) {
       set_error("attention: an FP8 KV cache is filled by the bf16 wgmma prefill only (no dropout, no dense mask, not VB_ATTN_SIMT)");
       return VB_ERR_UNSUPPORTED;
     }
-    VB_CHECK_ARG(kcache && vcache && vexp, "attention: FP8 cache: kcache, vcache, k_exp and v_exp are all needed");
+    VB_CHECK_ARG(kv.k && kv.v && kv.vexp, "attention: FP8 cache: kcache, vcache, k_exp and v_exp are all needed");
     return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                  max_seqlen, mask_mode, (bf16 *)out, kcache, vcache, cache_seq_stride, cache_cap, s,
-                                  kexp, vexp);
+                                  max_seqlen, mask_mode, (bf16 *)out, kv, s);
   }
   const size_t smem = 4 * 64 * 68 * sizeof(float);
   dim3 grid((max_seqlen + 63) / 64, n_head, B);
   if (dtype == VB_F32) {
     auto k = attn_varlen_simt_kernel<float>;
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<grid, 256, smem, s>>>((const float *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, (float *)out,
-                              (float *)kcache, (float *)vcache, cache_seq_stride, cache_cap, dense_mask, dense_ld, dc);
+    k<<<grid, 256, smem, s>>>((const float *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode,
+                              (float *)out, kv, dense_mask, dense_ld, dc);
   } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && tune("VB_ATTN_SIMT", 0) == 0) {
     return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
-                                  mask_mode, (bf16 *)out, kcache, vcache, cache_seq_stride, cache_cap, s);
+                                  mask_mode, (bf16 *)out, kv, s);
   } else if (dtype == VB_BF16) {
     auto k = attn_varlen_simt_kernel<bf16>;
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<grid, 256, smem, s>>>((const bf16 *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, (bf16 *)out,
-                              (bf16 *)kcache, (bf16 *)vcache, cache_seq_stride, cache_cap, dense_mask, dense_ld, dc);
+    k<<<grid, 256, smem, s>>>((const bf16 *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode,
+                              (bf16 *)out, kv, dense_mask, dense_ld, dc);
   } else {
     set_error("attention: bad dtype %d", dtype);
     return VB_ERR_ARG;
@@ -252,15 +249,10 @@ template <> __device__ __forceinline__ void KvRow8<bf16>::load(const bf16 *p, fl
   v.unpack(f);
 }
 
-// Optional fused prologue: q/k/v of the CURRENT token arrive as split-K partials of the QKV
-// projection (gemm_decode.cu); the CTA sums them in fixed order, adds the bias, appends k/v to the
-// cache (split 0) and serves the new key/value from shared memory.
-struct QkvPartials {
-  const float *part;  // [splits][64][ldp] or nullptr
-  const float *bias;  // [3d] (with a folded LayerNorm: bias + beta W^T)
-  int splits, ldp;
-  LnFoldStats fold;   // fold.stats != NULL: the partials are x (gamma o W)^T of the raw rows (gemm_decode_x_kernel)
-};
+// Optional fused prologue (qp.part != nullptr): q/k/v of the CURRENT token arrive as split-K partials of the QKV
+// projection (gemm_decode.cu); the CTA sums them in fixed order, adds the bias, appends k/v to the cache (split 0)
+// and serves the new key/value from shared memory.  qp.fold.stats != NULL: the partials are x (gamma o W)^T of the
+// raw rows (gemm_decode_x_kernel).
 
 // A finished utterance (stop rule fired, vb_ar_state.finished != 0) takes no further part in the step: its KV
 // cache stays as it is (nothing appended, nothing streamed) and its attention output row is zero.  Uniform
@@ -291,10 +283,7 @@ __device__ __forceinline__ bool decode_row_finished(const int32_t *finished, int
 // groups are merged once at the end (flash-decoding style).
 template <typename T>
 __global__ void __launch_bounds__(128)
-attn_decode_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, T *__restrict__ kcache,
-                   T *__restrict__ vcache, int64_t cache_seq_stride, int cache_cap,
-                   const int32_t *__restrict__ text_len, const int32_t *__restrict__ prompt_len,
-                   const int32_t *__restrict__ n_gen, const int32_t *__restrict__ finished,
+attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
                    float *__restrict__ out, bf16 *__restrict__ out16,
                    float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit) {
   __shared__ __align__(16) float qs[HD];
@@ -307,15 +296,14 @@ attn_decode_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, T *_
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int d = n_head * HD;
   pdl_wait();
-  if (decode_row_finished(finished, b, h, sp, d, threadIdx.x, nsplit, n_head, out, out16, part_o, part_ml)) return;
-  int kv_len = text_len[b] + prompt_len[b] + n_gen[b];
-  kv_len = max(1, min(kv_len, cache_cap));
-  const int pos = kv_len - 1;  // cache row of the current token
+  if (decode_row_finished(rows.finished, b, h, sp, d, threadIdx.x, nsplit, n_head, out, out16, part_o, part_ml)) return;
+  const int pos = rows.cur(b, rows.n_gen[b], kv.cap);  // cache row of the current token
+  const int kv_len = pos + 1;
   const int chunk = ((kv_len + nsplit - 1) / nsplit + 15) & ~15;
   const int c0 = sp * chunk, c1 = min(kv_len, c0 + chunk);
   const int n = max(0, c1 - c0);
-  T *kb = kcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
-  T *vb_ = vcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
+  T *kb = (T *)kv.k + kv.row(b, h, 0);
+  T *vb_ = (T *)kv.v + kv.row(b, h, 0);
   const bool has_new = qp.part != nullptr;
   if (tid < HD) {
     if (has_new) {
@@ -451,13 +439,9 @@ attn_decode_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, T *_
 // memory; split 0 appends their quantized rows.
 template <int U, typename CT>
 __global__ void __launch_bounds__(128, 8)
-attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_head, CT *__restrict__ kcache,
-                   CT *__restrict__ vcache, int64_t cache_seq_stride, int cache_cap,
-                   const int32_t *__restrict__ text_len, const int32_t *__restrict__ prompt_len,
-                   const int32_t *__restrict__ n_gen, const int32_t *__restrict__ finished,
+attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
                    float *__restrict__ out, bf16 *__restrict__ out16,
-                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
-                   uint8_t *__restrict__ kexp, uint8_t *__restrict__ vexp) {
+                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit) {
   constexpr bool kF8 = sizeof(CT) == 1;
   using Raw = typename std::conditional<kF8, uint2, uint4>::type;
   auto ld_raw = [](const CT *p) -> Raw {
@@ -489,8 +473,8 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int d = n_head * HD;
   using T = bf16;
-  CT *kb = kcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
-  CT *vb_ = vcache + (int64_t)b * cache_seq_stride + (int64_t)h * cache_cap * HD;
+  CT *kb = (CT *)kv.k + kv.row(b, h, 0);
+  CT *vb_ = (CT *)kv.v + kv.row(b, h, 0);
   const bool has_new = qp.part != nullptr;
   const int g = lane >> 3, j8 = (lane & 7) * 8;
   // The K rows of earlier tokens and the lengths do not depend on the kernels of THIS step that precede the
@@ -500,8 +484,8 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   int kv_len, pos, c0, c1, n;
   Raw kraw[U];
   auto setup = [&](int n_generated) {
-    kv_len = max(1, min(text_len[b] + prompt_len[b] + n_generated, cache_cap));
-    pos = kv_len - 1;  // cache row of the current token
+    pos = rows.cur(b, n_generated, kv.cap);  // cache row of the current token
+    kv_len = pos + 1;
     const int chunk = ((kv_len + nsplit - 1) / nsplit + 15) & ~15;
     c0 = sp * chunk;
     c1 = min(kv_len, c0 + chunk);
@@ -514,7 +498,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   };
   // (only with the fused QKV prologue: there the current token's row is served from shared memory; without it the
   // row was written to the cache by the kernel this launch depends on and nothing may be read ahead of the wait)
-  const int n_gen_early = has_new ? n_gen[b] : -1;
+  const int n_gen_early = has_new ? rows.n_gen[b] : -1;
   if (has_new) setup(n_gen_early);
   float qbias[3] = {0.f, 0.f, 0.f}, qc[3] = {0.f, 0.f, 0.f};
   if (tid < HD && has_new) {
@@ -527,23 +511,23 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
   pdl_wait();
   vb_trace(TR_ATTN * 2);
   vb_trace_cta(17);   // dependency resolved
-  if (decode_row_finished(finished, b, h, sp, d, tid, nsplit, n_head, out, out16, part_o, part_ml)) return;
+  if (decode_row_finished(rows.finished, b, h, sp, d, tid, nsplit, n_head, out, out16, part_o, part_ml)) return;
   int n_gen_now;
-  asm volatile("ld.global.cg.s32 %0, [%1];" : "=r"(n_gen_now) : "l"(n_gen + b) : "memory");
+  asm volatile("ld.global.cg.s32 %0, [%1];" : "=r"(n_gen_now) : "l"(rows.n_gen + b) : "memory");
   if (n_gen_now != n_gen_early) setup(n_gen_now);  // uniform over the CTA
-  // FP8: the chunk's exponent bytes -> shared memory (16-byte cp.async: c0 and cache_cap are multiples of 16), behind
+  // FP8: the chunk's exponent bytes -> shared memory (16-byte cp.async: c0 and kv.cap are multiples of 16), behind
   // the score buffer; read once the scores are in
   uint8_t *kes = nullptr, *ves = nullptr;
   if constexpr (kF8) {
-    const int sc_len = ((cache_cap + nsplit - 1) / nsplit + 32 + 15) & ~15;
+    const int sc_len = ((kv.cap + nsplit - 1) / nsplit + 32 + 15) & ~15;
     kes = reinterpret_cast<uint8_t *>(sc + sc_len);
     ves = kes + sc_len;
-    const int64_t e0 = ((int64_t)b * cache_seq_stride) / HD + (int64_t)h * cache_cap + c0;
+    const int64_t e0 = kv.exp_index(b, h, c0);
     for (int i = tid; i < (n + 15) / 16; i += 128) {
       asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(kes + 16 * i)),
-                   "l"(kexp + e0 + 16 * i) : "memory");
+                   "l"(kv.kexp + e0 + 16 * i) : "memory");
       asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(ves + 16 * i)),
-                   "l"(vexp + e0 + 16 * i) : "memory");
+                   "l"(kv.vexp + e0 + 16 * i) : "memory");
     }
     asm volatile("cp.async.commit_group;" ::: "memory");
   }
@@ -602,9 +586,9 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, QkvPartials qp, int n_
         kb[(int64_t)pos * HD + tid] = kv8_quant(knew[tid], ek);
         vb_[(int64_t)pos * HD + tid] = kv8_quant(vnew[tid], ev);
         if (tid == 0) {
-          const int64_t e0 = ((int64_t)b * cache_seq_stride) / HD + (int64_t)h * cache_cap + pos;
-          kexp[e0] = (uint8_t)ek;
-          vexp[e0] = (uint8_t)ev;
+          const int64_t e0 = kv.exp_index(b, h, pos);
+          kv.kexp[e0] = (uint8_t)ek;
+          kv.vexp[e0] = (uint8_t)ev;
         }
       }
     }
@@ -775,79 +759,65 @@ size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap) {
   return (size_t)B * n_head * ns * (head_dim + 2) * sizeof(float) + 256;
 }
 
+// VB_ATTN_CARVEOUT: shared-memory carve-out (percent) preferred for the two-phase decode kernels; -1 = the driver's
+// choice.  A fixed carve-out keeps the SMs from re-partitioning on the way in and out of every attention launch of the
+// chain; the largest carve-out leaves no L1 for the loads in flight.  (Default not re-tuned on H100.)  Set on the
+// current device whenever the knob differs from what kernel `kKernel` last got there; the driver's choice needs no
+// call until another value has been set.
+template <auto kKernel>
+static int set_attn_carveout() {
+  static int set[64];
+  static bool init = false;
+  if (!init) {
+    for (int i = 0; i < 64; ++i) set[i] = -2;
+    init = true;
+  }
+  int dev = 0;
+  cudaGetDevice(&dev);
+  const int carve = tune("VB_ATTN_CARVEOUT", 72);
+  if (set[dev & 63] != carve) {
+    const int want = carve >= 0 ? carve : (int)cudaSharedmemCarveoutDefault;
+    if (carve >= 0 || set[dev & 63] != -2)
+      VB_CUDA(cudaFuncSetAttribute(kKernel, cudaFuncAttributePreferredSharedMemoryCarveout, want));
+    set[dev & 63] = carve;
+  }
+  return VB_OK;
+}
+
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
                        void *workspace, bool pdl, cudaStream_t s) {
   VB_CHECK_ARG(kv.head_dim == HD, "attn_decode: head_dim=%d, only 64 is built", kv.head_dim);
-  const int cache_cap = kv.cache_cap;
+  const int cache_cap = kv.kv.cap;
   const int ns = decode_nsplit(B, n_head, cache_cap);
   VB_CHECK_ARG((cache_cap + ns - 1) / ns + 16 <= kDecMaxChunk, "attn_decode: cache_cap %d too large", cache_cap);
   float *part_o = (float *)workspace;
   float *part_ml = part_o + (size_t)B * n_head * ns * HD;
-  const QkvPartials qp{qkv.part, qkv.bias, qkv.splits, qkv.ldp, qkv.fold};
   dim3 grid(n_head, B, ns);
   if (dtype == VB_E4M3) {
     if (tune("VB_ATTN_DECODE_1PASS", 0) != 0) {
       set_error("attn_decode: VB_ATTN_DECODE_1PASS has no FP8-cache variant");
       return VB_ERR_UNSUPPORTED;
     }
-    VB_CHECK_ARG(qkv.part != nullptr && kv.kexp != nullptr && kv.vexp != nullptr && cache_cap % 16 == 0,
+    VB_CHECK_ARG(qkv.part != nullptr && kv.kv.kexp != nullptr && kv.kv.vexp != nullptr && cache_cap % 16 == 0,
                  "attn_decode: the FP8 cache needs the fused QKV prologue, exponent arrays and cache_cap %% 16 == 0");
     // score buffer as for bf16 (rounded to 16 floats), then the chunk's K and V exponent bytes
     const int sc_len = ((cache_cap + ns - 1) / ns + 32 + 15) & ~15;
     const size_t smem = align_up((size_t)sc_len * (sizeof(float) + 2), 1024);
-    auto k = attn_decode_2phase_pf_kernel<8, uint8_t>;
-    static int carve_f8[64];
-    static bool carve_f8_init = false;
-    if (!carve_f8_init) {
-      for (int i = 0; i < 64; ++i) carve_f8[i] = -2;
-      carve_f8_init = true;
-    }
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const int carve = tune("VB_ATTN_CARVEOUT", 72);
-    if (carve_f8[dev & 63] != carve) {
-      const int want = carve >= 0 ? carve : (int)cudaSharedmemCarveoutDefault;
-      if (carve >= 0 || carve_f8[dev & 63] != -2)
-        VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, want));
-      carve_f8[dev & 63] = carve;
-    }
-    VB_CUDA(launch_kernel(k, grid, dim3(128), smem, s, pdl, (const float *)kv.q, qp, n_head, (uint8_t *)kv.kcache,
-                          (uint8_t *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len, kv.prompt_len, kv.n_gen,
-                          kv.finished, out, (bf16 *)out16, part_o, part_ml, ns, kv.kexp, kv.vexp));
+    constexpr auto k = attn_decode_2phase_pf_kernel<8, uint8_t>;
+    VB_TRY(set_attn_carveout<k>());
+    VB_CUDA(launch_kernel(k, grid, dim3(128), smem, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
+                          (bf16 *)out16, part_o, part_ml, ns));
   } else if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
-    if (dtype == VB_F32)
-      VB_CUDA(launch_kernel(attn_decode_kernel<float>, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qp, n_head,
-                            (float *)kv.kcache, (float *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
-                            kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns));
-    else
-      VB_CUDA(launch_kernel(attn_decode_kernel<bf16>, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qp, n_head,
-                            (bf16 *)kv.kcache, (bf16 *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
-                            kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns));
+    VB_CUDA(launch_kernel(dtype == VB_F32 ? attn_decode_kernel<float> : attn_decode_kernel<bf16>, grid, dim3(128), 0, s,
+                          pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml,
+                          ns));
   } else {
     // score buffer: the chunk of one split, rounded as the kernel rounds it (+16), in 1 KB steps
     const size_t sc_bytes = align_up((size_t)((cache_cap + ns - 1) / ns + 32) * sizeof(float), 1024);
-    // VB_ATTN_CARVEOUT: shared-memory carve-out (percent) preferred for this kernel; -1 = the driver's choice.  A fixed
-    // carve-out keeps the SMs from re-partitioning on the way in and out of every attention launch of the chain; the
-    // largest carve-out leaves no L1 for the loads in flight.  (Default not re-tuned on H100.)
-    static int carve_set[64];
-    static bool carve_init = false;
-    if (!carve_init) {
-      for (int i = 0; i < 64; ++i) carve_set[i] = -2;
-      carve_init = true;
-    }
-    int dev = 0;
-    cudaGetDevice(&dev);
-    const int carve = tune("VB_ATTN_CARVEOUT", 72);
-    if (carve_set[dev & 63] != carve) {
-      const int want = carve >= 0 ? carve : (int)cudaSharedmemCarveoutDefault;
-      if (carve >= 0 || carve_set[dev & 63] != -2)
-        VB_CUDA(cudaFuncSetAttribute(attn_decode_2phase_pf_kernel<4, bf16>, cudaFuncAttributePreferredSharedMemoryCarveout, want));
-      carve_set[dev & 63] = carve;
-    }
-    VB_CUDA(launch_kernel(attn_decode_2phase_pf_kernel<4, bf16>, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q,
-                          qp, n_head, (bf16 *)kv.kcache, (bf16 *)kv.vcache, kv.cache_seq_stride, cache_cap, kv.text_len,
-                          kv.prompt_len, kv.n_gen, kv.finished, out, (bf16 *)out16, part_o, part_ml, ns,
-                          (uint8_t *)nullptr, (uint8_t *)nullptr));
+    constexpr auto k = attn_decode_2phase_pf_kernel<4, bf16>;
+    VB_TRY(set_attn_carveout<k>());
+    VB_CUDA(launch_kernel(k, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
+                          (bf16 *)out16, part_o, part_ml, ns));
   }
   count_launch();
   if (ns > 1) {
@@ -865,7 +835,7 @@ VB_API int vb_attention(const void *qkv, int dtype, int64_t M, int B, int n_head
                         int max_seqlen, int mask_mode, void *out, void *kcache, void *vcache,
                         int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
                         vb_stream_t stream) {
+  const vb::KvCache kv{kcache, vcache, nullptr, nullptr, cache_seq_stride, cache_cap, (int)vb::elem_size(dtype)};
   return vb::launch_attention_varlen(qkv, dtype, M, B, n_head, head_dim, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                     max_seqlen, mask_mode, out, kcache, vcache, cache_seq_stride, cache_cap,
-                                     dense_mask, dense_ld, (cudaStream_t)stream);
+                                     max_seqlen, mask_mode, out, kv, dense_mask, dense_ld, (cudaStream_t)stream);
 }

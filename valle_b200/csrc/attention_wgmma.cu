@@ -102,14 +102,13 @@ __device__ __forceinline__ void online_softmax(float (&s)[32], int j0, int t, co
   l_b = l_b * corr_b + rs_b;
 }
 
-// kF8: the KV cache is the FP8 one (include/valle_b200.h, vb_decoder_forward_kv8): kcache / vcache hold e4m3 bytes and
-// kexp / vexp the rows' exponents; the attention itself computes on the bf16 tiles either way
+// kF8: the KV cache is the FP8 one (include/valle_b200.h, vb_decoder_forward_kv8): e4m3 rows and their exponents;
+// the attention itself computes on the bf16 tiles either way
 template <bool kF8>
 __global__ void __launch_bounds__(kThreads, 2)
 attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
                   const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens, int seg1_start,
-                  int mask_mode, bf16 *__restrict__ out, bf16 *__restrict__ kcache, bf16 *__restrict__ vcache,
-                  int64_t cache_seq_stride, int cache_cap, uint8_t *__restrict__ kexp, uint8_t *__restrict__ vexp) {
+                  int mask_mode, bf16 *__restrict__ out, const __grid_constant__ KvCache kv) {
   const int b = blockIdx.z, h = blockIdx.y;
   const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
   const int q0 = blockIdx.x * BQ;
@@ -191,22 +190,21 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
   };
   // the prefill fills the KV cache: warpgroup `half` copies key tile q0 + 64 half (rows < L)
   auto fill_cache = [&](int j0, const uint8_t *sk) {
-    if (kcache == nullptr || j0 != q0 + half * 64) return;
+    if (kv.k == nullptr || j0 != q0 + half * 64) return;
     const uint8_t *sv = sk + kBoxBytes;
     if constexpr (kF8) {
       // 8 consecutive lanes hold one row (16 bytes = 8 bf16 each): the row's max |.| is one 8-lane shuffle reduction
-      uint8_t *kc8 = reinterpret_cast<uint8_t *>(kcache), *vc8 = reinterpret_cast<uint8_t *>(vcache);
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
         const int idx = t + i * 128;
         const int r = idx >> 3, c = idx & 7;
         const int so = r * 128 + ((c ^ (r & 7)) << 4);
-        Vec16<bf16> kv, vv;
-        kv.raw = *reinterpret_cast<const uint4 *>(sk + so);
-        vv.raw = *reinterpret_cast<const uint4 *>(sv + so);
+        Vec16<bf16> kt, vt;
+        kt.raw = *reinterpret_cast<const uint4 *>(sk + so);
+        vt.raw = *reinterpret_cast<const uint4 *>(sv + so);
         float kf[8], vf[8];
-        kv.unpack(kf);
-        vv.unpack(vf);
+        kt.unpack(kf);
+        vt.unpack(vf);
         float ak = 0.f, av = 0.f;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -226,12 +224,12 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
             kq[j >> 2] |= (uint32_t)kv8_quant(kf[j], ek) << (8 * (j & 3));
             vq[j >> 2] |= (uint32_t)kv8_quant(vf[j], ev) << (8 * (j & 3));
           }
-          const int64_t row = (int64_t)b * (cache_seq_stride / HD) + (int64_t)h * cache_cap + j0 + r;
-          *reinterpret_cast<uint2 *>(kc8 + row * HD + c * 8) = make_uint2(kq[0], kq[1]);
-          *reinterpret_cast<uint2 *>(vc8 + row * HD + c * 8) = make_uint2(vq[0], vq[1]);
+          const int64_t e = kv.exp_index(b, h, j0 + r), off = e * HD + c * 8;   // row(b, h, p) = 64 exp_index(b, h, p)
+          *reinterpret_cast<uint2 *>((uint8_t *)kv.k + off) = make_uint2(kq[0], kq[1]);
+          *reinterpret_cast<uint2 *>((uint8_t *)kv.v + off) = make_uint2(vq[0], vq[1]);
           if (c == 0) {
-            kexp[row] = (uint8_t)ek;
-            vexp[row] = (uint8_t)ev;
+            kv.kexp[e] = (uint8_t)ek;
+            kv.vexp[e] = (uint8_t)ev;
           }
         }
       }
@@ -241,10 +239,10 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
         const int idx = t + i * 128;
         const int r = idx >> 3, c = idx & 7;
         if (j0 + r < L) {
-          const int64_t off = (int64_t)b * cache_seq_stride + ((int64_t)h * cache_cap + j0 + r) * HD + c * 8;
+          const int64_t off = kv.row(b, h, j0 + r) + c * 8;
           const int so = r * 128 + ((c ^ (r & 7)) << 4);
-          *reinterpret_cast<uint4 *>(kcache + off) = *reinterpret_cast<const uint4 *>(sk + so);
-          *reinterpret_cast<uint4 *>(vcache + off) = *reinterpret_cast<const uint4 *>(sv + so);
+          *reinterpret_cast<uint4 *>((bf16 *)kv.k + off) = *reinterpret_cast<const uint4 *>(sk + so);
+          *reinterpret_cast<uint4 *>((bf16 *)kv.v + off) = *reinterpret_cast<const uint4 *>(sv + so);
         }
       }
     }
@@ -318,21 +316,19 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
 
 int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
                            const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, bf16 *out, void *kcache, void *vcache, int64_t cache_seq_stride,
-                           int cache_cap, cudaStream_t s, uint8_t *kexp, uint8_t *vexp) {
+                           int mask_mode, bf16 *out, const KvCache &kv, cudaStream_t s) {
   if (M == 0 || B == 0) return VB_OK;
   VB_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0, "wgmma attention: qkv must be 16-byte aligned");
   CUtensorMap tm;
   VB_TRY(tc::make_tmap(&tm, qkv, M, 3 * n_head * fa3::HD, 3 * (int64_t)n_head * fa3::HD, 64));
   dim3 grid((max_seqlen + fa3::BQ - 1) / fa3::BQ, n_head, B);
-  if (kexp != nullptr) {
+  if (kv.kexp != nullptr) {
     static PerDeviceOnce once8;
     if (once8.first())
       VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                    fa3::kSmemBytes));
     fa3::attn_wgmma_kernel<true><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(
-        tm, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, out, (bf16 *)kcache, (bf16 *)vcache,
-        cache_seq_stride, cache_cap, kexp, vexp);
+        tm, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, out, kv);
     VB_LAUNCH_CHECK();
     return VB_OK;
   }
@@ -341,10 +337,7 @@ int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const 
     VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  fa3::kSmemBytes));
   fa3::attn_wgmma_kernel<false><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(tm, n_head, cu_seqlens, text_lens,
-                                                                             seg1_lens, seg1_start, mask_mode, out,
-                                                                             (bf16 *)kcache, (bf16 *)vcache,
-                                                                             cache_seq_stride, cache_cap, nullptr,
-                                                                             nullptr);
+                                                                             seg1_lens, seg1_start, mask_mode, out, kv);
   VB_LAUNCH_CHECK();
   return VB_OK;
 }

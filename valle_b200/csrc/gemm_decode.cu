@@ -49,11 +49,7 @@ struct Epi {
   float *out_f32;      // [B, ld_out] (RESIDUAL: in/out; F32: out; QKV: q)
   bf16 *out_bf16;      // [B, ld_out] (RELU_BF16)
   int64_t ld_out;
-  // QKV scatter
-  int d, head_dim, cache_cap;
-  bf16 *kcache, *vcache;
-  int64_t cache_seq_stride;
-  const int32_t *text_len, *prompt_len, *n_gen, *finished;
+  QkvScatter qkv;      // DG_QKV
 };
 
 __device__ __forceinline__ void apply_epi(const Epi &e, int n, int b, float v) {
@@ -66,15 +62,14 @@ __device__ __forceinline__ void apply_epi(const Epi &e, int n, int b, float v) {
   } else if (e.mode == DG_RELU_BF16) {
     e.out_bf16[(int64_t)b * e.ld_out + n] = __float2bfloat16_rn(fmaxf(v, 0.f));
   } else {
-    const int part = n / e.d, c = n - part * e.d;
+    const QkvScatter &q = e.qkv;
+    const int part = n / q.d, c = n - part * q.d;
     if (part == 0) {
-      e.out_f32[(int64_t)b * e.ld_out + c] = v;
-    } else if (e.finished == nullptr || e.finished[b] == 0) {
-      const int h = c / e.head_dim, el = c - h * e.head_dim;
-      int pos = e.text_len[b] + e.prompt_len[b] + e.n_gen[b] - 1;
-      pos = max(0, min(pos, e.cache_cap - 1));
-      const int64_t off = (int64_t)b * e.cache_seq_stride + ((int64_t)h * e.cache_cap + pos) * e.head_dim + el;
-      (part == 1 ? e.kcache : e.vcache)[off] = __float2bfloat16_rn(v);
+      q.q[(int64_t)b * q.d + c] = v;
+    } else if (q.rows.finished == nullptr || q.rows.finished[b] == 0) {
+      const int h = c / q.head_dim, el = c - h * q.head_dim;
+      const int64_t off = q.kv.row(b, h, q.rows.cur(b, q.rows.n_gen[b], q.kv.cap)) + el;
+      ((bf16 *)(part == 1 ? q.kv.k : q.kv.v))[off] = __float2bfloat16_rn(v);
     }
   }
 }
@@ -441,12 +436,7 @@ int launch_gemm_decode(const bf16 *act, int B, int64_t ld_act, const bf16 *W, in
   e.out_f32 = out_f32; e.out_bf16 = out_bf16; e.ld_out = ld_out;
   if (mode == DG_QKV && splits == 1) {
     VB_CHECK_ARG(qkv != nullptr, "gemm_decode: qkv scatter parameters missing");
-    e.d = qkv->d; e.head_dim = qkv->head_dim; e.cache_cap = qkv->cache_cap;
-    e.kcache = (bf16 *)qkv->kcache; e.vcache = (bf16 *)qkv->vcache;
-    e.cache_seq_stride = qkv->cache_seq_stride;
-    e.text_len = qkv->text_len; e.prompt_len = qkv->prompt_len; e.n_gen = qkv->n_gen;
-    e.finished = qkv->finished;
-    e.out_f32 = qkv->q; e.ld_out = qkv->d;
+    e.qkv = *qkv;
   }
   static PerDeviceOnce once;
   if (once.first()) {

@@ -145,13 +145,7 @@ template <int VEC> __device__ __forceinline__ int xs_phys(int k, int K) {
 
 struct GemvEpi {
   int mode;  // 0 none, 1 relu, 2 residual (out += ), 3 qkv-scatter
-  // qkv scatter (mode 3): n in [0,d) -> q[b,n]; [d,2d) -> kcache; [2d,3d) -> vcache
-  int d, head_dim;
-  float *q;  // [B, d]
-  void *kcache, *vcache;
-  int64_t cache_seq_stride;  // elements between sequences within one layer
-  int cache_cap;
-  const int32_t *text_len, *prompt_len, *n_gen, *finished;
+  QkvScatter qkv;  // mode 3: n in [0,d) -> q[b,n]; [d,2d) -> the K cache; [2d,3d) -> the V cache
 };
 
 template <typename TW, int BT, int NPW>
@@ -254,16 +248,14 @@ gemv_kernel(const float *__restrict__ x, int64_t ldx, int B, const TW *__restric
             const int bb = b0 + b;
             float v = acc[j][b] + bn;
             if (epi.mode == 3) {
-              const int part = n / epi.d, c = n - part * epi.d;
+              const QkvScatter &q = epi.qkv;
+              const int part = n / q.d, c = n - part * q.d;
               if (part == 0) {
-                epi.q[(int64_t)bb * epi.d + c] = v;
-              } else if (epi.finished == nullptr || epi.finished[bb] == 0) {
-                const int h = c / epi.head_dim, e = c - h * epi.head_dim;
-                int pos = epi.text_len[bb] + epi.prompt_len[bb] + epi.n_gen[bb] - 1;
-                pos = max(0, min(pos, epi.cache_cap - 1));
-                const int64_t off = (int64_t)bb * epi.cache_seq_stride +
-                                    ((int64_t)h * epi.cache_cap + pos) * epi.head_dim + e;
-                TW *cache = reinterpret_cast<TW *>(part == 1 ? epi.kcache : epi.vcache);
+                q.q[(int64_t)bb * q.d + c] = v;
+              } else if (q.rows.finished == nullptr || q.rows.finished[bb] == 0) {
+                const int h = c / q.head_dim, e = c - h * q.head_dim;
+                const int64_t off = q.kv.row(bb, h, q.rows.cur(bb, q.rows.n_gen[bb], q.kv.cap)) + e;
+                TW *cache = reinterpret_cast<TW *>(part == 1 ? q.kv.k : q.kv.v);
                 cache[off] = from_f32<TW>(v);
               }
             } else {
@@ -330,11 +322,7 @@ int launch_gemv(const float *x, int64_t ldx, int B, const void *W, int w_dtype, 
   epi.mode = epi_mode;
   if (epi_mode == 3) {
     VB_CHECK_ARG(qkv != nullptr, "gemv: qkv scatter parameters missing");
-    epi.d = qkv->d; epi.head_dim = qkv->head_dim; epi.q = qkv->q;
-    epi.kcache = qkv->kcache; epi.vcache = qkv->vcache;
-    epi.cache_seq_stride = qkv->cache_seq_stride; epi.cache_cap = qkv->cache_cap;
-    epi.text_len = qkv->text_len; epi.prompt_len = qkv->prompt_len; epi.n_gen = qkv->n_gen;
-    epi.finished = qkv->finished;
+    epi.qkv = *qkv;
   }
   const float *g = ln ? ln->gamma : nullptr, *bt = ln ? ln->beta : nullptr, *ada = ln ? ln->ada_wb : nullptr;
   const float eps = ln ? ln->eps : 0.f;

@@ -63,6 +63,57 @@ __device__ __forceinline__ RowMask make_row_mask(int mode, int qr, int L, int S,
   return m;
 }
 
+// bytes per element of a VB_* dtype
+inline size_t elem_size(int dtype) { return dtype == VB_E4M3 ? 1 : dtype == VB_BF16 ? 2 : 4; }
+
+// The KV cache of the AR decoder, seen one layer at a time.  The whole cache is two arrays, K and V, of
+// [n_layer, B, H, cap, 64] rows (one row = one token's key or value of one head): layer l starts l * layer_stride
+// elements in, utterance b of a layer b * seq_stride elements in, and the cap rows of one (utterance, head) stream are
+// contiguous.  The elements are fp32, bf16 (the decoder's dtype) or, for the FP8 cache, e4m3 bytes; an FP8 row has one
+// exponent byte e + 127 as well and reads back as e4m3 * 2^e (kv8_* in common.cuh), and the exponent arrays
+// [n_layer, B, H, cap] have the cache's strides divided by 64 (both strides are multiples of 1024 there, so a row's
+// element offset is 64 times its exponent index).  Utterance b's stream holds KvRows::count rows, the current
+// token's being KvRows::cur.
+struct KvCache {
+  void *k, *v;            // this layer's K and V rows, or nullptr (no cache)
+  uint8_t *kexp, *vexp;   // this layer's exponent bytes (FP8 cache), else nullptr
+  int64_t seq_stride;     // elements between utterances
+  int cap;                // rows per (utterance, head) stream
+  int elem;               // bytes per element
+  // element offset of row `pos` of stream (b, h) from k / v
+  __host__ __device__ __forceinline__ int64_t row(int b, int h, int pos) const {
+    return (int64_t)b * seq_stride + ((int64_t)h * cap + pos) * 64;
+  }
+  // index of that row's exponent byte in kexp / vexp
+  __host__ __device__ __forceinline__ int64_t exp_index(int b, int h, int pos) const {
+    return (int64_t)b * (seq_stride / 64) + (int64_t)h * cap + pos;
+  }
+};
+// layer l's view, from the whole cache (the view whose pointers are the arrays' bases) and the elements between
+// layers; a null pointer stays null
+inline KvCache kv_cache_layer(KvCache c, int64_t layer_stride, int l) {
+  const size_t off = (size_t)l * layer_stride * c.elem, eoff = (size_t)l * layer_stride / 64;
+  if (c.k) c.k = (char *)c.k + off;
+  if (c.v) c.v = (char *)c.v + off;
+  if (c.kexp) c.kexp += eoff;
+  if (c.vexp) c.vexp += eoff;
+  return c;
+}
+// The rows of each utterance's cache streams during AR decoding (vb_ar_state): text_len[b] + prompt_len[b] + n_gen[b]
+// once n_gen[b] tokens are generated, at most cap.  n_gen[b] is an argument: the decode attention reads it twice.
+struct KvRows {
+  const int32_t *text_len, *prompt_len, *n_gen;
+  const int32_t *finished;  // NULL or [B]: rows that have stopped keep their cache untouched
+  __device__ __forceinline__ int count(int b, int n_gen_b, int cap) const {
+    return min(text_len[b] + prompt_len[b] + n_gen_b, cap);
+  }
+  // the current token's row, max(count, 1) - 1, written as a clamp: spelled with count, the QKV epilogue of
+  // gemv_kernel takes more registers and spills more
+  __device__ __forceinline__ int cur(int b, int n_gen_b, int cap) const {
+    return max(0, min(text_len[b] + prompt_len[b] + n_gen_b - 1, cap - 1));
+  }
+};
+
 // L2 prefetch of a slice of an upcoming layer's K and V cache, issued by the otherwise idle warps of the
 // split-K decode projections (gemm_decode.cu) while their weight tiles stream: the projection chain is latency
 // bound and leaves HBM mostly idle, the KV-cache attention that follows is HBM bound -- rows [row_lo, row_hi) of
@@ -70,17 +121,15 @@ __device__ __forceinline__ RowMask make_row_mask(int mode, int qr, int L, int S,
 // ahead of it.  Only a hint: the lengths may be one step stale (read before the dependency wait),
 // which changes what is prefetched, never what is computed.
 struct KvPrefetch {
-  const void *kbase, *vbase;  // caches of the target layer ([B, H, cap, 64]) or nullptr
-  int64_t seq_stride_bytes;   // bytes between utterances
-  int B, H, cap, row_bytes;   // row_bytes = 64 * element size
-  const int32_t *text_len, *prompt_len, *n_gen;
+  KvCache kv;   // the target layer (kv.k == nullptr: nothing to prefetch)
+  KvRows rows;
+  int B, H;
   int row_lo, row_hi;
-  const uint8_t *kexp, *vexp; // FP8 cache: the exponent arrays of the target layer ([B, H, cap]), else nullptr
 };
 // worker = one warp; `n_workers` warps of the grid share the streams.  Lane i of a warp fetches the lengths of the
 // warp's i-th stream up front (the three dependent global loads per stream would otherwise serialise the loop).
 __device__ __forceinline__ void kv_prefetch(const KvPrefetch &pf, int worker, int n_workers) {
-  if (pf.kbase == nullptr) return;
+  if (pf.kv.k == nullptr) return;
   const int lane = threadIdx.x & 31;
   const int n_streams = 2 * pf.B * pf.H;
   int kv_mine = 0;
@@ -88,27 +137,26 @@ __device__ __forceinline__ void kv_prefetch(const KvPrefetch &pf, int worker, in
     const int s_mine = worker + lane * n_workers;
     if (s_mine < n_streams) {
       const int b = (s_mine >> 1) / pf.H;
-      kv_mine = min(pf.text_len[b] + pf.prompt_len[b] + pf.n_gen[b], pf.cap);
+      kv_mine = pf.rows.count(b, pf.rows.n_gen[b], pf.kv.cap);
     }
   }
+  const int row_bytes = 64 * pf.kv.elem;
   for (int i = 0, sidx = worker; sidx < n_streams; ++i, sidx += n_workers) {
     int kv;
     if (i < 32) {
       kv = __shfl_sync(0xffffffffu, kv_mine, i);
     } else {
       const int b = (sidx >> 1) / pf.H;
-      kv = min(pf.text_len[b] + pf.prompt_len[b] + pf.n_gen[b], pf.cap);
+      kv = pf.rows.count(b, pf.rows.n_gen[b], pf.kv.cap);
     }
     const int pair = sidx >> 1;
     const int b = pair / pf.H, h = pair - b * pf.H;
     const int r_lo = min(kv, pf.row_lo), r_hi = min(kv, pf.row_hi);
-    const char *p = (const char *)((sidx & 1) ? pf.vbase : pf.kbase) + (int64_t)b * pf.seq_stride_bytes +
-                    ((int64_t)h * pf.cap + r_lo) * pf.row_bytes;
-    const int lines = ((r_hi - r_lo) * pf.row_bytes) >> 7;  // 128-byte lines
+    const char *p = (const char *)((sidx & 1) ? pf.kv.v : pf.kv.k) + pf.kv.row(b, h, r_lo) * pf.kv.elem;
+    const int lines = ((r_hi - r_lo) * row_bytes) >> 7;  // 128-byte lines
     for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + ((int64_t)l << 7)));
-    if (pf.kexp != nullptr && lane == 0 && r_hi > r_lo) {  // the rows' exponent bytes: one or two lines
-      const char *e = (const char *)((sidx & 1) ? pf.vexp : pf.kexp) + (int64_t)b * (pf.seq_stride_bytes >> 6) +
-                      (int64_t)h * pf.cap;
+    if (pf.kv.kexp != nullptr && lane == 0 && r_hi > r_lo) {  // the rows' exponent bytes: one or two lines
+      const char *e = (const char *)((sidx & 1) ? pf.kv.vexp : pf.kv.kexp) + pf.kv.exp_index(b, h, 0);
       const int64_t l0 = (r_lo + ((int64_t)(uintptr_t)e & 127)) >> 7, l1 = (r_hi - 1 + ((int64_t)(uintptr_t)e & 127)) >> 7;
       const char *e0 = (const char *)((uintptr_t)e & ~(uintptr_t)127);
       for (int64_t l = l0; l <= l1; ++l) asm volatile("prefetch.global.L2 [%0];" ::"l"(e0 + (l << 7)));
@@ -121,15 +169,12 @@ struct LnParams {
   float eps;
 };
 
+// The QKV projection of a decode step: q of the current token to q, its k and v appended to the layer's cache
 struct QkvScatter {
   int d, head_dim;
   float *q;  // [B, d] fp32
-  void *kcache, *vcache;  // this layer's cache base
-  int64_t cache_seq_stride;
-  int cache_cap;
-  const int32_t *text_len, *prompt_len, *n_gen;
-  const int32_t *finished;  // NULL or [B]: rows that have stopped keep their cache untouched
-  uint8_t *kexp = nullptr, *vexp = nullptr;  // FP8 cache (e4m3 kcache / vcache): this layer's exponent arrays [B, H, cap]
+  KvCache kv;
+  KvRows rows;
 };
 
 // gemm_simt.cu
@@ -205,21 +250,19 @@ int launch_ln_fold(const bf16 *W, int N, int K, const float *gamma, const float 
                    float *c, float *dvec, cudaStream_t s);
 
 // attention.cu
+// fills the layer's KV cache `kv` when kv.k != nullptr (kv.kexp != nullptr: the FP8 cache)
 int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_head, int head_dim,
                             const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
-                            int seg1_start, int max_seqlen, int mask_mode, void *out, void *kcache, void *vcache,
-                            int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
-                            cudaStream_t s, const DropCfg *drop = nullptr, uint8_t *kexp = nullptr,
-                            uint8_t *vexp = nullptr);
-// attention_wgmma.cu (bf16 flash attention on wgmma / TMA; fills the KV cache when kcache != nullptr: bf16, or with
-// kexp != nullptr the FP8 cache, e4m3 rows + exponent bytes)
+                            int seg1_start, int max_seqlen, int mask_mode, void *out, const KvCache &kv,
+                            const uint8_t *dense_mask, int64_t dense_ld, cudaStream_t s, const DropCfg *drop = nullptr);
+// attention_wgmma.cu (bf16 flash attention on wgmma / TMA; fills the KV cache when kv.k != nullptr: bf16, or with
+// kv.kexp != nullptr the FP8 cache, e4m3 rows + exponent bytes)
 int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
                            const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, bf16 *out, void *kcache, void *vcache, int64_t cache_seq_stride,
-                           int cache_cap, cudaStream_t s, uint8_t *kexp = nullptr, uint8_t *vexp = nullptr);
+                           int mask_mode, bf16 *out, const KvCache &kv, cudaStream_t s);
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
-// the current token's q, k, v (kv.q, or pending in qkv) against the layer's caches kv.kcache / kv.vcache.  dtype
-// VB_E4M3: the FP8 cache (kv.kexp / kv.vexp); q, k, v must then be pending in qkv
+// the current token's q, k, v (kv.q, or pending in qkv) against the layer's cache kv.kv.  dtype VB_E4M3: the FP8
+// cache; q, k, v must then be pending in qkv
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
                        void *workspace, bool pdl, cudaStream_t s);
 
