@@ -554,7 +554,8 @@ int vb_eve_step(const vb_eve_tensor *tensors, int n_tensors, float beta1, float 
  *      fp32, activations [B, C, T] (time contiguous).
  * ---------------------------------------------------------------------------------------- */
 /* SConv1d: y = conv1d(pad(act(x))) + bias (+ residual); act = ELU if pre_elu; padding (pad_left,
- * pad_right) reflect or zero.  wp: the conv weight [Cout, Cin, K] (weight-norm already folded,
+ * pad_right) reflect or zero.  Reflect padding follows EnCodec's pad1d: x is zero-extended to
+ * Te = max(Tin, max(pad_left, pad_right) + 1) samples and reflected over those, so pads >= Tin are accepted.  wp: the conv weight [Cout, Cin, K] (weight-norm already folded,
  * tokenizer.py:181-208) PRE-PACKED channel-fastest as [Cin, K, Cout].
  * phase > 1 -- the causal SConvTranspose1d with K == 2*stride and the right padding trimmed, as a stride-1 K=2
  * convolution onto Cout = C * phase "phase channels" c' = c * phase + r: wp[ci][0][c'] = w_T[ci][c][r + phase],

@@ -21,6 +21,7 @@ __device__ __forceinline__ float elu1(float x) { return x > 0.f ? x : expm1f(x);
 
 // ---- causal / asymmetric-padded Conv1d as a register-tiled implicit GEMM (+pre-ELU, +bias, +residual) -------
 //   out[b, co, t] = bias[co] + sum_{ci,k} W[co, ci, k] * act(x)[b, ci, t*stride - pad_left + k*dil]
+// Reflect padding maps g < 0 to -g and g >= Te to 2 (Te - 1) - g over x zero-extended to Te samples (vb_conv1d).
 // One CTA = CO_T output channels x T_T time steps of one utterance; a thread owns 8 channels x 8 time steps
 // (64 accumulators; per (ci, k): 2 broadcast LDS.128 of weights + 8 conflict-free LDS of inputs for 64 FFMA).
 // The weights arrive pre-packed as wp[Cin][K][Cout] (channel-fastest) so a chunk of CI_T input channels is one
@@ -33,8 +34,8 @@ template <int CO_T>
 __global__ void __launch_bounds__(256, 2)
 conv1d_tiled_kernel(const float *__restrict__ x, int Cin, int Tin, const float *__restrict__ wp,
                     const float *__restrict__ bias, int Cout, int K, int stride, int dil, int pad_left, int reflect,
-                    int pre_elu, const float *__restrict__ residual, float *__restrict__ out, int Tout, int in_w,
-                    int phase) {
+                    int Te, int pre_elu, const float *__restrict__ residual, float *__restrict__ out, int Tout,
+                    int in_w, int phase) {
   constexpr int TYN = CO_T / TH_CO;   // thread rows (channel groups)
   constexpr int TXN = 256 / TYN;      // thread columns; time steps of a thread: tx + j * TXN
   constexpr int T_T = TXN * TH_T;
@@ -63,9 +64,9 @@ conv1d_tiled_kernel(const float *__restrict__ x, int Cin, int Tin, const float *
       for (int i = tid; i < in_w; i += 256) {
         int g = g0 + i;
         float v = 0.f;
-        if (reflect) {  // F.pad(mode="reflect") index map (pads are < Tin on this path)
+        if (reflect) {  // F.pad(mode="reflect") of x zero-extended to Te = max(Tin, max pad + 1) samples
           if (g < 0) g = -g;
-          if (g >= Tin) g = 2 * (Tin - 1) - g;
+          if (g >= Te) g = 2 * (Te - 1) - g;
         }
         if (g >= 0 && g < Tin) {
           v = xrow[g];
@@ -375,8 +376,8 @@ using namespace vb;
 
 template <int CO_T>
 static int launch_conv1d(const float *x, int B, int Cin, int Tin, const float *wp, const float *bias, int Cout, int K,
-                         int stride, int dil, int pad_left, int reflect, int pre_elu, const float *residual, float *out,
-                         int Tout, int phase, cudaStream_t s) {
+                         int stride, int dil, int pad_left, int reflect, int Te, int pre_elu, const float *residual,
+                         float *out, int Tout, int phase, cudaStream_t s) {
   constexpr int TXN = 256 / (CO_T / ec::TH_CO), T_T = TXN * ec::TH_T;
   const int in_w = (T_T - 1) * stride + (K - 1) * dil + 1;
   const size_t smem = (size_t)(ec::CI_T * K * CO_T + ec::CI_T * in_w) * sizeof(float);
@@ -385,8 +386,8 @@ static int launch_conv1d(const float *x, int B, int Cin, int Tin, const float *w
   static PerDeviceOnce once;
   if (once.first()) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   dim3 grid((Tout + T_T - 1) / T_T, (Cout + CO_T - 1) / CO_T, B);
-  kern<<<grid, 256, smem, s>>>(x, Cin, Tin, wp, bias, Cout, K, stride, dil, pad_left, reflect, pre_elu, residual, out,
-                               Tout, in_w, phase);
+  kern<<<grid, 256, smem, s>>>(x, Cin, Tin, wp, bias, Cout, K, stride, dil, pad_left, reflect, Te, pre_elu, residual,
+                               out, Tout, in_w, phase);
   VB_LAUNCH_CHECK();
   return VB_OK;
 }
@@ -398,19 +399,20 @@ VB_API int vb_conv1d(const float *x, int B, int Cin, int Tin, const float *wp, c
   VB_CHECK_ARG(Tout == (Tin + pad_left + pad_right - (K - 1) * dilation - 1) / stride + 1,
                "vb_conv1d: Tout=%d inconsistent with Tin=%d pads=(%d,%d) K=%d stride=%d dil=%d", Tout, Tin, pad_left,
                pad_right, K, stride, dilation);
-  VB_CHECK_ARG(!reflect || (pad_left < Tin && pad_right < Tin), "vb_conv1d: reflect pad >= length");
   VB_CHECK_ARG(phase >= 1 && Cout % phase == 0 && (phase == 1 || (stride == 1 && residual == nullptr)),
                "vb_conv1d: bad phase %d", phase);
   if (B == 0 || Tout <= 0) return VB_OK;
   cudaStream_t s = (cudaStream_t)stream;
+  // a reflect pad as long as the input reflects over the input zero-extended to max pad + 1 samples (EnCodec's pad1d)
+  const int Te = max(Tin, max(pad_left, pad_right) + 1);
   if (Cout > 32)
-    return launch_conv1d<64>(x, B, Cin, Tin, wp, bias, Cout, K, stride, dilation, pad_left, reflect, pre_elu, residual,
-                             out, Tout, phase, s);
+    return launch_conv1d<64>(x, B, Cin, Tin, wp, bias, Cout, K, stride, dilation, pad_left, reflect, Te, pre_elu,
+                             residual, out, Tout, phase, s);
   if (Cout > 16)
-    return launch_conv1d<32>(x, B, Cin, Tin, wp, bias, Cout, K, stride, dilation, pad_left, reflect, pre_elu, residual,
-                             out, Tout, phase, s);
-  return launch_conv1d<16>(x, B, Cin, Tin, wp, bias, Cout, K, stride, dilation, pad_left, reflect, pre_elu, residual, out,
-                           Tout, phase, s);
+    return launch_conv1d<32>(x, B, Cin, Tin, wp, bias, Cout, K, stride, dilation, pad_left, reflect, Te, pre_elu,
+                             residual, out, Tout, phase, s);
+  return launch_conv1d<16>(x, B, Cin, Tin, wp, bias, Cout, K, stride, dilation, pad_left, reflect, Te, pre_elu,
+                           residual, out, Tout, phase, s);
 }
 
 VB_API int vb_lstm_layer(const float *xproj, const float *whh_t, int T, int B, int H, float *h_seq, float *c_state,
