@@ -103,11 +103,12 @@ def _forward(name):
     return r
 
 
-def _train(name):
+def _train(name, mode=None):
     """train_{pre,post}_{ln,adaln}_{f32,bf16}_{p0,p01}: autograd.DecoderStack forward + backward on the padded batch of
-    the NAR training pass (VB_MASK_PADDED)"""
+    the NAR training pass (VB_MASK_PADDED, or the mask mode given)"""
     from valle_b200 import _lib as L
     from valle_b200 import autograd as AG
+    mode = L.VB_MASK_PADDED if mode is None else mode
     _, order, norm, dt, pp = name.split("_")
     p = {"p0": 0.0, "p01": 0.1}[pp]
     enc, ada = _stack(order == "pre", norm == "adaln", 7)
@@ -122,7 +123,7 @@ def _train(name):
     xa = torch.randn(N * Lp, D, generator=g).to(DEV).requires_grad_()
     w = torch.randn(N * Lp, D, generator=g).to(DEV)
     ada = ada.to(DEV).requires_grad_() if ada is not None else None
-    geom = (cu, N, Lp, L.VB_MASK_PADDED, xl, yl, Smax, p, SEED)
+    geom = (cu, N, Lp, mode, xl, yl, Smax, p, SEED)
     r = {}
     out, r["launches_fwd"] = _launches(lambda: AG.DecoderStack.apply(xa, ada, nd, geom, *params))
     _, r["launches_bwd"] = _launches(lambda: (out * w).sum().backward())

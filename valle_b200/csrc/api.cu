@@ -259,10 +259,9 @@ DropCfg layer_drop(float p, uint64_t seed, int l, int site) { return make_drop(p
 // x = norm1(x + SA(x)); x = norm2(x + FF(x)); a post-norm writes the normalised rows back into x and into the
 // storage-dtype operand of the next GEMM, and layer 0 reads a plain cast.
 template <class Slots>
-int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32_t *cu_seqlens, const int32_t *text_lens,
-                  const int32_t *seg1_lens, int seg1_start, int max_seqlen, int mask_mode, const float *ada_wb,
-                  Slots slots, const KvCache &cache, int64_t cache_layer_stride, float *sub, float dropout_p,
-                  uint64_t dropout_seed, cudaStream_t s) {
+int stack_forward(const vb_decoder *dec, float *x, int64_t M, const Packed &pk, const float *ada_wb, Slots slots,
+                  const KvCache &cache, int64_t cache_layer_stride, float *sub, float dropout_p, uint64_t dropout_seed,
+                  cudaStream_t s) {
   const vb_decoder_desc &D = dec->desc;
   const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
   const vb_stream_t stream = (vb_stream_t)s;
@@ -290,8 +289,7 @@ int stack_forward(const vb_decoder *dec, float *x, int64_t M, int B, const int32
       VB_TRY(vb_linear(sv.xn1, dt, d, P.in_proj_w, dt, P.in_proj_b, sv.qkv, dt, 3 * d, M, 3 * d, d, VB_EPI_NONE, nullptr,
                        0, stream));
       const DropCfg dc = layer_drop(dropout_p, dropout_seed, l, 0);
-      VB_TRY(launch_attention_varlen(sv.qkv, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
-                                     seg1_start, max_seqlen, mask_mode, sv.att,
+      VB_TRY(launch_attention_varlen(sv.qkv, dt, M, D.n_head, d / D.n_head, pk, sv.att,
                                      kv_cache_layer(cache, cache_layer_stride, l), nullptr, 0, s, &dc));
       return residual(sv.att, d, P.out_proj_w, P.out_proj_b, 1);
     };
@@ -348,18 +346,17 @@ VB_API size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t 
 }
 
 // the body of vb_decoder_forward and vb_decoder_forward_kv8 (fn: the entry point's name, for the error message)
-static int decoder_forward(const char *fn, vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, const float *ada_wb, const KvCache &cache, int64_t cache_layer_stride,
-                           void *workspace, size_t workspace_bytes, vb_stream_t stream) {
+static int decoder_forward(const char *fn, vb_decoder_t dec, float *x, int64_t M, const Packed &pk, const float *ada_wb,
+                           const KvCache &cache, int64_t cache_layer_stride, void *workspace, size_t workspace_bytes,
+                           vb_stream_t stream) {
   const vb_decoder_desc &D = dec->desc;
   VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M), "%s: workspace too small (%zu < %zu)", fn,
                workspace_bytes, vb_decoder_forward_workspace(&D, M));
   if (M == 0) return VB_OK;
   Carve c(workspace);
   const LayerSave ws = carve_forward_ws(c, D, M);
-  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
-                       [&](int) { return ws; }, cache, cache_layer_stride, nullptr, 0.f, 0, (cudaStream_t)stream);
+  return stack_forward(dec, x, M, pk, ada_wb, [&](int) { return ws; }, cache, cache_layer_stride, nullptr, 0.f, 0,
+                       (cudaStream_t)stream);
 }
 
 VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
@@ -370,8 +367,9 @@ VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, cons
                                   void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && x && cu_seqlens, "vb_decoder_forward: null argument");
   const KvCache cache{kcache, vcache, nullptr, nullptr, cache_seq_stride, cache_cap, (int)elem_size(dec->desc.wdtype)};
-  return decoder_forward("vb_decoder_forward", dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
-                         mask_mode, ada_wb, cache, cache_layer_stride, workspace, workspace_bytes, stream);
+  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
+  return decoder_forward("vb_decoder_forward", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
+                         workspace_bytes, stream);
 }
 
 // the FP8 cache's exponent rows are read 16 bytes at a time (cp.async in the decode attention): every (layer, utterance,
@@ -395,8 +393,9 @@ VB_API int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, 
                "vb_decoder_forward_kv8: FP8 cache: strides must be multiples of 1024, cache_cap a multiple of 16 and "
                "k_exp / v_exp 16-byte aligned");
   const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap, (int)elem_size(VB_E4M3)};
-  return decoder_forward("vb_decoder_forward_kv8", dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                         max_seqlen, mask_mode, ada_wb, cache, cache_layer_stride, workspace, workspace_bytes, stream);
+  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
+  return decoder_forward("vb_decoder_forward_kv8", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
+                         workspace_bytes, stream);
 }
 
 VB_API size_t vb_decoder_train_save_bytes(const vb_decoder_desc *desc, int64_t M) {
@@ -414,9 +413,9 @@ VB_API int vb_decoder_forward_train(vb_decoder_t dec, float *x, int64_t M, int B
   if (M == 0) return VB_OK;
   Carve c(save);
   float *sub = carve_train_save(c, D, M);
-  return stack_forward(dec, x, M, B, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen, mask_mode, ada_wb,
-                       [&](int l) { return layer_save(D, M, save, l); }, KvCache{}, 0, sub, dropout_p, dropout_seed,
-                       (cudaStream_t)stream);
+  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
+  return stack_forward(dec, x, M, pk, ada_wb, [&](int l) { return layer_save(D, M, save, l); }, KvCache{}, 0, sub,
+                       dropout_p, dropout_seed, (cudaStream_t)stream);
 }
 
 VB_API size_t vb_decoder_backward_workspace(const vb_decoder_desc *desc, int64_t M) {
@@ -438,6 +437,7 @@ VB_API int vb_decoder_backward(vb_decoder_t dec, float *dx, int64_t M, int B, co
   const int d = D.d_model, dff = D.d_ff, dt = D.wdtype;
   Carve c(workspace);
   const BackwardWs w = carve_backward_ws(c, D, M);
+  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
   const bool drop = dropout_p > 0.f;
   const float inv_keep = drop ? 1.f / (1.f - dropout_p) : 1.f;
   // dx holds the gradient of the stack output on entry.  dx_dt, the residual stream's gradient in the storage dtype
@@ -474,8 +474,8 @@ VB_API int vb_decoder_backward(vb_decoder_t dec, float *dx, int64_t M, int B, co
       VB_TRY(vb_linear_backward(sv.att, dt, d, T.out_proj_wt, dy, d, w.dO, dt, d, VB_EPI_NONE, G.out_proj_w, G.out_proj_b,
                                 M, d, d, w.lin_ws, w.lin_ws_bytes, stream));
       const DropCfg dc = layer_drop(dropout_p, dropout_seed, l, 0);
-      VB_TRY(attention_backward(sv.qkv, sv.att, w.dO, dt, M, B, D.n_head, d / D.n_head, cu_seqlens, text_lens, seg1_lens,
-                                seg1_start, max_seqlen, mask_mode, w.dqkv, w.attn_ws, w.attn_ws_bytes, &dc, s));
+      VB_TRY(attention_backward(sv.qkv, sv.att, w.dO, dt, M, D.n_head, d / D.n_head, pk, w.dqkv, w.attn_ws,
+                                w.attn_ws_bytes, &dc, s));
       return vb_linear_backward(sv.xn1, dt, d, T.in_proj_wt, w.dqkv, 3 * d, dst, VB_F32, d, epi, G.in_proj_w,
                                 G.in_proj_b, M, 3 * d, d, w.lin_ws, w.lin_ws_bytes, stream);
     };

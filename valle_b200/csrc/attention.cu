@@ -24,10 +24,8 @@ static constexpr int HD = 64;
 // ------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void __launch_bounds__(256)
-attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
-                        const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens,
-                        int seg1_start, int mask_mode, T *__restrict__ out, KvCache kv,
-                        const uint8_t *__restrict__ dmask, int64_t dld, DropCfg drop) {
+attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const Packed pk, T *__restrict__ out,
+                        KvCache kv, const uint8_t *__restrict__ dmask, int64_t dld, DropCfg drop) {
   constexpr int LDT = 68;  // padded leading dim (floats), keeps float4 alignment
   extern __shared__ __align__(16) float smem[];
   float *Qt = smem;             // [64 e][LDT rows]
@@ -36,11 +34,10 @@ attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__
   float *Pt = Vs + 64 * LDT;    // [64 keys][LDT rows]
 
   const int b = blockIdx.z, h = blockIdx.y;
-  const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
+  const Packed::Seq sb = pk.seq(b);
+  const int r0 = sb.r0, L = sb.L;
   const int q0 = blockIdx.x * 64;
   if (q0 >= L) return;
-  const int S = (mask_mode != VB_MASK_FULL) ? text_lens[b] : 0;
-  const int c1 = (mask_mode >= VB_MASK_PADDED_AR) ? seg1_lens[b] : 0;
   const int d = n_head * HD;
   const int64_t ld = 3 * (int64_t)d;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -55,9 +52,8 @@ attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__
   }
   RowMask lim[4];  // visibility rule per owned row
 #pragma unroll
-  for (int i = 0; i < 4; ++i) lim[i] = make_row_mask(mask_mode, q0 + ty * 4 + i, L, S, seg1_start, c1);
-  const int q_hi = min(q0 + 64, L);
-  const int kv_max = (mask_mode == VB_MASK_VALLE_AR) ? max(S, q_hi) : L;
+  for (int i = 0; i < 4; ++i) lim[i] = pk.row_mask(sb, q0 + ty * 4 + i);
+  const int kv_max = pk.kv_max(sb, min(q0 + 64, L));
 
   float m_run[4], l_run[4], o[4][4];
 #pragma unroll
@@ -178,55 +174,44 @@ attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const int32_t *__
   }
 }
 
-int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_head, int head_dim,
-                            const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
-                            int seg1_start, int max_seqlen, int mask_mode, void *out, const KvCache &kv,
-                            const uint8_t *dense_mask, int64_t dense_ld, cudaStream_t s, const DropCfg *drop) {
+int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int n_head, int head_dim, const Packed &pk,
+                            void *out, const KvCache &kv, const uint8_t *dense_mask, int64_t dense_ld, cudaStream_t s,
+                            const DropCfg *drop) {
   VB_CHECK_ARG(head_dim == HD, "attention: head_dim=%d, only 64 is built", head_dim);
   DropCfg dc{};
   if (drop) dc = *drop;
-  dc.lmax = max_seqlen;
-  const bool dropping = dc.thresh != 0;   // attention-probability dropout: the CUDA-core kernel carries the mask
-  VB_CHECK_ARG(mask_mode >= VB_MASK_FULL && mask_mode <= VB_MASK_DENSE, "attention: bad mask mode %d", mask_mode);
-  if (mask_mode == VB_MASK_DENSE) {
-    VB_CHECK_ARG(dense_mask != nullptr && dense_ld >= max_seqlen, "attention: VB_MASK_DENSE needs a [>=L, >=L] byte mask");
-    mask_mode = VB_MASK_FULL;  // every key of the sequence, minus the blocked entries of the dense mask
+  dc.lmax = pk.max_seqlen;
+  Packed p = pk;
+  if (p.mask_mode == VB_MASK_DENSE) {
+    VB_CHECK_ARG(dense_mask != nullptr && dense_ld >= p.max_seqlen, "attention: VB_MASK_DENSE needs a [>=L, >=L] byte mask");
+    p.mask_mode = VB_MASK_FULL;  // every key of the sequence, minus the blocked entries of the dense mask
   } else {
     dense_mask = nullptr;
   }
-  VB_CHECK_ARG(mask_mode == VB_MASK_FULL || text_lens != nullptr, "attention: this mask mode needs text_lens");
-  VB_CHECK_ARG(mask_mode < VB_MASK_PADDED_AR || seg1_lens != nullptr, "attention: padded mask modes need seg1_lens");
-  if (M == 0 || B == 0) return VB_OK;
+  VB_TRY(check_packed(p, "attention"));
+  if (M == 0 || p.B == 0) return VB_OK;
+  // attention-probability dropout and the dense mask are carried by the CUDA-core kernel only
+  const bool wgmma = dtype == VB_BF16 && dc.thresh == 0 && dense_mask == nullptr && tune("VB_ATTN_SIMT", 0) == 0;
   if (kv.kexp != nullptr) {   // an FP8 cache is filled by the wgmma kernel only
-    if (dtype != VB_BF16 || dropping || dense_mask != nullptr || tune("VB_ATTN_SIMT", 0) != 0) {
+    if (!wgmma) {
       set_error("attention: an FP8 KV cache is filled by the bf16 wgmma prefill only (no dropout, no dense mask, not VB_ATTN_SIMT)");
       return VB_ERR_UNSUPPORTED;
     }
     VB_CHECK_ARG(kv.k && kv.v && kv.vexp, "attention: FP8 cache: kcache, vcache, k_exp and v_exp are all needed");
-    return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                  max_seqlen, mask_mode, (bf16 *)out, kv, s);
   }
-  const size_t smem = 4 * 64 * 68 * sizeof(float);
-  dim3 grid((max_seqlen + 63) / 64, n_head, B);
-  if (dtype == VB_F32) {
-    auto k = attn_varlen_simt_kernel<float>;
+  if (wgmma) return launch_attention_wgmma((const bf16 *)qkv, M, n_head, p, (bf16 *)out, kv, s);
+  VB_CHECK_ARG(dtype == VB_F32 || dtype == VB_BF16, "attention: bad dtype %d", dtype);
+  auto simt = [&](auto elem) -> int {
+    using T = decltype(elem);
+    const size_t smem = 4 * 64 * 68 * sizeof(float);
+    auto k = attn_varlen_simt_kernel<T>;
     VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<grid, 256, smem, s>>>((const float *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode,
-                              (float *)out, kv, dense_mask, dense_ld, dc);
-  } else if (dtype == VB_BF16 && !dropping && dense_mask == nullptr && tune("VB_ATTN_SIMT", 0) == 0) {
-    return launch_attention_wgmma((const bf16 *)qkv, M, B, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, max_seqlen,
-                                  mask_mode, (bf16 *)out, kv, s);
-  } else if (dtype == VB_BF16) {
-    auto k = attn_varlen_simt_kernel<bf16>;
-    VB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<grid, 256, smem, s>>>((const bf16 *)qkv, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode,
-                              (bf16 *)out, kv, dense_mask, dense_ld, dc);
-  } else {
-    set_error("attention: bad dtype %d", dtype);
-    return VB_ERR_ARG;
-  }
-  VB_LAUNCH_CHECK();
-  return VB_OK;
+    k<<<dim3((p.max_seqlen + 63) / 64, n_head, p.B), 256, smem, s>>>((const T *)qkv, n_head, p, (T *)out, kv,
+                                                                     dense_mask, dense_ld, dc);
+    VB_LAUNCH_CHECK();
+    return VB_OK;
+  };
+  return dtype == VB_F32 ? simt(float{}) : simt(bf16{});
 }
 
 // ------------------------------------------------------------------------------------------
@@ -836,6 +821,7 @@ VB_API int vb_attention(const void *qkv, int dtype, int64_t M, int B, int n_head
                         int64_t cache_seq_stride, int cache_cap, const uint8_t *dense_mask, int64_t dense_ld,
                         vb_stream_t stream) {
   const vb::KvCache kv{kcache, vcache, nullptr, nullptr, cache_seq_stride, cache_cap, (int)vb::elem_size(dtype)};
-  return vb::launch_attention_varlen(qkv, dtype, M, B, n_head, head_dim, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                     max_seqlen, mask_mode, out, kv, dense_mask, dense_ld, (cudaStream_t)stream);
+  const vb::Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
+  return vb::launch_attention_varlen(qkv, dtype, M, n_head, head_dim, pk, out, kv, dense_mask, dense_ld,
+                                     (cudaStream_t)stream);
 }

@@ -106,19 +106,15 @@ __device__ __forceinline__ void online_softmax(float (&s)[32], int j0, int t, co
 // the attention itself computes on the bf16 tiles either way
 template <bool kF8>
 __global__ void __launch_bounds__(kThreads, 2)
-attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, const int32_t *__restrict__ cu_seqlens,
-                  const int32_t *__restrict__ text_lens, const int32_t *__restrict__ seg1_lens, int seg1_start,
-                  int mask_mode, bf16 *__restrict__ out, const __grid_constant__ KvCache kv) {
+attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, const Packed pk,
+                  bf16 *__restrict__ out, const __grid_constant__ KvCache kv) {
   const int b = blockIdx.z, h = blockIdx.y;
-  const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
+  const Packed::Seq sb = pk.seq(b);
+  const int r0 = sb.r0, L = sb.L;
   const int q0 = blockIdx.x * BQ;
   if (q0 >= L) return;
-  const int S = (mask_mode != VB_MASK_FULL) ? text_lens[b] : 0;
-  const int c1 = (mask_mode >= VB_MASK_PADDED_AR) ? seg1_lens[b] : 0;
   const int d = n_head * HD;
-  const int q_hi = min(q0 + BQ, L);
-  const int kv_max = (mask_mode == VB_MASK_VALLE_AR) ? max(S, q_hi) : L;
-  const int n_tiles = (kv_max + BKV - 1) / BKV;
+  const int n_tiles = (pk.kv_max(sb, min(q0 + BQ, L)) + BKV - 1) / BKV;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *sq = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -160,11 +156,10 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
   // ===== consumers =====
   const int half = wg;
   const int row_a = q0 + half * 64 + wg_row(t, 0), row_b = row_a + 8;  // the two query rows of this thread
-  const RowMask lim_a = make_row_mask(mask_mode, row_a, L, S, seg1_start, c1);
-  const RowMask lim_b = make_row_mask(mask_mode, row_b, L, S, seg1_start, c1);
+  const RowMask lim_a = pk.row_mask(sb, row_a), lim_b = pk.row_mask(sb, row_b);
   // every row of the warpgroup sees keys [0, kfree): lim0 does not decrease with the row in any mask mode, so the
   // warpgroup's first row has the smallest.  Tiles below it skip the mask tests (they would all pass).
-  const int kfree = make_row_mask(mask_mode, q0 + half * 64, L, S, seg1_start, c1).lim0;
+  const int kfree = pk.row_mask(sb, q0 + half * 64).lim0;
   const uint64_t qdesc = make_smem_desc(smem_u32(sq + half * kBoxBytes));
 
   float o[32];
@@ -314,32 +309,27 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
 
 }  // namespace fa3
 
-int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
-                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, bf16 *out, const KvCache &kv, cudaStream_t s) {
-  if (M == 0 || B == 0) return VB_OK;
+template <bool kF8>
+static int launch_wgmma(const CUtensorMap &tm, int n_head, const Packed &pk, bf16 *out, const KvCache &kv,
+                        cudaStream_t s) {
+  static PerDeviceOnce once;
+  if (once.first())
+    VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<kF8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 fa3::kSmemBytes));
+  const dim3 grid((pk.max_seqlen + fa3::BQ - 1) / fa3::BQ, n_head, pk.B);
+  fa3::attn_wgmma_kernel<kF8><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(tm, n_head, pk, out, kv);
+  VB_LAUNCH_CHECK();
+  return VB_OK;
+}
+
+int launch_attention_wgmma(const bf16 *qkv, int64_t M, int n_head, const Packed &pk, bf16 *out, const KvCache &kv,
+                           cudaStream_t s) {
+  if (M == 0 || pk.B == 0) return VB_OK;
   VB_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0, "wgmma attention: qkv must be 16-byte aligned");
   CUtensorMap tm;
   VB_TRY(tc::make_tmap(&tm, qkv, M, 3 * n_head * fa3::HD, 3 * (int64_t)n_head * fa3::HD, 64));
-  dim3 grid((max_seqlen + fa3::BQ - 1) / fa3::BQ, n_head, B);
-  if (kv.kexp != nullptr) {
-    static PerDeviceOnce once8;
-    if (once8.first())
-      VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                   fa3::kSmemBytes));
-    fa3::attn_wgmma_kernel<true><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(
-        tm, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start, mask_mode, out, kv);
-    VB_LAUNCH_CHECK();
-    return VB_OK;
-  }
-  static PerDeviceOnce once;
-  if (once.first())
-    VB_CUDA(cudaFuncSetAttribute(fa3::attn_wgmma_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 fa3::kSmemBytes));
-  fa3::attn_wgmma_kernel<false><<<grid, fa3::kThreads, fa3::kSmemBytes, s>>>(tm, n_head, cu_seqlens, text_lens,
-                                                                             seg1_lens, seg1_start, mask_mode, out, kv);
-  VB_LAUNCH_CHECK();
-  return VB_OK;
+  return kv.kexp != nullptr ? launch_wgmma<true>(tm, n_head, pk, out, kv, s)
+                            : launch_wgmma<false>(tm, n_head, pk, out, kv, s);
 }
 
 }  // namespace vb

@@ -275,9 +275,8 @@ __device__ __forceinline__ void mm_tt(const float *A, const float *B, int ty, in
 template <typename T>
 __global__ void __launch_bounds__(256)
 attn_bwd_dq_kernel(const T *__restrict__ qkv, const T *__restrict__ o, const T *__restrict__ dout, int n_head,
-                   const int32_t *__restrict__ cu_seqlens, const int32_t *__restrict__ text_lens,
-                   const int32_t *__restrict__ seg1_lens, int seg1_start, int mask_mode, T *__restrict__ dqkv,
-                   float *__restrict__ lse_out, float *__restrict__ dsum_out, DropCfg drop) {
+                   const Packed pk, T *__restrict__ dqkv, float *__restrict__ lse_out,
+                   float *__restrict__ dsum_out, DropCfg drop) {
   extern __shared__ __align__(16) float smem[];
   float *Qt = smem;              // [e][q]
   float *dOt = Qt + 64 * LDT;    // [e][q]
@@ -287,11 +286,10 @@ attn_bwd_dq_kernel(const T *__restrict__ qkv, const T *__restrict__ o, const T *
   float *dSt = Kn + 64 * LDT;    // [key][q]
   __shared__ float s_lse[64], s_D[64];
   const int b = blockIdx.z, h = blockIdx.y;
-  const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
+  const Packed::Seq sb = pk.seq(b);
+  const int r0 = sb.r0, L = sb.L;
   const int q0 = blockIdx.x * 64;
   if (q0 >= L) return;
-  const int S = (mask_mode != VB_MASK_FULL) ? text_lens[b] : 0;
-  const int c1 = (mask_mode >= VB_MASK_PADDED_AR) ? seg1_lens[b] : 0;
   const int d = n_head * HD;
   const int64_t ld = 3 * (int64_t)d;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -314,9 +312,8 @@ attn_bwd_dq_kernel(const T *__restrict__ qkv, const T *__restrict__ o, const T *
   }
   RowMask lim[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i) lim[i] = make_row_mask(mask_mode, q0 + ty * 4 + i, L, S, seg1_start, c1);
-  const int q_hi = min(q0 + 64, L);
-  const int kv_max = (mask_mode == VB_MASK_VALLE_AR) ? max(S, q_hi) : L;
+  for (int i = 0; i < 4; ++i) lim[i] = pk.row_mask(sb, q0 + ty * 4 + i);
+  const int kv_max = pk.kv_max(sb, min(q0 + 64, L));
   // ---- sweep 1: log-sum-exp of every query row ----
   float m_run[4], l_run[4];
 #pragma unroll
@@ -409,10 +406,9 @@ attn_bwd_dq_kernel(const T *__restrict__ qkv, const T *__restrict__ o, const T *
 // pass 2: per (key block, head, sequence): dK, dV
 template <typename T>
 __global__ void __launch_bounds__(256)
-attn_bwd_dkv_kernel(const T *__restrict__ qkv, const T *__restrict__ dout, int n_head,
-                    const int32_t *__restrict__ cu_seqlens, const int32_t *__restrict__ text_lens,
-                    const int32_t *__restrict__ seg1_lens, int seg1_start, int mask_mode, T *__restrict__ dqkv,
-                    const float *__restrict__ lse_in, const float *__restrict__ dsum_in, DropCfg drop) {
+attn_bwd_dkv_kernel(const T *__restrict__ qkv, const T *__restrict__ dout, int n_head, const Packed pk,
+                    T *__restrict__ dqkv, const float *__restrict__ lse_in, const float *__restrict__ dsum_in,
+                    DropCfg drop) {
   extern __shared__ __align__(16) float smem[];
   float *Kt = smem;              // [e][key]
   float *Vt = Kt + 64 * LDT;     // [e][key]
@@ -424,11 +420,10 @@ attn_bwd_dkv_kernel(const T *__restrict__ qkv, const T *__restrict__ dout, int n
   float *dSt = Pt + 64 * LDT;    // [q][key]
   __shared__ float s_lse[64], s_D[64];
   const int b = blockIdx.z, h = blockIdx.y;
-  const int r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0;
+  const Packed::Seq sb = pk.seq(b);
+  const int r0 = sb.r0, L = sb.L;
   const int k0 = blockIdx.x * 64;
   if (k0 >= L) return;
-  const int S = (mask_mode != VB_MASK_FULL) ? text_lens[b] : 0;
-  const int c1 = (mask_mode >= VB_MASK_PADDED_AR) ? seg1_lens[b] : 0;
   const int d = n_head * HD;
   const int64_t ld = 3 * (int64_t)d;
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;   // here: ty -> 4 keys, tx -> 4 head dims
@@ -455,7 +450,7 @@ attn_bwd_dkv_kernel(const T *__restrict__ qkv, const T *__restrict__ dout, int n
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int qr = q0 + ty * 4 + i;
-      const RowMask lim = make_row_mask(mask_mode, qr, L, S, seg1_start, c1);
+      const RowMask lim = pk.row_mask(sb, qr);
       const float lse = s_lse[ty * 4 + i], Dv = s_D[ty * 4 + i];
       const uint64_t base = ((uint64_t)(b * n_head + h) * drop.lmax + qr) * drop.lmax + k0 + tx * 4;
 #pragma unroll
@@ -715,53 +710,38 @@ VB_API int vb_attention_backward(const void *qkv, const void *out, const void *d
                                  int n_head, int head_dim, const int32_t *cu_seqlens, const int32_t *text_lens,
                                  const int32_t *seg1_lens, int seg1_start, int max_seqlen, int mask_mode, void *dqkv,
                                  void *workspace, size_t workspace_bytes, vb_stream_t stream) {
-  return vb::attention_backward(qkv, out, dout, dtype, M, B, n_head, head_dim, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                max_seqlen, mask_mode, dqkv, workspace, workspace_bytes, nullptr, (cudaStream_t)stream);
+  const vb::Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
+  return vb::attention_backward(qkv, out, dout, dtype, M, n_head, head_dim, pk, dqkv, workspace, workspace_bytes, nullptr,
+                                (cudaStream_t)stream);
 }
 
-int vb::attention_backward(const void *qkv, const void *out, const void *dout, int dtype, int64_t M, int B, int n_head,
-                           int head_dim, const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
-                           int seg1_start, int max_seqlen, int mask_mode, void *dqkv, void *workspace,
-                           size_t workspace_bytes, const DropCfg *drop, cudaStream_t s) {
+int vb::attention_backward(const void *qkv, const void *out, const void *dout, int dtype, int64_t M, int n_head,
+                           int head_dim, const Packed &pk, void *dqkv, void *workspace, size_t workspace_bytes,
+                           const DropCfg *drop, cudaStream_t s) {
   DropCfg dc{};
   if (drop) dc = *drop;
-  dc.lmax = max_seqlen;
+  dc.lmax = pk.max_seqlen;
   VB_CHECK_ARG(head_dim == bw::HD, "vb_attention_backward: head_dim=%d, only 64 is built", head_dim);
-  VB_CHECK_ARG(mask_mode >= VB_MASK_FULL && mask_mode <= VB_MASK_PADDED, "vb_attention_backward: bad mask mode");
-  VB_CHECK_ARG(mask_mode == VB_MASK_FULL || text_lens != nullptr, "vb_attention_backward: this mask mode needs text_lens");
-  VB_CHECK_ARG(mask_mode < VB_MASK_PADDED_AR || seg1_lens != nullptr, "vb_attention_backward: padded modes need seg1_lens");
+  VB_TRY(check_packed(pk, "vb_attention_backward"));
   VB_CHECK_ARG(workspace && workspace_bytes >= vb_attention_backward_workspace(M, n_head),
                "vb_attention_backward: workspace too small");
-  if (M == 0 || B == 0) return VB_OK;
+  if (M == 0 || pk.B == 0) return VB_OK;
+  VB_CHECK_ARG(dtype == VB_F32 || dtype == VB_BF16, "vb_attention_backward: bad dtype %d", dtype);
   float *lse = (float *)workspace;
   float *dsum = lse + (size_t)M * n_head;
-  dim3 grid((max_seqlen + 63) / 64, n_head, B);
-  const size_t smem_q = (size_t)6 * 64 * bw::LDT * sizeof(float), smem_k = (size_t)8 * 64 * bw::LDT * sizeof(float);
-  if (dtype == VB_F32) {
-    auto kq = bw::attn_bwd_dq_kernel<float>;
-    auto kk = bw::attn_bwd_dkv_kernel<float>;
+  auto launch = [&](auto elem) -> int {
+    using T = decltype(elem);
+    const dim3 grid((pk.max_seqlen + 63) / 64, n_head, pk.B);
+    const size_t smem_q = (size_t)6 * 64 * bw::LDT * sizeof(float), smem_k = (size_t)8 * 64 * bw::LDT * sizeof(float);
+    auto kq = bw::attn_bwd_dq_kernel<T>;
+    auto kk = bw::attn_bwd_dkv_kernel<T>;
     VB_CUDA(cudaFuncSetAttribute(kq, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_q));
     VB_CUDA(cudaFuncSetAttribute(kk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_k));
-    kq<<<grid, 256, smem_q, s>>>((const float *)qkv, (const float *)out, (const float *)dout, n_head, cu_seqlens, text_lens,
-                                 seg1_lens, seg1_start, mask_mode, (float *)dqkv, lse, dsum, dc);
+    kq<<<grid, 256, smem_q, s>>>((const T *)qkv, (const T *)out, (const T *)dout, n_head, pk, (T *)dqkv, lse, dsum, dc);
     VB_LAUNCH_CHECK();
-    kk<<<grid, 256, smem_k, s>>>((const float *)qkv, (const float *)dout, n_head, cu_seqlens, text_lens, seg1_lens,
-                                 seg1_start, mask_mode, (float *)dqkv, lse, dsum, dc);
+    kk<<<grid, 256, smem_k, s>>>((const T *)qkv, (const T *)dout, n_head, pk, (T *)dqkv, lse, dsum, dc);
     VB_LAUNCH_CHECK();
-  } else if (dtype == VB_BF16) {
-    auto kq = bw::attn_bwd_dq_kernel<bf16>;
-    auto kk = bw::attn_bwd_dkv_kernel<bf16>;
-    VB_CUDA(cudaFuncSetAttribute(kq, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_q));
-    VB_CUDA(cudaFuncSetAttribute(kk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_k));
-    kq<<<grid, 256, smem_q, s>>>((const bf16 *)qkv, (const bf16 *)out, (const bf16 *)dout, n_head, cu_seqlens, text_lens,
-                                 seg1_lens, seg1_start, mask_mode, (bf16 *)dqkv, lse, dsum, dc);
-    VB_LAUNCH_CHECK();
-    kk<<<grid, 256, smem_k, s>>>((const bf16 *)qkv, (const bf16 *)dout, n_head, cu_seqlens, text_lens, seg1_lens, seg1_start,
-                                 mask_mode, (bf16 *)dqkv, lse, dsum, dc);
-    VB_LAUNCH_CHECK();
-  } else {
-    set_error("vb_attention_backward: bad dtype %d", dtype);
-    return VB_ERR_ARG;
-  }
-  return VB_OK;
+    return VB_OK;
+  };
+  return dtype == VB_F32 ? launch(float{}) : launch(bf16{});
 }

@@ -4,7 +4,6 @@
 
 namespace vb {
 
-// Visibility rule of one query row (see vb_mask_mode): key c is seen iff c < lim0 or s1 <= c < hi1.
 // Training-mode dropout (valle/modules/transformer.py:329,333-334, activation.py attention dropout, embedding.py:97):
 // a stateless Bernoulli mask keyed by (seed of the forward call, stream id of the site, element index), so the backward
 // pass regenerates the mask of the forward pass instead of storing it.  splitmix64 finaliser; keep <=> hash >= thresh
@@ -43,24 +42,64 @@ inline DropCfg make_drop(float p, uint64_t seed, uint32_t stream, int64_t lmax =
   return c;
 }
 
+// Visibility rule of one query row: key c is seen iff c < lim0 or s1 <= c < hi1.
 struct RowMask {
   int lim0, s1, hi1;
   __device__ __forceinline__ bool ok(int c) const { return c < lim0 || (c >= s1 && c < hi1); }
 };
-__device__ __forceinline__ RowMask make_row_mask(int mode, int qr, int L, int S, int seg1_start, int seg1_len) {
-  RowMask m{0, 0, 0};
-  if (qr >= L) return m;
-  if (mode == VB_MASK_FULL) {
-    m.lim0 = L; m.s1 = L; m.hi1 = L;
-  } else if (mode == VB_MASK_VALLE_AR) {
-    m.lim0 = max(S, qr + 1); m.s1 = L; m.hi1 = L;
-  } else if (mode == VB_MASK_PADDED_AR) {
-    m.lim0 = S; m.s1 = seg1_start;
-    m.hi1 = qr >= seg1_start ? seg1_start + min(seg1_len, qr - seg1_start + 1) : seg1_start;
-  } else {  // VB_MASK_PADDED
-    m.lim0 = S; m.s1 = seg1_start; m.hi1 = seg1_start + seg1_len;
+// A batch of packed ragged sequences and the attention mask over them (vb_mask_mode VB_MASK_FULL .. VB_MASK_PADDED).
+// Sequence b is rows [r0, r0 + L) of the packed [M, .] matrices, r0 = cu_seqlens[b], L = cu_seqlens[b + 1] - r0 <=
+// max_seqlen; its rows and keys are counted from 0.  S = text_lens[b] is read in every mode but FULL, c1 = seg1_lens[b]
+// in the padded modes (a padded sequence is [text padded to seg1_start | audio padded]).  Query row qr < L sees key c
+// iff c < lim0 or s1 <= c < hi1, with
+//   FULL       lim0 = L                        (NAR: the whole sequence)
+//   VALLE_AR   lim0 = max(S, qr + 1)           (AR inference: all text, causal audio)
+//   PADDED_AR  lim0 = S; s1 = seg1_start, hi1 = seg1_start + clamp(qr - seg1_start + 1, 0, c1)
+//                                              (AR training: text, and the audio causally)
+//   PADDED     lim0 = S; s1 = seg1_start, hi1 = seg1_start + c1
+//                                              (NAR training: key padding only)
+// and a row qr >= L sees nothing.
+struct Packed {
+  const int32_t *cu_seqlens, *text_lens, *seg1_lens;
+  int B, max_seqlen, seg1_start, mask_mode;
+  struct Seq {
+    int r0, L, S, c1;
+  };
+  // read-only loads (ld.global.nc): no kernel writes the length arrays
+  __device__ __forceinline__ Seq seq(int b) const {
+    Seq q;
+    q.r0 = __ldg(cu_seqlens + b);
+    q.L = __ldg(cu_seqlens + b + 1) - q.r0;
+    q.S = mask_mode != VB_MASK_FULL ? __ldg(text_lens + b) : 0;
+    q.c1 = mask_mode >= VB_MASK_PADDED_AR ? __ldg(seg1_lens + b) : 0;
+    return q;
   }
-  return m;
+  __device__ __forceinline__ RowMask row_mask(const Seq &q, int qr) const {
+    RowMask m{0, 0, 0};
+    if (qr >= q.L) return m;
+    if (mask_mode == VB_MASK_FULL) {
+      m.lim0 = q.L; m.s1 = q.L; m.hi1 = q.L;
+    } else if (mask_mode == VB_MASK_VALLE_AR) {
+      m.lim0 = max(q.S, qr + 1); m.s1 = q.L; m.hi1 = q.L;
+    } else if (mask_mode == VB_MASK_PADDED_AR) {
+      m.lim0 = q.S; m.s1 = seg1_start;
+      m.hi1 = qr >= seg1_start ? seg1_start + min(q.c1, qr - seg1_start + 1) : seg1_start;
+    } else {  // VB_MASK_PADDED
+      m.lim0 = q.S; m.s1 = seg1_start; m.hi1 = seg1_start + q.c1;
+    }
+    return m;
+  }
+  // keys [0, kv_max) hold every key that the query rows below q_hi (<= L) see
+  __device__ __forceinline__ int kv_max(const Seq &q, int q_hi) const {
+    return mask_mode == VB_MASK_VALLE_AR ? max(q.S, q_hi) : q.L;
+  }
+};
+// the mask mode, and the length arrays it reads (fn: the caller, for the message)
+inline int check_packed(const Packed &p, const char *fn) {
+  VB_CHECK_ARG(p.mask_mode >= VB_MASK_FULL && p.mask_mode <= VB_MASK_PADDED, "%s: bad mask mode %d", fn, p.mask_mode);
+  VB_CHECK_ARG(p.mask_mode == VB_MASK_FULL || p.text_lens != nullptr, "%s: this mask mode needs text_lens", fn);
+  VB_CHECK_ARG(p.mask_mode < VB_MASK_PADDED_AR || p.seg1_lens != nullptr, "%s: padded mask modes need seg1_lens", fn);
+  return VB_OK;
 }
 
 // bytes per element of a VB_* dtype
@@ -251,15 +290,14 @@ int launch_ln_fold(const bf16 *W, int N, int K, const float *gamma, const float 
 
 // attention.cu
 // fills the layer's KV cache `kv` when kv.k != nullptr (kv.kexp != nullptr: the FP8 cache)
-int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int B, int n_head, int head_dim,
-                            const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
-                            int seg1_start, int max_seqlen, int mask_mode, void *out, const KvCache &kv,
-                            const uint8_t *dense_mask, int64_t dense_ld, cudaStream_t s, const DropCfg *drop = nullptr);
+// pk.mask_mode may also be VB_MASK_DENSE, with the byte mask dense_mask
+int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int n_head, int head_dim, const Packed &pk,
+                            void *out, const KvCache &kv, const uint8_t *dense_mask, int64_t dense_ld, cudaStream_t s,
+                            const DropCfg *drop = nullptr);
 // attention_wgmma.cu (bf16 flash attention on wgmma / TMA; fills the KV cache when kv.k != nullptr: bf16, or with
 // kv.kexp != nullptr the FP8 cache, e4m3 rows + exponent bytes)
-int launch_attention_wgmma(const bf16 *qkv, int64_t M, int B, int n_head, const int32_t *cu_seqlens,
-                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, bf16 *out, const KvCache &kv, cudaStream_t s);
+int launch_attention_wgmma(const bf16 *qkv, int64_t M, int n_head, const Packed &pk, bf16 *out, const KvCache &kv,
+                           cudaStream_t s);
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
 // the current token's q, k, v (kv.q, or pending in qkv) against the layer's cache kv.kv.  dtype VB_E4M3: the FP8
 // cache; q, k, v must then be pending in qkv
@@ -282,9 +320,8 @@ int launch_transpose_pad(const void *in, int dtype, int64_t ld_in, int64_t R, in
                          cudaStream_t s);
 int launch_colsum(const void *in, int dtype, int64_t ld, int64_t R, int N, float *out, cudaStream_t s);
 int launch_relu_bwd(void *dh, const void *h, int dtype, int64_t n, float scale, cudaStream_t s);
-int attention_backward(const void *qkv, const void *out, const void *dout, int dtype, int64_t M, int B, int n_head,
-                       int head_dim, const int32_t *cu_seqlens, const int32_t *text_lens, const int32_t *seg1_lens,
-                       int seg1_start, int max_seqlen, int mask_mode, void *dqkv, void *workspace, size_t workspace_bytes,
+int attention_backward(const void *qkv, const void *out, const void *dout, int dtype, int64_t M, int n_head,
+                       int head_dim, const Packed &pk, void *dqkv, void *workspace, size_t workspace_bytes,
                        const DropCfg *drop, cudaStream_t s);
 // out[i] = keep(i) ? in[i] / (1 - p) : 0 (in place allowed); x[i] += keep(i) ? t[i] / (1 - p) : 0
 int launch_dropout(const void *in, void *out, int dtype, int64_t n, const DropCfg &cfg, cudaStream_t s);
