@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 9
+#define VB_ABI_VERSION 10
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
@@ -194,6 +194,19 @@ int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, const i
                            uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
                            void *workspace, size_t workspace_bytes, vb_stream_t stream);
 
+/* Prefill into chosen cache streams (ABI 10; continuous batching: new utterances refill the stopped slots of a running
+ * batch).  vb_decoder_forward over the B packed sequences, except that sequence b fills cache stream cache_slots[b]
+ * ([n_layer, <cache batch>, H, cache_cap, hd] caches; FP8: its exponent rows as well) instead of stream b.
+ * cache_slots: device int32 [B] of distinct values in [0, cache batch), or NULL = identity (then the call computes what
+ * vb_decoder_forward / vb_decoder_forward_kv8 computes).  Every other stream of the cache is left untouched; x is the
+ * same as without the map.  kcache / vcache non-NULL; k_exp / v_exp both NULL (a cache of the decoder's wdtype) or both
+ * set (the FP8 cache, under the layout rules of vb_decoder_forward_kv8). */
+int vb_decoder_forward_slots(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                             const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                             int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
+                             uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
+                             const int32_t *cache_slots, void *workspace, size_t workspace_bytes, vb_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * a2 / f2  Training: VALLE.forward with gradients (valle/models/valle.py:762-959; loss.backward() at
  *     valle/bin/trainer.py:674).  The backward functions produce what torch.autograd produces for the reference's
@@ -359,6 +372,20 @@ size_t vb_ar_step_workspace(const vb_decoder_desc *desc, int B, int cache_cap);
  * (valle.py:1013-1015).  Used after prefill and at the end of every decode step. */
 int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
                     void *workspace, size_t workspace_bytes, vb_stream_t stream);
+
+/* bytes of scratch vb_ar_admit needs for k rows (n_vocab: the head's) */
+size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab);
+
+/* Admit k new utterances into rows slots[0..k) (device int32 [k], distinct, in [0, st->B)) of a running state (ABI 10;
+ * after their prefill through vb_decoder_forward_slots).  h: fp32 [k, d], the last prefill row of each.  On entry the
+ * slots' text_len, prompt_len, max_new (and, for head->greedy == 2, sample_seed / top_k / temperature) hold the new
+ * utterances' values.  The call runs vb_ar_head_step on a k-row state built from those rows, with n_gen = 0 and
+ * finished = 0, so admitted row i gets exactly what vb_ar_head_step on a fresh k-row state gives its row i.
+ * Writes, for the slots only: n_gen, finished, tokens[slot, 0], x_cur[slot, :] and logits[slot, 0:n_vocab].  Every other
+ * row of every array, the slots' other entries and the KV cache are left unchanged.  No host reads: safe to capture in
+ * a CUDA graph. */
+int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h, int k, const int32_t *slots,
+                vb_ar_state *st, void *workspace, size_t workspace_bytes, vb_stream_t stream);
 
 /* one decode step for all B rows: 12 x (LN -> QKV -> KV append -> single-query attention over
  * the cache -> out-proj -> LN -> FFN), then vb_ar_head_step.  Post-LN stacks run

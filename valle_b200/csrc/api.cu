@@ -379,22 +379,47 @@ static bool kv8_layout_ok(const void *k_exp, const void *v_exp, int64_t layer_st
          (reinterpret_cast<uintptr_t>(k_exp) & 15) == 0 && (reinterpret_cast<uintptr_t>(v_exp) & 15) == 0;
 }
 
+// the FP8 cache's requirements (fn: the entry point's name, for the message)
+static int check_kv8(const char *fn, const vb_decoder_t dec, const uint8_t *k_exp, const uint8_t *v_exp,
+                     int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap) {
+  if (dec->desc.wdtype != VB_BF16) {
+    set_error("%s: the FP8 KV cache needs a bf16 decoder", fn);
+    return VB_ERR_UNSUPPORTED;
+  }
+  VB_CHECK_ARG(kv8_layout_ok(k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap),
+               "%s: FP8 cache: strides must be multiples of 1024, cache_cap a multiple of 16 and "
+               "k_exp / v_exp 16-byte aligned", fn);
+  return VB_OK;
+}
+
 VB_API int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
                                   const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
                                   int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
                                   uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
                                   void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && x && cu_seqlens && kcache && vcache && k_exp && v_exp, "vb_decoder_forward_kv8: null argument");
-  if (dec->desc.wdtype != VB_BF16) {
-    set_error("vb_decoder_forward_kv8: the FP8 KV cache needs a bf16 decoder");
-    return VB_ERR_UNSUPPORTED;
-  }
-  VB_CHECK_ARG(kv8_layout_ok(k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap),
-               "vb_decoder_forward_kv8: FP8 cache: strides must be multiples of 1024, cache_cap a multiple of 16 and "
-               "k_exp / v_exp 16-byte aligned");
+  VB_TRY(check_kv8("vb_decoder_forward_kv8", dec, k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap));
   const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap, (int)elem_size(VB_E4M3)};
   const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
   return decoder_forward("vb_decoder_forward_kv8", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
+                         workspace_bytes, stream);
+}
+
+VB_API int vb_decoder_forward_slots(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                                    const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                                    int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
+                                    uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
+                                    const int32_t *cache_slots, void *workspace, size_t workspace_bytes,
+                                    vb_stream_t stream) {
+  VB_CHECK_ARG(dec && x && cu_seqlens && kcache && vcache, "vb_decoder_forward_slots: null argument");
+  VB_CHECK_ARG(!k_exp == !v_exp, "vb_decoder_forward_slots: k_exp / v_exp: both or neither");
+  const bool f8 = k_exp != nullptr;
+  if (f8)
+    VB_TRY(check_kv8("vb_decoder_forward_slots", dec, k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap));
+  const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap,
+                      (int)elem_size(f8 ? VB_E4M3 : dec->desc.wdtype)};
+  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode, cache_slots};
+  return decoder_forward("vb_decoder_forward_slots", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
                          workspace_bytes, stream);
 }
 
@@ -617,6 +642,62 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
                      D.final_norm_w ? &ln : nullptr, 0, nullptr, s));
   if (head->greedy) VB_TRY(launch_ar_sample(st->logits, ldl, SplitK{}, head, st, d, nullptr, 0, false, s));
   return VB_OK;
+}
+
+namespace {
+// vb_ar_admit's workspace: a k-row state (cs, tok_stride 1) for the head step of the admitted rows, then that head
+// step's own workspace
+struct AdmitWs {
+  vb_ar_state cs;
+  void *head_ws;
+  size_t head_ws_bytes;
+};
+constexpr int kAdmitCap = 64;  // the k-row state holds no cache: the smallest capacity sizes the head's workspace
+AdmitWs carve_admit_ws(Carve &c, const vb_decoder_desc &D, int k, int n_vocab) {
+  AdmitWs w{};
+  vb_ar_state &cs = w.cs;
+  cs.B = k;
+  cs.tok_stride = 1;
+  cs.text_len = c.take<int32_t>(k * 4);
+  cs.prompt_len = c.take<int32_t>(k * 4);
+  cs.max_new = c.take<int32_t>(k * 4);
+  cs.n_gen = c.take<int32_t>(k * 4);
+  cs.finished = c.take<int32_t>(k * 4);
+  cs.tokens = c.take<int32_t>(k * 4);
+  cs.x_cur = c.take<float>((size_t)k * D.d_model * 4);
+  cs.logits = c.take<float>((size_t)k * ((n_vocab + 3) & ~3) * 4);
+  cs.cache_cap = kAdmitCap;
+  cs.sample_seed = c.take<uint64_t>(k * 8);
+  cs.top_k = c.take<int32_t>(k * 4);
+  cs.temperature = c.take<float>(k * 4);
+  w.head_ws_bytes = vb_ar_step_workspace(&D, k, kAdmitCap);
+  w.head_ws = c.take(w.head_ws_bytes);
+  return w;
+}
+}  // namespace
+
+VB_API size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab) {
+  return carved_bytes(carve_admit_ws, *desc, k, n_vocab);
+}
+
+VB_API int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h, int k, const int32_t *slots,
+                       vb_ar_state *st, void *workspace, size_t workspace_bytes, vb_stream_t stream) {
+  VB_CHECK_ARG(dec && head && h && slots && st, "vb_ar_admit: null argument");
+  VB_CHECK_ARG(k >= 1 && k <= st->B, "vb_ar_admit: k=%d not in [1, B=%d]", k, st->B);
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_admit: greedy %d not in {0, 1, 2}", head->greedy);
+  VB_CHECK_ARG(head->greedy != 2 || (st->sample_seed && st->top_k && st->temperature),
+               "vb_ar_admit: vb_ar_head.greedy == 2: sampler arrays not set");
+  const vb_decoder_desc &D = dec->desc;
+  VB_CHECK_ARG(workspace && workspace_bytes >= vb_ar_admit_workspace(&D, k, head->n_vocab),
+               "vb_ar_admit: workspace too small (%zu < %zu)", workspace_bytes,
+               vb_ar_admit_workspace(&D, k, head->n_vocab));
+  cudaStream_t s = (cudaStream_t)stream;
+  Carve c(workspace);
+  AdmitWs w = carve_admit_ws(c, D, k, head->n_vocab);
+  const int ldl = (head->n_vocab + 3) & ~3;
+  VB_TRY(launch_ar_admit_copy(st, &w.cs, slots, D.d_model, ldl, head->n_vocab, false, s));
+  VB_TRY(vb_ar_head_step(dec, head, h, &w.cs, w.head_ws, w.head_ws_bytes, stream));
+  return launch_ar_admit_copy(st, &w.cs, slots, D.d_model, ldl, head->n_vocab, true, s);
 }
 
 VB_API int vb_cast_from_f32(const float *in, void *out, int dtype, int64_t n, vb_stream_t stream) {

@@ -83,7 +83,8 @@ attn_varlen_simt_kernel(const T *__restrict__ qkv, int n_head, const Packed pk, 
         Vs[lrow * LDT + le0 + i] = ok ? to_f32(vraw[i]) : 0.f;
       }
       if (kv.k != nullptr && j0 == q0 && ok) {  // this CTA owns rows [q0, q0+64) of the cache
-        T *kc = (T *)kv.k + kv.row(b, h, kr) + le0, *vc = (T *)kv.v + kv.row(b, h, kr) + le0;
+        const int64_t off = kv.row(pk.cache_seq(b), h, kr) + le0;
+        T *kc = (T *)kv.k + off, *vc = (T *)kv.v + off;
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
           kc[i] = kraw[i];

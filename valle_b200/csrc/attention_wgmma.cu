@@ -187,6 +187,7 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
   auto fill_cache = [&](int j0, const uint8_t *sk) {
     if (kv.k == nullptr || j0 != q0 + half * 64) return;
     const uint8_t *sv = sk + kBoxBytes;
+    const int cb = pk.cache_seq(b);
     if constexpr (kF8) {
       // 8 consecutive lanes hold one row (16 bytes = 8 bf16 each): the row's max |.| is one 8-lane shuffle reduction
 #pragma unroll
@@ -219,7 +220,7 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
             kq[j >> 2] |= (uint32_t)kv8_quant(kf[j], ek) << (8 * (j & 3));
             vq[j >> 2] |= (uint32_t)kv8_quant(vf[j], ev) << (8 * (j & 3));
           }
-          const int64_t e = kv.exp_index(b, h, j0 + r), off = e * HD + c * 8;   // row(b, h, p) = 64 exp_index(b, h, p)
+          const int64_t e = kv.exp_index(cb, h, j0 + r), off = e * HD + c * 8;   // row(b, h, p) = 64 exp_index(b, h, p)
           *reinterpret_cast<uint2 *>((uint8_t *)kv.k + off) = make_uint2(kq[0], kq[1]);
           *reinterpret_cast<uint2 *>((uint8_t *)kv.v + off) = make_uint2(vq[0], vq[1]);
           if (c == 0) {
@@ -234,7 +235,7 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
         const int idx = t + i * 128;
         const int r = idx >> 3, c = idx & 7;
         if (j0 + r < L) {
-          const int64_t off = kv.row(b, h, j0 + r) + c * 8;
+          const int64_t off = kv.row(cb, h, j0 + r) + c * 8;
           const int so = r * 128 + ((c ^ (r & 7)) << 4);
           *reinterpret_cast<uint4 *>((bf16 *)kv.k + off) = *reinterpret_cast<const uint4 *>(sk + so);
           *reinterpret_cast<uint4 *>((bf16 *)kv.v + off) = *reinterpret_cast<const uint4 *>(sv + so);

@@ -58,10 +58,13 @@ struct RowMask {
 //                                              (AR training: text, and the audio causally)
 //   PADDED     lim0 = S; s1 = seg1_start, hi1 = seg1_start + c1
 //                                              (NAR training: key padding only)
-// and a row qr >= L sees nothing.
+// and a row qr >= L sees nothing.  A prefill that fills a KV cache writes sequence b's rows into the cache's stream
+// cache_seq(b): cache_slot[b] when a slot map is given (continuous batching refills one slot of a running batch),
+// else b.
 struct Packed {
   const int32_t *cu_seqlens, *text_lens, *seg1_lens;
   int B, max_seqlen, seg1_start, mask_mode;
+  const int32_t *cache_slot = nullptr;
   struct Seq {
     int r0, L, S, c1;
   };
@@ -93,6 +96,7 @@ struct Packed {
   __device__ __forceinline__ int kv_max(const Seq &q, int q_hi) const {
     return mask_mode == VB_MASK_VALLE_AR ? max(q.S, q_hi) : q.L;
   }
+  __device__ __forceinline__ int cache_seq(int b) const { return cache_slot ? __ldg(cache_slot + b) : b; }
 };
 // the mask mode, and the length arrays it reads (fn: the caller, for the message)
 inline int check_packed(const Packed &p, const char *fn) {
@@ -334,5 +338,10 @@ int launch_cast_from_f32(const float *in, void *out, int dtype, int64_t n, cudaS
 // in: the head projection's pending partials (in.part == NULL: the logits are complete)
 int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const vb_ar_head *head, vb_ar_state *st,
                      int d, const int64_t *forced, int reduce_only, bool pdl, cudaStream_t s);
+// vb_ar_admit: row i of the k-row state cs <-> row slots[i] of the running state st.  Gather (scatter = false): the
+// lengths and sampler parameters into cs, n_gen / finished / tokens of cs zeroed.  Scatter: n_gen, finished,
+// tokens[., 0], x_cur and logits[., 0:n_vocab] back into the slots
+int launch_ar_admit_copy(vb_ar_state *st, const vb_ar_state *cs, const int32_t *slots, int d, int ldl, int n_vocab,
+                         bool scatter, cudaStream_t s);
 
 }  // namespace vb

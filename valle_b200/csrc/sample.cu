@@ -286,6 +286,44 @@ int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const v
   return VB_OK;
 }
 
+// one CTA per admitted row i, slot = slots[i] (launch_ar_admit_copy)
+__global__ void __launch_bounds__(256)
+ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__ slots, int d, int ldl, int n_vocab,
+                     int scatter) {
+  const int i = blockIdx.x, tid = threadIdx.x;
+  const int s = slots[i];
+  if (!scatter) {
+    if (tid == 0) {
+      const_cast<int32_t *>(cs.text_len)[i] = st.text_len[s];
+      const_cast<int32_t *>(cs.prompt_len)[i] = st.prompt_len[s];
+      const_cast<int32_t *>(cs.max_new)[i] = st.max_new[s];
+      cs.n_gen[i] = 0;
+      cs.finished[i] = 0;
+      cs.tokens[i] = 0;
+      if (st.sample_seed) {
+        const_cast<uint64_t *>(cs.sample_seed)[i] = st.sample_seed[s];
+        const_cast<int32_t *>(cs.top_k)[i] = st.top_k[s];
+        const_cast<float *>(cs.temperature)[i] = st.temperature[s];
+      }
+    }
+    return;
+  }
+  if (tid == 0) {
+    st.n_gen[s] = cs.n_gen[i];
+    st.finished[s] = cs.finished[i];
+    st.tokens[(int64_t)s * st.tok_stride] = cs.tokens[i];
+  }
+  for (int c = tid; c < d; c += 256) st.x_cur[(int64_t)s * d + c] = cs.x_cur[(int64_t)i * d + c];
+  for (int c = tid; c < n_vocab; c += 256) st.logits[(int64_t)s * ldl + c] = cs.logits[(int64_t)i * ldl + c];
+}
+
+int launch_ar_admit_copy(vb_ar_state *st, const vb_ar_state *cs, const int32_t *slots, int d, int ldl, int n_vocab,
+                         bool scatter, cudaStream_t s) {
+  ar_admit_copy_kernel<<<cs->B, 256, 0, s>>>(*st, *cs, slots, d, ldl, n_vocab, scatter ? 1 : 0);
+  VB_LAUNCH_CHECK();
+  return VB_OK;
+}
+
 __global__ void __launch_bounds__(256)
 sample_logits_kernel(const float *__restrict__ logits, int64_t ld, int n_vocab, const uint64_t *__restrict__ seeds,
                      const int32_t *__restrict__ steps, const int32_t *__restrict__ top_k,

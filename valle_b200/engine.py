@@ -23,7 +23,7 @@ import os
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Dict, Iterable, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -59,11 +59,27 @@ def _check_ids(tensors, hi: int, what: str):
 
 @dataclass
 class EngineStats:
-    """CUDA-event timings (ms) of the phases of the last generate() call and the number of decode steps"""
+    """CUDA-event timings (ms) of the phases of the last generate() / generate_stream() call and the number of decode
+    steps; generate_stream() also counts the utterances it admitted into decode slots and the decode steps they ran
+    (slot occupancy = slot_steps / (ar_steps * slots))"""
     ar_steps: int = 0
     ar_ms: float = 0.0
     prefill_ms: float = 0.0
     nar_ms: float = 0.0
+    admissions: int = 0
+    slot_steps: int = 0
+
+
+class StreamRequest(NamedTuple):
+    """One utterance of ValleEngine.generate_stream: text int64 [S] phoneme ids, prompt int64 [Tp, Q] codec ids, and
+    what generate() takes per utterance.  top_k != 1 needs a seed (the seeded device sampler)."""
+    text: torch.Tensor
+    prompt: torch.Tensor
+    enroll_len: Optional[int] = None
+    seed: Optional[int] = None
+    top_k: int = 1
+    temperature: float = 1.0
+    max_new_tokens: Optional[int] = None
 
 
 class _ArBuffers:
@@ -112,6 +128,10 @@ class _ArBuffers:
         #: (head tables, draw mode, steps) -> (graph of that many decode steps, kernels per replay, head struct)
         self.graphs: Dict[tuple, Tuple[torch.cuda.CUDAGraph, int, L.ArHead]] = {}
         self.eng = eng
+
+
+class _Prefill:
+    """the device-side inputs of one packed AR prefill (ValleEngine._prefill_inputs)"""
 
 
 def _is_seq(v) -> bool:
@@ -327,7 +347,7 @@ class ValleEngine:
     @_on_device
     def generate(self, texts: Sequence[torch.Tensor], prompts: Sequence[torch.Tensor],
                  enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1, temperature: float = 1.0,
-                 max_new_tokens: Optional[int] = None, poll: int = 32,
+                 max_new_tokens=None, poll: int = 32,
                  return_device: bool = False, trace: Optional[dict] = None,
                  forced: Optional[Sequence[torch.Tensor]] = None, seed=None) -> List[torch.Tensor]:
         """texts[b]: int64 [S_b] phoneme ids; prompts[b]: int64 [Tp_b, Q] codec ids (host or device).
@@ -338,6 +358,7 @@ class ValleEngine:
         (vb_sample_logits): utterance b draws from seed s + b (or seed[b]) and its decode step, inside the CUDA-graph
         decode step, so its codes do not depend on the batch it shares, its slot, or how the call is split.  With a
         seed, top_k and temperature may be per-utterance sequences; every top_k == 1 is the greedy path.
+        max_new_tokens: None, one int, or a sequence of B ints (one cap per utterance).
 
         Test hooks: `trace` collects AR logits (trace["steps"] = set of iterations or "all") and, with
         trace["nar"] = True, the NAR logits / argmax of every stage; `forced[b]` = int64 [T_b, Q] codes the decode is
@@ -369,8 +390,9 @@ class ValleEngine:
                     kw = dict(top_k=top_k, temperature=temperature)
                 else:   # by absolute utterance index
                     kw = dict(seed=sampler[0][b0:b1], top_k=sampler[1][b0:b1], temperature=sampler[2][b0:b1])
+                mnt = max_new_tokens[b0:b1] if _is_seq(max_new_tokens) else max_new_tokens
                 outs += self.generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
-                                      max_new_tokens=max_new_tokens, poll=poll, return_device=return_device, **kw)
+                                      max_new_tokens=mnt, poll=poll, return_device=return_device, **kw)
                 stats.ar_steps += self.stats.ar_steps
                 stats.ar_ms += self.stats.ar_ms
                 stats.prefill_ms += self.stats.prefill_ms
@@ -385,12 +407,7 @@ class ValleEngine:
         _check_ids(texts, NUM_TEXT_TOKENS, "phoneme")
         _check_ids([p[:, :1] for p in prompts], NUM_AUDIO_TOKENS + 1, "prompt code (first codebook)")  # 1025-row tables
         _check_ids([p[:, 1:] for p in prompts], NUM_AUDIO_TOKENS, "prompt code")
-        cap_new = [16 * s for s in S]  # valle.py:1047: stop when n_new > 16 * S
-        if self.prepend_bos:
-            # y carries the <BOS> the prompt does not: (y.shape[1] - prompts.shape[1]) = n_new + 1 (valle.py:1045-1047)
-            cap_new = [c - 1 for c in cap_new]
-        if max_new_tokens is not None:
-            cap_new = [min(c, max_new_tokens - 1) for c in cap_new]
+        cap_new = self._cap_new(S, max_new_tokens)
         tok_stride = (max(cap_new) + 2 + 7) // 8 * 8
         cap = (max(S[b] + Tp[b] + cap_new[b] + 2 for b in range(B)) + 63) // 64 * 64
         greedy = sampler is None and top_k == 1 and forced is None
@@ -406,41 +423,16 @@ class ValleEngine:
             cap_new = [min(c, int(f.shape[0])) for c, f in zip(cap_new, forced)]
 
         # ---- host -> device (once per batch) ----
-        text_all = torch.cat([t.reshape(-1).to(torch.int64) for t in texts]).to(dev, non_blocking=True)
-        prm_all = torch.cat([p.to(torch.int64) for p in prompts]).contiguous().to(dev, non_blocking=True)
-        Tp_nar = Tp
-        if self.prepend_bos:   # the AR stack sees [<BOS> | first-codebook prompt]; the NAR stages see the prompt only
-            bos = torch.full((1,), NUM_AUDIO_TOKENS + 1, dtype=torch.int64)
-            ar_tok = torch.cat([torch.cat([bos, p[:, 0].to(torch.int64).cpu()]) for p in prompts]).to(dev, non_blocking=True)
-            Tp = [t + 1 for t in Tp]
-        seq_len = [S[b] + Tp[b] for b in range(B)]
-        cu = [0]
-        for n in seq_len:
-            cu.append(cu[-1] + n)
-        M = cu[-1]
-        cu_np = np.asarray(cu, dtype=np.int64)
-        text_rows, text_pos = _seg_ranges(cu_np[:-1], S)
-        aud_rows, aud_pos = _seg_ranges(cu_np[:-1] + np.asarray(S, dtype=np.int64), Tp)
-        meta = torch.from_numpy(np.concatenate([cu_np, S, Tp, cap_new, text_rows, text_pos, aud_rows, aud_pos,
-                                                cu_np[1:] - 1]).astype(np.int32)).to(dev, non_blocking=True)
-        o = 0
-        def take(n):
-            nonlocal o
-            v = meta[o:o + n]
-            o += n
-            return v
-        cu_d, S_d, Tp_d, capn_d = take(B + 1), take(B), take(B), take(B)
-        trow_d, tpos_d = take(sum(S)), take(sum(S))
-        arow_d, apos_d = take(sum(Tp)), take(sum(Tp))
-        last_d = take(B)
+        p = self._prefill_inputs(texts, prompts, cap_new)
+        Tp_nar, Tp, text_all, prm_all = p.Tp_nar, p.Tp, p.text_all, p.prm_all
 
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         ev[0].record()
         # ---- AR prefill (valle.py:995-997,1013-1016) ----
         buf = self._buffers(B, cap, tok_stride, kv_dtype)
-        buf.text_len.copy_(S_d)
-        buf.prompt_len.copy_(Tp_d)
-        buf.max_new.copy_(capn_d)
+        buf.text_len.copy_(p.S_d)
+        buf.prompt_len.copy_(p.Tp_d)
+        buf.max_new.copy_(p.capn_d)
         buf.n_gen.zero_()
         buf.finished.zero_()
         if native:
@@ -448,18 +440,8 @@ class ValleEngine:
             buf.sample_seed.copy_(torch.tensor([x - (1 << 64) if x >= 1 << 63 else x for x in seeds], dtype=torch.int64))
             buf.top_k.copy_(torch.tensor(ks, dtype=torch.int32))
             buf.temperature.copy_(torch.tensor(ts, dtype=torch.float32))
-        pe_t = self._pe(m.ar_text_position, max(S))
         pe_a = self._pe(m.ar_audio_position, max(Tp) + max(cap_new) + 2)
-        x = torch.empty((M, d), dtype=torch.float32, device=dev)
-        self._embed_pe(text_all, 1, m.ar_text_embedding.weight, pe_t, m.ar_text_position.alpha, sum(S), x, trow_d, tpos_d,
-                       prenet=("ar_text", S) if self.pre else None)
-        if self.prepend_bos:
-            self._embed_pe(ar_tok, 1, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, arow_d, apos_d)
-        else:
-            self._embed_pe(prm_all, Q, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, arow_d, apos_d)
-        self.ar.forward(x, cu_d, B, max(seq_len), L.VB_MASK_VALLE_AR, S_d, None, buf.kcache, buf.vcache, cap,
-                        k_exp=buf.k_exp, v_exp=buf.v_exp)
-        h_last = ops.gather_rows(x, last_d)
+        h_last = self._prefill(buf, p, pe_a)
         head = self._head(pe_a, 2 if native else int(greedy))
         self._head_ref = head
         L.check(self.lib.vb_ar_head_step(self.ar.handle, C.byref(head), h_last.data_ptr(), C.byref(buf.st),
@@ -486,13 +468,7 @@ class ValleEngine:
         while steps < max_steps:
             n = min(poll, max_steps - steps)
             if (greedy or native) and self.use_cuda_graph:
-                # whole groups of `steps_per_graph` decode steps as one graph replay (no launch gap between the
-                # steps of a group), the remainder one step at a time
-                done = 0
-                while done < n:
-                    k = self.steps_per_graph if n - done >= self.steps_per_graph else 1
-                    self._replay_steps(buf, head, k)
-                    done += k
+                self._device_steps(buf, head, n)
             else:
                 for _ in range(n):
                     fs = None
@@ -543,6 +519,301 @@ class ValleEngine:
             return [codes[cu_g[b]:cu_g[b + 1]] for b in range(B)]
         host = codes.cpu()
         return [host[cu_g[b]:cu_g[b + 1]] for b in range(B)]
+
+    def generate_stream(self, requests: Iterable, slots: Optional[int] = None, max_context: Optional[int] = None,
+                        poll: int = 32, nar_batch: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor]]:
+        """Continuous batching: decode `requests` (StreamRequest records, or tuples in its field order) in `slots`
+        decode rows, refilling a row with the next request as soon as its utterance stops, and yield (index, codes) in
+        completion order.  codes: int64 [Tgen, Q] on the device, what generate() returns for that utterance; index:
+        the request's position in `requests`.
+
+        requests may be a lazy iterator (pulled from while decoding runs); the KV cache holds `max_context` rows per
+        slot (text + prompt + new tokens + 2; default: the largest request of a sequence, required for an iterator),
+        and a request that needs more raises ValueError when it is pulled.  slots: default min(#requests, 64); bf16
+        takes at most 64 (one tensor-core decode group).  New requests are admitted, and the stop flags read, every
+        `poll` decode steps; the NAR runs over every `nar_batch` (default `slots`) finished utterances, and over the
+        rest once nothing is left to decode.  Sampling is greedy, or seeded per request (`seed`, with top_k /
+        temperature): the draws depend on the seed and the step only, never on the slot or the schedule."""
+        with torch.cuda.device(self.device):
+            self._refresh()
+        kv_dtype = self.kv_cache_dtype()
+        if self.sample_on_host:
+            raise ValueError("generate_stream draws on the device: sample_on_host = True is not supported")
+        if isinstance(requests, (list, tuple)):
+            reqs = [StreamRequest(*r) for r in requests]
+            if not reqs:
+                return iter(())
+            if max_context is None:
+                max_context = max(self._context(r) for r in reqs)
+            slots = min(len(reqs), self.max_tc_batch) if slots is None else slots
+            it = iter(reqs)
+        else:
+            if max_context is None:
+                raise ValueError("generate_stream: an iterator of requests needs max_context")
+            slots = self.max_tc_batch if slots is None else slots
+            it = (StreamRequest(*r) for r in requests)
+        slots, poll = int(slots), int(poll)
+        nar_batch = slots if nar_batch is None else int(nar_batch)
+        if slots < 1 or poll < 1 or nar_batch < 1:
+            raise ValueError("generate_stream: slots, poll and nar_batch must be >= 1")
+        if self.dtype == torch.bfloat16 and slots > self.max_tc_batch:
+            raise ValueError(f"generate_stream: bf16 decodes at most {self.max_tc_batch} slots (got {slots})")
+        return self._stream(it, slots, int(max_context), poll, nar_batch, kv_dtype)
+
+    def _context(self, r: StreamRequest) -> int:
+        """KV-cache rows a request needs: text + prompt + the most tokens it may generate + 2"""
+        S = int(r.text.numel())
+        return S + int(r.prompt.shape[0]) + self._cap_new([S], r.max_new_tokens)[0] + 2
+
+    @torch.no_grad()
+    def _stream(self, it, n_slots: int, max_context: int, poll: int, nar_batch: int, kv_dtype):
+        m, dev, Q = self.model, self.device, self.Q
+        cap = (max_context + 63) // 64 * 64
+        tok_stride = (max_context + 2 + 7) // 8 * 8
+        pm = self.prefix_mode
+        stats = EngineStats()
+        phases: Dict[str, list] = {"prefill_ms": [], "ar_ms": [], "nar_ms": []}
+
+        def timed(name):
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            phases[name].append([e])
+            return phases[name][-1]
+
+        with torch.cuda.device(dev):
+            buf = self._buffers(n_slots, cap, tok_stride, kv_dtype)
+            buf.n_gen.zero_()
+            buf.finished.fill_(1)              # a slot that is never filled never runs
+            buf.x_cur.zero_()
+            buf.sample_seed.zero_()
+            buf.top_k.fill_(1)
+            buf.temperature.fill_(1.0)
+            pe_a = self._pe(m.ar_audio_position, cap + 2)
+            heads = {g: self._head(pe_a, g) for g in (1, 2)}
+            ws = torch.empty(self.lib.vb_ar_admit_workspace(C.byref(self.ar.desc), n_slots, self.n_vocab),
+                             dtype=torch.uint8, device=dev)
+        mode = 1                               # 2 (the seeded sampler) from the first seeded request on
+        free = list(range(n_slots))
+        active: Dict[int, tuple] = {}          # slot -> (index, S, Tp prompt, Tp AR, text ids, prompt ids, enroll_len)
+        pending: list = []                     # finished utterances waiting for the NAR
+        n_pulled, exhausted, device_ids = 0, False, False
+
+        def pull(k):
+            nonlocal n_pulled, exhausted, mode
+            out = []
+            while len(out) < k and not exhausted:
+                try:
+                    r = next(it)
+                except StopIteration:
+                    exhausted = True
+                    break
+                idx = n_pulled
+                n_pulled += 1
+                if r.text.ndim != 1 or r.text.numel() == 0 or r.prompt.ndim != 2 or r.prompt.shape[1] != Q:
+                    raise ValueError(f"request {idx}: text must be [S > 0] ids and prompt [Tp, {Q}] codes")
+                seed, top_k = r.seed, r.top_k
+                if seed is None:
+                    if top_k != 1:
+                        raise ValueError(f"request {idx}: top_k={top_k} needs a seed (the seeded device sampler)")
+                    seed = 0
+                seeds, ks, ts = _sampler_args(1, seed, top_k, r.temperature)
+                if pm in (2, 4) and r.enroll_len is None:
+                    raise ValueError(f"request {idx}: prefix_mode {pm} needs enroll_len")
+                if self._context(r) > max_context:
+                    raise ValueError(f"request {idx} needs {self._context(r)} KV-cache rows > max_context={max_context}")
+                _check_ids([r.text], NUM_TEXT_TOKENS, "phoneme")
+                _check_ids([r.prompt[:, :1]], NUM_AUDIO_TOKENS + 1, "prompt code (first codebook)")
+                _check_ids([r.prompt[:, 1:]], NUM_AUDIO_TOKENS, "prompt code")
+                if ks[0] != 1:
+                    mode = 2
+                out.append((idx, r, seeds[0], ks[0], ts[0]))
+            return out
+
+        def admit(new):
+            nonlocal device_ids
+            k = len(new)
+            sl = free[:k]
+            del free[:k]
+            texts = [r.text for _, r, *_ in new]
+            prompts = [r.prompt for _, r, *_ in new]
+            S = [int(t.numel()) for t in texts]
+            cap_new = [self._cap_new([S[i]], new[i][1].max_new_tokens)[0] for i in range(k)]
+            p = self._prefill_inputs(texts, prompts, cap_new, slots=sl)
+            ev = timed("prefill_ms")
+            idx_d = p.slots_d.long()
+            buf.text_len.index_copy_(0, idx_d, p.S_d)
+            buf.prompt_len.index_copy_(0, idx_d, p.Tp_d)
+            buf.max_new.index_copy_(0, idx_d, p.capn_d)
+            seeds = [x - (1 << 64) if x >= 1 << 63 else x for x in (n[2] for n in new)]
+            buf.sample_seed.index_copy_(0, idx_d, torch.tensor(seeds, dtype=torch.int64).to(dev, non_blocking=True))
+            buf.top_k.index_copy_(0, idx_d, torch.tensor([n[3] for n in new], dtype=torch.int32).to(dev, non_blocking=True))
+            buf.temperature.index_copy_(0, idx_d, torch.tensor([n[4] for n in new], dtype=torch.float32).to(
+                dev, non_blocking=True))
+            h = self._prefill(buf, p, pe_a)
+            L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), k, p.slots_d.data_ptr(),
+                                         C.byref(buf.st), ws.data_ptr(), ws.numel(), L.stream_ptr()), "vb_ar_admit")
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            ev.append(e)
+            to, po = 0, 0
+            for i, (idx, r, *_) in enumerate(new):
+                active[sl[i]] = (idx, S[i], p.Tp_nar[i], p.Tp[i], p.text_all[to:to + S[i]],
+                                 p.prm_all[po:po + p.Tp_nar[i]], r.enroll_len)
+                to += S[i]
+                po += p.Tp_nar[i]
+            device_ids |= any(t.is_cuda for t in texts + prompts)
+            stats.admissions += k
+
+        def nar(batch):
+            ev = timed("nar_ms")
+            Tg = [int(c.shape[0]) for *_, c in batch]
+            cu_g = [0]
+            for n in Tg:
+                cu_g.append(cu_g[-1] + n)
+            codes = torch.empty((cu_g[-1], Q), dtype=torch.int64, device=dev)
+            codes[:, 0] = torch.cat([c for *_, c in batch])
+            if Q > 1:
+                self._nar(None, torch.cat([b[4] for b in batch]), torch.cat([b[5] for b in batch]),
+                          [b[1] for b in batch], [b[2] for b in batch], Tg, cu_g, codes, [b[6] for b in batch])
+            e = torch.cuda.Event(enable_timing=True)
+            e.record()
+            ev.append(e)
+            return [(b[0], codes[cu_g[i]:cu_g[i + 1]]) for i, b in enumerate(batch)]
+
+        def advance():
+            """admission, `poll` decode steps and the stop flags; returns the utterances whose codes are ready"""
+            if free and not exhausted:
+                new = pull(len(free))
+                if new:
+                    admit(new)
+            if active:
+                ev = timed("ar_ms")
+                head = heads[mode]
+                if self.use_cuda_graph:
+                    self._device_steps(buf, head, poll)
+                else:
+                    for _ in range(poll):
+                        self._launch_step(buf, head)
+                e = torch.cuda.Event(enable_timing=True)
+                e.record()
+                ev.append(e)
+                stats.ar_steps += poll
+                fin, n_gen = torch.stack([buf.finished, buf.n_gen]).cpu().tolist()   # one D2H sync per `poll` steps
+                for s in sorted(active):
+                    if fin[s] == 0:
+                        continue
+                    if fin[s] == 2:
+                        raise SyntaxError("well trained model shouldn't reach here.")  # valle.py:1049-1052
+                    idx, S, Tp_nar, Tp, text_d, prm_d, enroll = active.pop(s)
+                    if not self.quiet:
+                        print(f"VALL-E EOS [{Tp_nar} -> {Tp + n_gen[s]}]")  # valle.py:1054
+                    pending.append((idx, S, Tp_nar, Tp, text_d, prm_d, enroll,
+                                    buf.tokens[s, :n_gen[s]].to(torch.int64)))
+                    stats.slot_steps += n_gen[s]
+                    free.append(s)
+                free.sort()
+            ready = []
+            drain = exhausted and not active
+            while len(pending) >= nar_batch or (drain and pending):
+                batch = pending[:nar_batch]
+                del pending[:nar_batch]
+                ready += nar(batch)
+            if device_ids:
+                ops.check_oob(dev)
+            return ready
+
+        while True:
+            with torch.cuda.device(dev):
+                ready = advance()
+            yield from ready
+            if exhausted and not active and not pending:
+                break
+        torch.cuda.synchronize(dev)
+        for name, evs in phases.items():
+            setattr(stats, name, sum(a.elapsed_time(b) for a, b in evs))
+        self.stats = stats
+
+    # ---- shared by generate() and generate_stream() ----------------------------------------
+    def _cap_new(self, S: Sequence[int], max_new_tokens) -> List[int]:
+        """per utterance: the n_gen past which the stop rule fires (valle.py:1047: n_new > 16 * S), lowered to
+        max_new_tokens - 1 (one int, or one per utterance)"""
+        cap_new = [16 * s for s in S]
+        if self.prepend_bos:
+            # y carries the <BOS> the prompt does not: (y.shape[1] - prompts.shape[1]) = n_new + 1 (valle.py:1045-1047)
+            cap_new = [c - 1 for c in cap_new]
+        if max_new_tokens is not None:
+            mnt = [int(x) for x in max_new_tokens] if _is_seq(max_new_tokens) else [int(max_new_tokens)] * len(S)
+            if len(mnt) != len(S):
+                raise ValueError(f"max_new_tokens: {len(mnt)} values for {len(S)} utterances")
+            cap_new = [min(c, t - 1) for c, t in zip(cap_new, mnt)]
+        return cap_new
+
+    def _prefill_inputs(self, texts, prompts, cap_new, slots: Optional[Sequence[int]] = None):
+        """the host -> device copies of one packed AR prefill (ids, and one int32 block of lengths and row maps);
+        slots: the decode slots the utterances go to (generate_stream)"""
+        dev, Q = self.device, self.Q
+        B = len(texts)
+        S = [int(t.numel()) for t in texts]
+        Tp = [int(p.shape[0]) for p in prompts]
+        text_all = torch.cat([t.reshape(-1).to(torch.int64) for t in texts]).to(dev, non_blocking=True)
+        prm_all = torch.cat([p.to(torch.int64) for p in prompts]).contiguous().to(dev, non_blocking=True)
+        Tp_nar, ar_tok = Tp, None
+        if self.prepend_bos:   # the AR stack sees [<BOS> | first-codebook prompt]; the NAR stages see the prompt only
+            bos = torch.full((1,), NUM_AUDIO_TOKENS + 1, dtype=torch.int64)
+            ar_tok = torch.cat([torch.cat([bos, p[:, 0].to(torch.int64).cpu()]) for p in prompts]).to(dev, non_blocking=True)
+            Tp = [t + 1 for t in Tp]
+        seq_len = [S[b] + Tp[b] for b in range(B)]
+        cu = [0]
+        for n in seq_len:
+            cu.append(cu[-1] + n)
+        cu_np = np.asarray(cu, dtype=np.int64)
+        text_rows, text_pos = _seg_ranges(cu_np[:-1], S)
+        aud_rows, aud_pos = _seg_ranges(cu_np[:-1] + np.asarray(S, dtype=np.int64), Tp)
+        meta = torch.from_numpy(np.concatenate([cu_np, S, Tp, cap_new, text_rows, text_pos, aud_rows, aud_pos,
+                                                cu_np[1:] - 1, [] if slots is None else slots]).astype(np.int32)
+                                ).to(dev, non_blocking=True)
+        o = 0
+        def take(n):
+            nonlocal o
+            v = meta[o:o + n]
+            o += n
+            return v
+        p = _Prefill()
+        p.B, p.S, p.Tp, p.Tp_nar, p.M, p.max_len = B, S, Tp, Tp_nar, cu[-1], max(seq_len)
+        p.text_all, p.prm_all, p.ar_tok = text_all, prm_all, ar_tok
+        p.cu_d, p.S_d, p.Tp_d, p.capn_d = take(B + 1), take(B), take(B), take(B)
+        p.trow_d, p.tpos_d = take(sum(S)), take(sum(S))
+        p.arow_d, p.apos_d = take(sum(Tp)), take(sum(Tp))
+        p.last_d = take(B)
+        p.slots_d = take(B) if slots is not None else None
+        return p
+
+    def _prefill(self, buf: _ArBuffers, p: "_Prefill", pe_a: torch.Tensor) -> torch.Tensor:
+        """embedding (+ pre-net) + positions of every [text | prompt] row and the AR prefill (valle.py:995-997,
+        1013-1016), which fills cache stream b of buf, or p.slots_d[b]; returns the last row of each utterance [B, d]"""
+        m = self.model
+        S, Tp = p.S, p.Tp
+        pe_t = self._pe(m.ar_text_position, max(S))
+        x = torch.empty((p.M, self.d), dtype=torch.float32, device=self.device)
+        self._embed_pe(p.text_all, 1, m.ar_text_embedding.weight, pe_t, m.ar_text_position.alpha, sum(S), x, p.trow_d,
+                       p.tpos_d, prenet=("ar_text", S) if self.pre else None)
+        if self.prepend_bos:
+            self._embed_pe(p.ar_tok, 1, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, p.arow_d, p.apos_d)
+        else:
+            self._embed_pe(p.prm_all, self.Q, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, p.arow_d,
+                           p.apos_d)
+        self.ar.forward(x, p.cu_d, p.B, p.max_len, L.VB_MASK_VALLE_AR, p.S_d, None, buf.kcache, buf.vcache, buf.cap,
+                        k_exp=buf.k_exp, v_exp=buf.v_exp, cache_slots=p.slots_d)
+        return ops.gather_rows(x, p.last_d)
+
+    def _device_steps(self, buf: _ArBuffers, head: L.ArHead, n: int):
+        """n decode steps that draw on the device: whole groups of `steps_per_graph` steps as one graph replay (no launch
+        gap between the steps of a group), the remainder one step at a time"""
+        done = 0
+        while done < n:
+            k = self.steps_per_graph if n - done >= self.steps_per_graph else 1
+            self._replay_steps(buf, head, k)
+            done += k
 
     @torch.no_grad()
     @_on_device

@@ -231,17 +231,27 @@ class VALLE(nn.Module):
     @torch.no_grad()
     def inference_batch(self, texts: Sequence[torch.Tensor], prompts: Sequence[torch.Tensor],
                         enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1,
-                        temperature: float = 1.0, max_new_tokens: Optional[int] = None,
+                        temperature: float = 1.0, max_new_tokens=None,
                         dtype: Optional[torch.dtype] = None, return_device: bool = False,
                         seed=None) -> List[torch.Tensor]:
         """Engine feature (the reference asserts batch 1, valle.py:989): B independent utterances
         decoded together; result[b] equals `inference()` on utterance b alone.  Codes come back on the host, or
         (return_device=True) stay on the GPU, e.g. for the data-parallel gather of valle_b200.dist.
         Sampling (top_k != 1) keeps that promise with `seed` (an int s, or B ints): utterance b then equals
-        `inference(..., seed=s + b)`; top_k and temperature may be per-utterance sequences."""
+        `inference(..., seed=s + b)`; top_k and temperature may be per-utterance sequences.  max_new_tokens: one int
+        or one per utterance."""
         return self.engine(dtype).generate(texts, prompts, enroll_lens=enroll_lens, top_k=top_k,
                                            temperature=temperature, max_new_tokens=max_new_tokens,
                                            return_device=return_device, seed=seed)
+
+    def inference_stream(self, requests, slots: Optional[int] = None, max_context: Optional[int] = None,
+                         poll: int = 32, nar_batch: Optional[int] = None, dtype: Optional[torch.dtype] = None):
+        """Engine feature: continuous batching (ValleEngine.generate_stream).  requests: StreamRequest records
+        (text, prompt, enroll_len, seed, top_k, temperature, max_new_tokens), a sequence or a lazy iterator; yields
+        (index, codes [Tgen, 8] on the GPU) as each utterance completes, codes equal to `inference()` of that request
+        alone.  Decodes in `engine_dtype` (or `dtype`) with the model's `kv_cache_dtype`."""
+        return self.engine(dtype).generate_stream(requests, slots=slots, max_context=max_context, poll=poll,
+                                                  nar_batch=nar_batch)
 
     @torch.no_grad()
     def continual(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
