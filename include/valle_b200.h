@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 10
+#define VB_ABI_VERSION 11
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
@@ -346,6 +346,13 @@ typedef struct vb_ar_state {
   int32_t kv_dtype;
   int32_t kv_pad_unused;
   uint8_t *k_exp, *v_exp;
+  /* nucleus and repetition-aware sampling (ABI 11; vb_ar_head.greedy == 2 only), per row; see vb_sample_logits_ex.
+   * NULL, top_p == 1 and ras_window == 0 mean off, so a zero-initialised tail samples as before.  The window counts
+   * tokens[b, max(0, n_gen - ras_window) .. n_gen): the row's own generated ids only.  Not range-checked here (the
+   * step reads no host values); vb_sample_logits_ex states and checks the ranges. */
+  const float *top_p;          /* [B] in (0, 1] */
+  const int32_t *ras_window;   /* [B] in [0, 256] */
+  const int32_t *ras_max;      /* [B] >= 0: fall back when the draw's count in the window exceeds it */
 } vb_ar_state;
 
 typedef struct vb_ar_head {
@@ -358,7 +365,8 @@ typedef struct vb_ar_head {
   int32_t pe_rows;
   int32_t greedy;             /* 1: argmax + stop rule + append on device; 0: logits only (the caller draws and
                                  calls vb_ar_push_tokens); 2: seeded draw on the device from the state's sampler
-                                 arrays (vb_sample_logits), then the stop rule + append as for 1 */
+                                 arrays (vb_sample_logits_ex, with the row's n_gen as step and its tokens row as
+                                 history), then the stop rule + append as for 1 */
   vb_ln_fold fold;            /* final LayerNorm folded into predict_w (all-NULL: separate LayerNorm launch) */
 } vb_ar_head;
 
@@ -378,7 +386,7 @@ size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab);
 
 /* Admit k new utterances into rows slots[0..k) (device int32 [k], distinct, in [0, st->B)) of a running state (ABI 10;
  * after their prefill through vb_decoder_forward_slots).  h: fp32 [k, d], the last prefill row of each.  On entry the
- * slots' text_len, prompt_len, max_new (and, for head->greedy == 2, sample_seed / top_k / temperature) hold the new
+ * slots' text_len, prompt_len, max_new (and, for head->greedy == 2, the sampler arrays, top_p / ras_* included) hold the new
  * utterances' values.  The call runs vb_ar_head_step on a k-row state built from those rows, with n_gen = 0 and
  * finished = 0, so admitted row i gets exactly what vb_ar_head_step on a fresh k-row state gives its row i.
  * Writes, for the slots only: n_gen, finished, tokens[slot, 0], x_cur[slot, :] and logits[slot, 0:n_vocab].  Every other
@@ -416,6 +424,31 @@ int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int64_t *sa
 int vb_sample_logits(const float *logits, int64_t ld, int64_t n_rows, int n_vocab, const uint64_t *seeds,
                      const int32_t *steps, const int32_t *top_k, const float *temperature, int64_t *out_ids,
                      vb_stream_t stream);
+
+/* vb_sample_logits plus nucleus (top-p) filtering and repetition-aware sampling (ABI 11; VALL-E 2, Chen et al.
+ * 2024).  Row r, step n = steps[r], l' and the kept top-k set as in vb_sample_logits; then:
+ *   Nucleus, when top_p[r] < 1 (after top-k, as valle.py:1242-1284): the kept tokens in the order l' descending, ties
+ *   by ascending id, at positions j = 0 .. m-1; e_j = expf(l'_j - l'_0) (rounded fp32 subtraction).  Prefix sums, all
+ *   additions rounded fp32: positions are padded with e = 0 to 1280 and split into 256 runs of 5 (run t = positions
+ *   5t .. 5t+4); L_t,q = sequential sum of run t's first q+1 entries; the run totals L_t,4 get an inclusive Hillis-
+ *   Steele scan inside each group of 32 runs (for o = 1, 2, 4, 8, 16: s_t = s_t + s_{t-o} where t - o lies in the
+ *   group, all t at once); W_w = the scan at group w's last run; O_w = (((0 + W_0) + W_1) + ...) + W_{w-1} (O_0 = 0);
+ *   Z = O_7 + W_7; c_{5t+q} = (O_w(t) + s_{t-1}) + L_t,q, with s_{t-1} = 0 for a group's first run.  The nucleus is
+ *   positions 0 .. j* for the first j* with c_j* > top_p * Z (rounded fp32 product), or all m if none: the
+ *   reference's cumsum(softmax) > top_p, shifted right by one, with the division moved to the other side.  The draw is
+ *   the same Gumbel-max with the same g_i over the nucleus, so top_p = 1 gives vb_sample_logits's ids.
+ *   Repetition-aware sampling (RAS), when ras_window[r] = K >= 1: d = the draw above (argmax(l) when k == 1), c = the
+ *   number of j in [max(0, n - K), n) with tokens[r * tok_ld + j] == d.  If c > ras_max[r], d is replaced by the
+ *   Gumbel-max over ALL V tokens of l' (no top-k or top-p) with noise g'_i = g of the hash index i + 2048 (the same
+ *   splitmix64 of (seed, n, i + 2^11)).  With ras_max = floor(t_r K), c > ras_max is exactly c / K > t_r.
+ * top_p / ras_window / ras_max / tokens may be NULL (off).  VB_ERR_ARG when top_p is outside (0, 1], ras_window
+ * outside [0, 256] or ras_max < 0: the call reads those arrays back to the host to check them, so it waits for the
+ * stream and cannot be captured in a CUDA graph (vb_sample_logits can).  The AR decode tail (vb_ar_head.greedy == 2)
+ * runs the same function on vb_ar_state's arrays, with tokens = the state's tokens and n = the row's n_gen. */
+int vb_sample_logits_ex(const float *logits, int64_t ld, int64_t n_rows, int n_vocab, const uint64_t *seeds,
+                        const int32_t *steps, const int32_t *top_k, const float *temperature, const float *top_p,
+                        const int32_t *ras_window, const int32_t *ras_max, const int32_t *tokens, int64_t tok_ld,
+                        int64_t *out_ids, vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * a1  NAR stage tail (valle.py:1128-1134): samples = argmax(logits) over rows, written to

@@ -8,6 +8,8 @@ Modes, each warmed up first, then run in alternation `--repeats` times:
   torch        top_k=-100, seed=None: the per-step torch draw (topk_sampling + vb_ar_push_tokens), no graphs
   native       top_k=-100, seed=...: the seeded sampler in the decode step's tail, CUDA-graph replays
   native_k50   top_k=50, temperature=0.8, seed=...
+  native_p09   top_k=-100, top_p=0.9, seed=...: the nucleus (sort and scan of the whole row in the sampler)
+  native_p09_ras  native_p09 plus repetition-aware sampling, ras=(10, 0.1)
 Per mode: AR us per decode step from the engine's device events, ar_steps, library kernels and graph replays per
 step, frames generated (live rows), and the wall time of a synchronised generate().
 
@@ -39,6 +41,8 @@ MODES = {
     "torch": dict(top_k=-100),
     "native": dict(top_k=-100, seed=1234),
     "native_k50": dict(top_k=50, temperature=0.8, seed=1234),
+    "native_p09": dict(top_k=-100, top_p=0.9, seed=1234),
+    "native_p09_ras": dict(top_k=-100, top_p=0.9, ras=(10, 0.1), seed=1234),
 }
 
 
@@ -66,7 +70,7 @@ def run(eng, texts, prompts, kw):
 def profile(eng, texts, prompts, steps):
     from torch.profiler import ProfilerActivity, profile as prof
     res = {}
-    for name in ("greedy", "native"):
+    for name in ("greedy", "native", "native_p09", "native_p09_ras"):
         eng.generate(texts, prompts, max_new_tokens=steps, **MODES[name])   # warm, captured
         with prof(activities=[ProfilerActivity.CUDA]) as p:
             eng.generate(texts, prompts, max_new_tokens=steps, **MODES[name])
@@ -112,7 +116,7 @@ def main():
                        wall_ms=[round(r["wall_ms"], 1) for r in rs])
             print(json.dumps(out), flush=True)
         g = statistics.median(r["ar_us_per_step"] for r in rec["greedy"])
-        for name in ("torch", "native", "native_k50"):
+        for name in [n for n in MODES if n != "greedy"]:
             v = statistics.median(r["ar_us_per_step"] for r in rec[name])
             print(json.dumps(dict(B=B, mode=name, ar_us_per_step_vs_greedy=round(v / g - 1, 4))), flush=True)
         if a.profile_steps:

@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 VB_F32, VB_BF16, VB_E4M3 = 0, 1, 2
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -46,7 +46,8 @@ class ArState(C.Structure):
                 ("cache_layer_stride", C.c_int64), ("cache_seq_stride", C.c_int64),
                 ("cache_cap", C.c_int32), ("_unused", C.c_int32),
                 ("sample_seed", vp), ("top_k", vp), ("temperature", vp),
-                ("kv_dtype", C.c_int32), ("_kv_pad", C.c_int32), ("k_exp", vp), ("v_exp", vp)]
+                ("kv_dtype", C.c_int32), ("_kv_pad", C.c_int32), ("k_exp", vp), ("v_exp", vp),
+                ("top_p", vp), ("ras_window", vp), ("ras_max", vp)]
 
 
 class LnFold(C.Structure):
@@ -167,6 +168,8 @@ PROTOTYPES = {
     "vb_ar_decode_step": (C.c_int, [vp, C.POINTER(ArHead), C.POINTER(ArState), vp, C.c_size_t, vp]),
     "vb_ar_push_tokens": (C.c_int, [C.POINTER(ArHead), C.POINTER(ArState), vp, C.c_int, vp]),
     "vb_sample_logits": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp, vp]),
+    "vb_sample_logits_ex": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int64,
+                                      vp, vp]),
     "vb_nar_argmax_accumulate": (C.c_int, [vp, C.c_int64, C.c_int, C.c_int64, vp, C.c_int64, vp, vp,
                                            C.c_int64, vp, C.c_int, vp]),
     "vb_cross_entropy": (C.c_int, [vp, C.c_int64, vp, C.c_int64, C.c_int, C.c_int64, vp, vp]),

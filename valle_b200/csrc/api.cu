@@ -670,6 +670,9 @@ AdmitWs carve_admit_ws(Carve &c, const vb_decoder_desc &D, int k, int n_vocab) {
   cs.sample_seed = c.take<uint64_t>(k * 8);
   cs.top_k = c.take<int32_t>(k * 4);
   cs.temperature = c.take<float>(k * 4);
+  cs.top_p = c.take<float>(k * 4);
+  cs.ras_window = c.take<int32_t>(k * 4);
+  cs.ras_max = c.take<int32_t>(k * 4);
   w.head_ws_bytes = vb_ar_step_workspace(&D, k, kAdmitCap);
   w.head_ws = c.take(w.head_ws_bytes);
   return w;

@@ -4,10 +4,12 @@
 //     of the appended token (:1013-1015) so the next decode step needs no host round trip
 //     (the reference syncs to the host once per token).
 //     ar_sample_kernel<true> draws the token with the seeded sampler (sample_row) instead of taking the argmax.
-//   * sample_logits_kernel: the same sampler on caller-given logits (vb_sample_logits).
+//   * sample_logits_kernel: the same sampler on caller-given logits (vb_sample_logits, vb_sample_logits_ex).
 //   * nar_argmax_accumulate_kernel: samples = argmax(logits) (:1130) and
 //     y_emb[:, Tp:] += nar_audio_embeddings[i+1](samples) (:1133-1134).
 #include <math_constants.h>
+
+#include <vector>
 
 #include "common.cuh"
 #include "kernels.cuh"
@@ -33,18 +35,39 @@ __device__ __forceinline__ ArgMax warp_argmax(ArgMax a) {
   return a;
 }
 
-// ---- seeded top-k / temperature sampler (include/valle_b200.h vb_sample_logits), one CTA of 256 threads per row, the
-// row held in registers as 5 values per thread (element i = threadIdx.x + 256 j, V <= 1280)
+// ---- seeded top-k / temperature / nucleus sampler with repetition-aware fallback (include/valle_b200.h
+// vb_sample_logits_ex), one CTA of 256 threads per row, the row held in registers as 5 values per thread
+// (element i = threadIdx.x + 256 j, V <= 1280)
 struct SamplerArgs {
   const uint64_t *seed;
   const int32_t *top_k;
   const float *temperature;
+  const float *top_p;         // NULL: 1 (no nucleus)
+  const int32_t *ras_window;  // NULL: 0 (no repetition-aware fallback)
+  const int32_t *ras_max;
 };
+// one row's sampler parameters; hist: the utterance's generated ids [0, step) (read only when ras_window > 0)
+struct RowSampler {
+  uint64_t seed;
+  int step, k;
+  float temp, top_p;
+  int ras_window, ras_max;
+  const int32_t *hist;
+};
+__device__ __forceinline__ RowSampler row_sampler(const SamplerArgs &sa, int64_t r, int step, const int32_t *hist) {
+  return RowSampler{sa.seed[r], step, sa.top_k[r], sa.temperature[r], sa.top_p ? sa.top_p[r] : 1.f,
+                    sa.ras_window ? sa.ras_window[r] : 0, sa.ras_max ? sa.ras_max[r] : 0, hist};
+}
+constexpr int kSortMax = 2048;  // power of two >= 5 * 256
+constexpr int kRasStream = 2048;  // the fallback draw hashes id i at index i + 2^11 (disjoint from the first draw's)
 struct SamplerSmem {
   unsigned hist[256];
   unsigned wsum[8];
   ArgMax wbest[8];
   int sel_bin, sel_k;
+  float wsumf[8];
+  int count, cut, ras_count;
+  unsigned long long keys[kSortMax];  // nucleus: (float_key(l'), ~id) of the kept tokens, sorted descending
 };
 // order-preserving float <-> uint32 (larger float, larger key)
 __device__ __forceinline__ uint32_t float_key(float f) {
@@ -103,30 +126,139 @@ __device__ float radix_kth(const float (&x)[5], int n, int k, SamplerSmem &sm) {
   }
   return key_float(prefix);
 }
-// Gumbel-max draw over the top-k set of l / T; `amax` = argmax(l), returned for k == 1.  Called by all 256 threads,
-// returns the id to every thread.
-__device__ int sample_row(const float (&l)[5], int n, int amax, uint64_t seed, int step, int k, float temp,
-                          SamplerSmem &sm) {
-  if (k == 1) return amax;
+// Gumbel noise g_i of (seed, step, hash index): 23 bits, m + 0.5 fits fp32's 24-bit significand, so u is exact, in
+// [2^-24, 1 - 2^-24] and g finite (a 24-bit m + 0.5 would round 2^24 - 0.5 up to 2^24: u = 1, g = +inf)
+__device__ __forceinline__ float gumbel(uint64_t seed, int step, int idx) {
+  const uint64_t h = mix64(seed, (uint64_t)(int64_t)step, (uint64_t)idx);
+  const float u = ((float)(uint32_t)(h >> 41) + 0.5f) * 1.1920928955078125e-7f;
+  return -logf(-logf(u));
+}
+// (value, ascending id) order of the nucleus as one integer: a larger key comes first
+__device__ __forceinline__ unsigned long long order_key(float v, int i) {
+  return ((unsigned long long)float_key(v) << 32) | (0xFFFFFFFFu - (uint32_t)i);
+}
+// Nucleus of the kept set (include/valle_b200.h vb_sample_logits_ex): sorts the kept tokens by order_key (bitonic, in
+// shared memory, over the next power of two >= their count), sums e = expf(l' - max) over sorted positions in the
+// association order the header states (5 positions per thread in sequence, a Hillis-Steele warp scan, the warp
+// totals in sequence) and returns the order key of the first position whose prefix sum exceeds top_p * Z (of the last
+// kept token if none does): the nucleus is every kept token whose order key is >= it.
+__device__ unsigned long long nucleus_cut(const float (&x)[5], const bool (&kept)[5], float top_p, SamplerSmem &sm) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // gather the kept keys into keys[0, m) (in any order: the keys are distinct, so the sort fixes the result), zeros up
+  // to N
+  if (tid == 0) sm.count = 0;
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < 5; ++j)
+    if (kept[j]) sm.keys[atomicAdd(&sm.count, 1)] = order_key(x[j], tid + j * 256);
+  __syncthreads();
+  const int m = sm.count;
+  int N = 2;
+  while (N < m) N <<= 1;
+  for (int i = m + tid; i < N; i += 256) sm.keys[i] = 0ull;
+  if (tid == 0) sm.cut = m - 1;
+  __syncthreads();
+#pragma unroll 1
+  for (int size = 2; size <= N; size <<= 1) {
+#pragma unroll 1
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = tid; t < (N >> 1); t += 256) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        const unsigned long long a = sm.keys[lo], b = sm.keys[hi];
+        if ((a < b) == ((lo & size) == 0)) {  // descending where bit `size` of lo is clear
+          sm.keys[lo] = b;
+          sm.keys[hi] = a;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  const float mx = key_float((uint32_t)(sm.keys[0] >> 32));
+  float c[5], s = 0.f;
+#pragma unroll
+  for (int q = 0; q < 5; ++q) {
+    const int p = tid * 5 + q;
+    const float e = p < m ? expf(__fsub_rn(key_float((uint32_t)(sm.keys[p] >> 32)), mx)) : 0.f;
+    s = __fadd_rn(s, e);
+    c[q] = s;
+  }
+  float ws = s;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float t = __shfl_up_sync(0xffffffffu, ws, o);
+    if (lane >= o) ws = __fadd_rn(ws, t);
+  }
+  float ex = __shfl_up_sync(0xffffffffu, ws, 1);
+  if (lane == 0) ex = 0.f;
+  if (lane == 31) sm.wsumf[warp] = ws;
+  __syncthreads();
+  float off = 0.f, Z = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) {
+    if (w == warp) off = Z;
+    Z = __fadd_rn(Z, sm.wsumf[w]);
+  }
+  const float thr = __fmul_rn(top_p, Z), base = __fadd_rn(off, ex);
+#pragma unroll
+  for (int q = 0; q < 5; ++q) {
+    const int p = tid * 5 + q;
+    if (p < m && __fadd_rn(base, c[q]) > thr) {
+      atomicMin(&sm.cut, p);
+      break;
+    }
+  }
+  __syncthreads();
+  return sm.keys[sm.cut];
+}
+// Gumbel-max draw over the top-k set of l / T, narrowed to its nucleus when top_p < 1; `amax` = argmax(l), the draw
+// for k == 1.  With ras_window > 0, a draw that fills more than ras_max of the last ras_window ids of `hist` is
+// replaced by a Gumbel-max draw over all of l / T.  Called by all 256 threads, returns the id to every thread.
+__device__ int sample_row(const float (&l)[5], int n, int amax, const RowSampler &r, SamplerSmem &sm) {
+  const bool ras = r.ras_window > 0;
+  if (r.k == 1 && !ras) return amax;
   const int tid = threadIdx.x;
   float x[5];
 #pragma unroll
-  for (int j = 0; j < 5; ++j) x[j] = temp != 1.f ? __fdiv_rn(l[j], temp) : l[j];
-  const float kth = (k > 0 && k < n) ? radix_kth(x, n, k, sm) : -CUDART_INF_F;
-  ArgMax best{-CUDART_INF_F, 0x7fffffff};
+  for (int j = 0; j < 5; ++j) x[j] = r.temp != 1.f ? __fdiv_rn(l[j], r.temp) : l[j];
+  int d = amax;
+  if (r.k != 1) {
+    const float kth = (r.k > 0 && r.k < n) ? radix_kth(x, n, r.k, sm) : -CUDART_INF_F;
+    bool kept[5];
 #pragma unroll
-  for (int j = 0; j < 5; ++j) {
-    const int i = tid + j * 256;
-    if (i < n && x[j] >= kth) {
-      const uint64_t h = mix64(seed, (uint64_t)(int64_t)step, (uint64_t)i);
-      // 23 bits: m + 0.5 fits fp32's 24-bit significand, so u is exact, in [2^-24, 1 - 2^-24] and g finite
-      // (a 24-bit m + 0.5 would round 2^24 - 0.5 up to 2^24: u = 1, g = +inf)
-      const float u = ((float)(uint32_t)(h >> 41) + 0.5f) * 1.1920928955078125e-7f;
-      const float g = -logf(-logf(u));
-      best = better(best, ArgMax{__fadd_rn(x[j], g), i});
+    for (int j = 0; j < 5; ++j) kept[j] = tid + j * 256 < n && x[j] >= kth;
+    if (r.top_p < 1.f) {
+      const unsigned long long cut = nucleus_cut(x, kept, r.top_p, sm);
+#pragma unroll
+      for (int j = 0; j < 5; ++j) kept[j] = kept[j] && order_key(x[j], tid + j * 256) >= cut;
+    }
+    ArgMax best{-CUDART_INF_F, 0x7fffffff};
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      const int i = tid + j * 256;
+      if (kept[j]) best = better(best, ArgMax{__fadd_rn(x[j], gumbel(r.seed, r.step, i)), i});
+    }
+    d = block_argmax(best, sm.wbest).i;
+  }
+  if (ras) {
+    // count of d among the utterance's last ras_window ids (warp 0), then the unfiltered redraw if it is too high
+    if (tid < 32) {
+      int c = 0;
+      for (int j = max(0, r.step - r.ras_window) + tid; j < r.step; j += 32) c += r.hist[j] == d;
+      c = __reduce_add_sync(0xffffffffu, c);
+      if (tid == 0) sm.ras_count = c;
+    }
+    __syncthreads();  // also orders the reads of sm.wbest above before the writes below
+    if (sm.ras_count > r.ras_max) {
+      ArgMax best{-CUDART_INF_F, 0x7fffffff};
+#pragma unroll
+      for (int j = 0; j < 5; ++j) {
+        const int i = tid + j * 256;
+        if (i < n) best = better(best, ArgMax{__fadd_rn(x[j], gumbel(r.seed, r.step, i + kRasStream)), i});
+      }
+      d = block_argmax(best, sm.wbest).i;
     }
   }
-  return block_argmax(best, sm.wbest).i;
+  return d;
 }
 
 template <bool kSample>
@@ -157,14 +289,8 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
   // scalars of the stop rule: in flight together with the logits instead of after the argmax
   const int n_new = n_gen[b], p_len = prompt_len[b], cap_new = max_new[b];
   const int forced_tok = forced ? (int)forced[b] : -1;
-  uint64_t seed = 0;
-  int top_k = 0;
-  float temp = 1.f;
-  if constexpr (kSample) {
-    seed = sa.seed[b];
-    top_k = sa.top_k[b];
-    temp = sa.temperature[b];
-  }
+  RowSampler rs{};
+  if constexpr (kSample) rs = row_sampler(sa, b, n_new, tokens + (int64_t)b * tok_stride);
   float *row = logits + (int64_t)b * ld_logits;
   float lv[5];  // kSample: the row in registers, element tid + 256 j
   ArgMax best{-CUDART_INF_F, 0x7fffffff};
@@ -223,7 +349,7 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
   if constexpr (kSample) {
     __shared__ SamplerSmem smp;
     best = block_argmax(best, wbest);
-    draw = sample_row(lv, n_vocab, best.i, seed, n_new, top_k, temp, smp);
+    draw = sample_row(lv, n_vocab, best.i, rs, smp);
   } else {
     best = warp_argmax(best);
     if (lane == 0) wbest[warp] = best;
@@ -275,7 +401,7 @@ int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const v
   if (sample) {
     VB_CHECK_ARG(st->sample_seed && st->top_k && st->temperature, "vb_ar_head.greedy == 2: sampler arrays not set");
     VB_CHECK_ARG(head->n_vocab <= 5 * 256, "device sampler: n_vocab %d > 1280", head->n_vocab);
-    sa = SamplerArgs{st->sample_seed, st->top_k, st->temperature};
+    sa = SamplerArgs{st->sample_seed, st->top_k, st->temperature, st->top_p, st->ras_window, st->ras_max};
   }
   VB_CUDA(launch_kernel(sample ? ar_sample_kernel<true> : ar_sample_kernel<false>, dim3(st->B), dim3(256), 0, s, pdl,
                         logits, ld_logits, in.part, in.splits, in.ldp, head->n_vocab, head->eos_id, head->audio_emb,
@@ -304,6 +430,9 @@ ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__
         const_cast<uint64_t *>(cs.sample_seed)[i] = st.sample_seed[s];
         const_cast<int32_t *>(cs.top_k)[i] = st.top_k[s];
         const_cast<float *>(cs.temperature)[i] = st.temperature[s];
+        const_cast<float *>(cs.top_p)[i] = st.top_p ? st.top_p[s] : 1.f;
+        const_cast<int32_t *>(cs.ras_window)[i] = st.ras_window ? st.ras_window[s] : 0;
+        const_cast<int32_t *>(cs.ras_max)[i] = st.ras_max ? st.ras_max[s] : 0;
       }
     }
     return;
@@ -325,9 +454,9 @@ int launch_ar_admit_copy(vb_ar_state *st, const vb_ar_state *cs, const int32_t *
 }
 
 __global__ void __launch_bounds__(256)
-sample_logits_kernel(const float *__restrict__ logits, int64_t ld, int n_vocab, const uint64_t *__restrict__ seeds,
-                     const int32_t *__restrict__ steps, const int32_t *__restrict__ top_k,
-                     const float *__restrict__ temperature, int64_t *__restrict__ out_ids) {
+sample_logits_kernel(const float *__restrict__ logits, int64_t ld, int n_vocab, SamplerArgs sa,
+                     const int32_t *__restrict__ steps, const int32_t *__restrict__ tokens, int64_t tok_ld,
+                     int64_t *__restrict__ out_ids) {
   __shared__ SamplerSmem sm;
   const int64_t r = blockIdx.x;
   const int tid = threadIdx.x;
@@ -342,7 +471,7 @@ sample_logits_kernel(const float *__restrict__ logits, int64_t ld, int n_vocab, 
   }
   best = block_argmax(best, sm.wbest);
   __syncthreads();  // sm.wbest is reused by the draw
-  const int id = sample_row(l, n_vocab, best.i, seeds[r], steps[r], top_k[r], temperature[r], sm);
+  const int id = sample_row(l, n_vocab, best.i, row_sampler(sa, r, steps[r], tokens + r * tok_ld), sm);
   if (tid == 0) out_ids[r] = id;
 }
 
@@ -394,12 +523,51 @@ VB_API int vb_nar_argmax_accumulate(const float *logits, int64_t n_rows, int n_v
 VB_API int vb_sample_logits(const float *logits, int64_t ld, int64_t n_rows, int n_vocab, const uint64_t *seeds,
                             const int32_t *steps, const int32_t *top_k, const float *temperature, int64_t *out_ids,
                             vb_stream_t stream) {
+  return vb_sample_logits_ex(logits, ld, n_rows, n_vocab, seeds, steps, top_k, temperature, nullptr, nullptr, nullptr,
+                             nullptr, 0, out_ids, stream);
+}
+
+namespace {
+// copies n device values to the host (on `s`, waiting for them) to check the per-row sampler parameters
+template <class T>
+int fetch_rows(const T *dev, int64_t n, std::vector<T> &host, cudaStream_t s) {
+  host.resize((size_t)n);
+  VB_CUDA(cudaMemcpyAsync(host.data(), dev, (size_t)n * sizeof(T), cudaMemcpyDeviceToHost, s));
+  VB_CUDA(cudaStreamSynchronize(s));
+  return VB_OK;
+}
+}  // namespace
+
+VB_API int vb_sample_logits_ex(const float *logits, int64_t ld, int64_t n_rows, int n_vocab, const uint64_t *seeds,
+                               const int32_t *steps, const int32_t *top_k, const float *temperature,
+                               const float *top_p, const int32_t *ras_window, const int32_t *ras_max,
+                               const int32_t *tokens, int64_t tok_ld, int64_t *out_ids, vb_stream_t stream) {
   VB_CHECK_ARG(n_vocab >= 1 && n_vocab <= 5 * 256, "vb_sample_logits: n_vocab %d not in [1, 1280]", n_vocab);
   VB_CHECK_ARG(n_rows >= 0 && n_rows < (1ll << 31), "vb_sample_logits: n_rows out of range");
   if (n_rows == 0) return VB_OK;
   VB_CHECK_ARG(logits && seeds && steps && top_k && temperature && out_ids, "vb_sample_logits: null argument");
-  sample_logits_kernel<<<(unsigned)n_rows, 256, 0, (cudaStream_t)stream>>>(logits, ld, n_vocab, seeds, steps, top_k,
-                                                                          temperature, out_ids);
+  VB_CHECK_ARG(!ras_window || (ras_max && tokens), "vb_sample_logits_ex: ras_window needs ras_max and tokens");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (top_p) {
+    std::vector<float> p;
+    VB_TRY(fetch_rows(top_p, n_rows, p, s));
+    for (int64_t r = 0; r < n_rows; ++r)
+      VB_CHECK_ARG(p[r] > 0.f && p[r] <= 1.f, "vb_sample_logits_ex: top_p[%lld] = %g not in (0, 1]", (long long)r,
+                   (double)p[r]);
+  }
+  if (ras_window) {
+    std::vector<int32_t> w, mx;
+    VB_TRY(fetch_rows(ras_window, n_rows, w, s));
+    VB_TRY(fetch_rows(ras_max, n_rows, mx, s));
+    for (int64_t r = 0; r < n_rows; ++r) {
+      VB_CHECK_ARG(w[r] >= 0 && w[r] <= 256, "vb_sample_logits_ex: ras_window[%lld] = %d not in [0, 256]",
+                   (long long)r, w[r]);
+      VB_CHECK_ARG(mx[r] >= 0, "vb_sample_logits_ex: ras_max[%lld] = %d < 0", (long long)r, mx[r]);
+    }
+  }
+  sample_logits_kernel<<<(unsigned)n_rows, 256, 0, s>>>(
+      logits, ld, n_vocab, SamplerArgs{seeds, top_k, temperature, top_p, ras_window, ras_max}, steps, tokens, tok_ld,
+      out_ids);
   VB_LAUNCH_CHECK();
   return VB_OK;
 }

@@ -72,7 +72,7 @@ class EngineStats:
 
 class StreamRequest(NamedTuple):
     """One utterance of ValleEngine.generate_stream: text int64 [S] phoneme ids, prompt int64 [Tp, Q] codec ids, and
-    what generate() takes per utterance.  top_k != 1 needs a seed (the seeded device sampler)."""
+    what generate() takes per utterance.  top_k != 1 and ras need a seed (the seeded device sampler)."""
     text: torch.Tensor
     prompt: torch.Tensor
     enroll_len: Optional[int] = None
@@ -80,6 +80,8 @@ class StreamRequest(NamedTuple):
     top_k: int = 1
     temperature: float = 1.0
     max_new_tokens: Optional[int] = None
+    top_p: float = 1.0
+    ras: Optional[Tuple[int, float]] = None
 
 
 class _ArBuffers:
@@ -111,6 +113,9 @@ class _ArBuffers:
         self.sample_seed = torch.zeros(B, dtype=torch.int64, device=dev)
         self.top_k = torch.zeros(B, **i32)
         self.temperature = torch.ones(B, dtype=torch.float32, device=dev)
+        self.top_p = torch.ones(B, dtype=torch.float32, device=dev)
+        self.ras_window = torch.zeros(B, **i32)
+        self.ras_max = torch.zeros(B, **i32)
         st = L.ArState()
         st.B, st.tok_stride = B, tok_stride
         st.text_len, st.prompt_len, st.max_new = self.text_len.data_ptr(), self.prompt_len.data_ptr(), self.max_new.data_ptr()
@@ -120,6 +125,7 @@ class _ArBuffers:
         st.cache_layer_stride, st.cache_seq_stride, st.cache_cap = self.kcache.stride(0), self.kcache.stride(1), cap
         st.sample_seed, st.top_k = self.sample_seed.data_ptr(), self.top_k.data_ptr()
         st.temperature = self.temperature.data_ptr()
+        st.top_p, st.ras_window, st.ras_max = self.top_p.data_ptr(), self.ras_window.data_ptr(), self.ras_max.data_ptr()
         if fp8:
             st.kv_dtype, st.k_exp, st.v_exp = L.VB_E4M3, self.k_exp.data_ptr(), self.v_exp.data_ptr()
         self.st = st
@@ -138,10 +144,55 @@ def _is_seq(v) -> bool:
     return isinstance(v, (list, tuple)) or (isinstance(v, (torch.Tensor, np.ndarray)) and v.ndim > 0)
 
 
-def _sampler_args(B: int, seed, top_k, temperature):
-    """Validated per-utterance (seeds, top_k, temperature) lists of a seeded call: an int seed s stands for s, s+1, ...,
-    s+B-1 (so utterance b decoded alone with seed s+b draws what it draws in the batch); top_k / temperature are one
-    value or a sequence of B."""
+def _check_top_p(ps):
+    if any(not 0.0 < p <= 1.0 for p in ps):   # NaN fails too
+        raise ValueError("top_p must lie in (0, 1]")
+
+
+def _ras_rows(B: int, ras) -> List[Optional[Tuple[int, float]]]:
+    """Validated per-utterance repetition-aware sampling settings: None (off), one (window, threshold) pair for every
+    utterance, or a sequence of B pairs / Nones.  window: an int in [1, 256]; threshold in [0, 1)."""
+    if ras is None:
+        return [None] * B
+    per = _is_seq(ras) and len(ras) > 0 and (ras[0] is None or _is_seq(ras[0]))
+    rows = list(ras) if per else [ras] * B
+    if len(rows) != B:
+        raise ValueError(f"ras: {len(rows)} values for {B} utterances")
+    out = []
+    for r in rows:
+        if r is None:
+            out.append(None)
+            continue
+        if not _is_seq(r) or len(r) != 2:
+            raise ValueError(f"ras: expected a (window, threshold) pair, got {r!r}")
+        w, t = r
+        if isinstance(w, bool) or not isinstance(w, (int, np.integer)) or not 1 <= int(w) <= 256:
+            raise ValueError(f"ras: the window must be an int in [1, 256] (got {w!r})")
+        t = float(t)
+        if not 0.0 <= t < 1.0:
+            raise ValueError(f"ras: the threshold must lie in [0, 1) (got {t!r})")
+        out.append((int(w), t))
+    return out
+
+
+def _ras_arrays(rows) -> Tuple[List[int], List[int]]:
+    """(ras_window, ras_max) of vb_ar_state per utterance: ras_max = floor(t K), the largest count c with c / K <= t, so
+    that the device's integer test count > ras_max is exactly count / K > t as Python evaluates it (t K rounded to a
+    double can land just below an integer: 0.29 * 100 = 28.999...)"""
+    def ras_max(K, t):
+        c = math.floor(t * K)
+        while (c + 1) / K <= t:
+            c += 1
+        while c > 0 and c / K > t:
+            c -= 1
+        return c
+    return [0 if r is None else r[0] for r in rows], [0 if r is None else ras_max(*r) for r in rows]
+
+
+def _sampler_args(B: int, seed, top_k, temperature, top_p=1.0, ras=None):
+    """Validated per-utterance (seeds, top_k, temperature, top_p, ras) lists of a seeded call: an int seed s stands for
+    s, s+1, ..., s+B-1 (so utterance b decoded alone with seed s+b draws what it draws in the batch); top_k /
+    temperature / top_p are one value or a sequence of B; ras as _ras_rows takes it."""
     def per_row(v, what):
         if _is_seq(v):
             v = [x.item() if hasattr(x, "item") else x for x in v]
@@ -160,7 +211,9 @@ def _sampler_args(B: int, seed, top_k, temperature):
     ts = [float(x) for x in per_row(temperature, "temperature")]
     if any(not math.isfinite(t) or t <= 0.0 for t in ts):
         raise ValueError("temperature must be finite and > 0")
-    return seeds, ks, ts
+    ps = [float(x) for x in per_row(top_p, "top_p")]
+    _check_top_p(ps)
+    return seeds, ks, ts, ps, _ras_rows(B, ras)
 
 
 def _seg_ranges(starts, lens):
@@ -349,7 +402,8 @@ class ValleEngine:
                  enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1, temperature: float = 1.0,
                  max_new_tokens=None, poll: int = 32,
                  return_device: bool = False, trace: Optional[dict] = None,
-                 forced: Optional[Sequence[torch.Tensor]] = None, seed=None) -> List[torch.Tensor]:
+                 forced: Optional[Sequence[torch.Tensor]] = None, seed=None, top_p=1.0,
+                 ras=None) -> List[torch.Tensor]:
         """texts[b]: int64 [S_b] phoneme ids; prompts[b]: int64 [Tp_b, Q] codec ids (host or device).
         Returns codes[b]: int64 [Tgen_b, Q] -- per utterance exactly what VALLE.inference returns.
 
@@ -357,8 +411,14 @@ class ValleEngine:
         `sample_on_host`).  An int s, or a sequence of B ints in [0, 2**64), selects the seeded device sampler
         (vb_sample_logits): utterance b draws from seed s + b (or seed[b]) and its decode step, inside the CUDA-graph
         decode step, so its codes do not depend on the batch it shares, its slot, or how the call is split.  With a
-        seed, top_k and temperature may be per-utterance sequences; every top_k == 1 is the greedy path.
-        max_new_tokens: None, one int, or a sequence of B ints (one cap per utterance).
+        seed, top_k, temperature and top_p may be per-utterance sequences; every top_k == 1 without ras is the greedy
+        path.  max_new_tokens: None, one int, or a sequence of B ints (one cap per utterance).
+        top_p: nucleus filtering after top-k (valle.py:1242-1284), in (0, 1]; 1 is off.  Without a seed it goes to the
+        reference's own topk_sampling.
+        ras: repetition-aware sampling (VALL-E 2), seeded calls only: a (window, threshold) pair, or one pair / None per
+        utterance.  A draw that already makes up more than `threshold` of the utterance's last `window` codes (window
+        in [1, 256], threshold in [0, 1)) is replaced by a draw from the unfiltered distribution; see
+        include/valle_b200.h vb_sample_logits_ex.
 
         Test hooks: `trace` collects AR logits (trace["steps"] = set of iterations or "all") and, with
         trace["nar"] = True, the NAR logits / argmax of every stage; `forced[b]` = int64 [T_b, Q] codes the decode is
@@ -370,14 +430,21 @@ class ValleEngine:
         assert B == len(prompts) and B >= 1
         kv_dtype = self.kv_cache_dtype()
         sampler = None
+        if ras is not None and self.sample_on_host:
+            raise ValueError("ras draws on the device; it cannot be combined with sample_on_host = True")
         if seed is not None:
             if self.sample_on_host:
                 raise ValueError("seed= selects the device sampler; it cannot be combined with sample_on_host = True")
-            sampler = _sampler_args(B, seed, top_k, temperature)
-            if all(k == 1 for k in sampler[1]):
+            sampler = _sampler_args(B, seed, top_k, temperature, top_p, ras)
+            if all(k == 1 for k in sampler[1]) and all(r is None for r in sampler[4]):
                 sampler, top_k = None, 1          # greedy: the seed draws nothing
-        elif _is_seq(top_k) or _is_seq(temperature):
-            raise ValueError("per-utterance top_k / temperature need seed= (the seeded device sampler)")
+        elif ras is not None:
+            raise ValueError("ras needs seed= (the seeded device sampler)")
+        elif _is_seq(top_k) or _is_seq(temperature) or _is_seq(top_p):
+            raise ValueError("per-utterance top_k / temperature / top_p need seed= (the seeded device sampler)")
+        else:
+            top_p = float(top_p)
+            _check_top_p([top_p])
         if B > self.max_tc_batch and self.dtype == torch.bfloat16 and trace is None and forced is None:
             # the tensor-core decode projections take up to 64 rows (one UMMA N tile): a larger batch is decoded as
             # consecutive groups of <= 64 utterances instead of falling onto the CUDA-core GEMV path
@@ -387,9 +454,10 @@ class ValleEngine:
             for b0 in range(0, B, self.max_tc_batch):
                 b1 = min(B, b0 + self.max_tc_batch)
                 if sampler is None:
-                    kw = dict(top_k=top_k, temperature=temperature)
+                    kw = dict(top_k=top_k, temperature=temperature, top_p=top_p)
                 else:   # by absolute utterance index
-                    kw = dict(seed=sampler[0][b0:b1], top_k=sampler[1][b0:b1], temperature=sampler[2][b0:b1])
+                    kw = dict(seed=sampler[0][b0:b1], top_k=sampler[1][b0:b1], temperature=sampler[2][b0:b1],
+                              top_p=sampler[3][b0:b1], ras=sampler[4][b0:b1])
                 mnt = max_new_tokens[b0:b1] if _is_seq(max_new_tokens) else max_new_tokens
                 outs += self.generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
                                       max_new_tokens=mnt, poll=poll, return_device=return_device, **kw)
@@ -436,10 +504,14 @@ class ValleEngine:
         buf.n_gen.zero_()
         buf.finished.zero_()
         if native:
-            seeds, ks, ts = sampler
+            seeds, ks, ts, ps, rr = sampler
             buf.sample_seed.copy_(torch.tensor([x - (1 << 64) if x >= 1 << 63 else x for x in seeds], dtype=torch.int64))
             buf.top_k.copy_(torch.tensor(ks, dtype=torch.int32))
             buf.temperature.copy_(torch.tensor(ts, dtype=torch.float32))
+            buf.top_p.copy_(torch.tensor(ps, dtype=torch.float32))
+            rw, rm = _ras_arrays(rr)
+            buf.ras_window.copy_(torch.tensor(rw, dtype=torch.int32))
+            buf.ras_max.copy_(torch.tensor(rm, dtype=torch.int32))
         pe_a = self._pe(m.ar_audio_position, max(Tp) + max(cap_new) + 2)
         h_last = self._prefill(buf, p, pe_a)
         head = self._head(pe_a, 2 if native else int(greedy))
@@ -457,7 +529,7 @@ class ValleEngine:
         if forced_steps is not None:
             poll = 1
         if not (greedy or native):
-            self._sample_push(buf, head, top_k, temperature, None if forced_steps is None else forced_steps[0])
+            self._sample_push(buf, head, top_k, temperature, None if forced_steps is None else forced_steps[0], top_p)
         if any(t.is_cuda for t in list(texts) + list(prompts)):
             ops.check_oob(dev)  # ids that were already on the device are range-checked by the embedding kernels
         ev[1].record()
@@ -474,7 +546,7 @@ class ValleEngine:
                     fs = None
                     if forced_steps is not None:
                         fs = forced_steps[min(steps + 1, forced_steps.shape[0] - 1)]
-                    self._decode_step(buf, head, greedy or native, top_k, temperature, fs)
+                    self._decode_step(buf, head, greedy or native, top_k, temperature, fs, top_p)
             steps += n
             if trace is not None and want(steps):  # poll == 1 here: the logits row of iteration `steps`
                 trace["ar_logits"][steps] = buf.logits[:, : self.n_vocab].clone()
@@ -533,7 +605,8 @@ class ValleEngine:
         takes at most 64 (one tensor-core decode group).  New requests are admitted, and the stop flags read, every
         `poll` decode steps; the NAR runs over every `nar_batch` (default `slots`) finished utterances, and over the
         rest once nothing is left to decode.  Sampling is greedy, or seeded per request (`seed`, with top_k /
-        temperature): the draws depend on the seed and the step only, never on the slot or the schedule."""
+        temperature / top_p / ras): the draws depend on the seed, the step and the request's own codes only, never on
+        the slot or the schedule."""
         with torch.cuda.device(self.device):
             self._refresh()
         kv_dtype = self.kv_cache_dtype()
@@ -588,6 +661,9 @@ class ValleEngine:
             buf.sample_seed.zero_()
             buf.top_k.fill_(1)
             buf.temperature.fill_(1.0)
+            buf.top_p.fill_(1.0)
+            buf.ras_window.zero_()
+            buf.ras_max.zero_()
             pe_a = self._pe(m.ar_audio_position, cap + 2)
             heads = {g: self._head(pe_a, g) for g in (1, 2)}
             ws = torch.empty(self.lib.vb_ar_admit_workspace(C.byref(self.ar.desc), n_slots, self.n_vocab),
@@ -613,10 +689,11 @@ class ValleEngine:
                     raise ValueError(f"request {idx}: text must be [S > 0] ids and prompt [Tp, {Q}] codes")
                 seed, top_k = r.seed, r.top_k
                 if seed is None:
-                    if top_k != 1:
-                        raise ValueError(f"request {idx}: top_k={top_k} needs a seed (the seeded device sampler)")
+                    if top_k != 1 or r.ras is not None:
+                        raise ValueError(f"request {idx}: top_k={top_k} / ras need a seed (the seeded device sampler)")
                     seed = 0
-                seeds, ks, ts = _sampler_args(1, seed, top_k, r.temperature)
+                seeds, ks, ts, ps, rr = _sampler_args(1, seed, top_k, r.temperature, r.top_p,
+                                                      None if r.ras is None else [r.ras])
                 if pm in (2, 4) and r.enroll_len is None:
                     raise ValueError(f"request {idx}: prefix_mode {pm} needs enroll_len")
                 if self._context(r) > max_context:
@@ -624,9 +701,9 @@ class ValleEngine:
                 _check_ids([r.text], NUM_TEXT_TOKENS, "phoneme")
                 _check_ids([r.prompt[:, :1]], NUM_AUDIO_TOKENS + 1, "prompt code (first codebook)")
                 _check_ids([r.prompt[:, 1:]], NUM_AUDIO_TOKENS, "prompt code")
-                if ks[0] != 1:
+                if ks[0] != 1 or rr[0] is not None:
                     mode = 2
-                out.append((idx, r, seeds[0], ks[0], ts[0]))
+                out.append((idx, r, seeds[0], ks[0], ts[0], ps[0], rr[0]))
             return out
 
         def admit(new):
@@ -649,6 +726,10 @@ class ValleEngine:
             buf.top_k.index_copy_(0, idx_d, torch.tensor([n[3] for n in new], dtype=torch.int32).to(dev, non_blocking=True))
             buf.temperature.index_copy_(0, idx_d, torch.tensor([n[4] for n in new], dtype=torch.float32).to(
                 dev, non_blocking=True))
+            buf.top_p.index_copy_(0, idx_d, torch.tensor([n[5] for n in new], dtype=torch.float32).to(dev, non_blocking=True))
+            rw, rm = _ras_arrays([n[6] for n in new])
+            buf.ras_window.index_copy_(0, idx_d, torch.tensor(rw, dtype=torch.int32).to(dev, non_blocking=True))
+            buf.ras_max.index_copy_(0, idx_d, torch.tensor(rm, dtype=torch.int32).to(dev, non_blocking=True))
             h = self._prefill(buf, p, pe_a)
             L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), k, p.slots_d.data_ptr(),
                                          C.byref(buf.st), ws.data_ptr(), ws.numel(), L.stream_ptr()), "vb_ar_admit")
@@ -857,12 +938,12 @@ class ValleEngine:
         ops.add_pe(tmp, pe, alpha.detach(), x, n, positions=pos, out_rows=rows)
 
     def _decode_step(self, buf: _ArBuffers, head: L.ArHead, greedy: bool, top_k: int, temperature: float,
-                     forced_step: Optional[torch.Tensor] = None):
+                     forced_step: Optional[torch.Tensor] = None, top_p: float = 1.0):
         """one decode step without a graph; greedy: the step draws on the device (argmax, or the seeded sampler when
         head.greedy == 2), else on the host"""
         self._launch_step(buf, head)
         if not greedy:
-            self._sample_push(buf, head, top_k, temperature, forced_step)
+            self._sample_push(buf, head, top_k, temperature, forced_step, top_p)
 
     def _replay_steps(self, buf: _ArBuffers, head: L.ArHead, k: int):
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
@@ -892,7 +973,7 @@ class ValleEngine:
                                            buf.ws.numel(), L.stream_ptr()), "vb_ar_decode_step")
 
     def _sample_push(self, buf: _ArBuffers, head: L.ArHead, top_k: int, temperature: float,
-                     forced_step: Optional[torch.Tensor] = None):
+                     forced_step: Optional[torch.Tensor] = None, top_p: float = 1.0):
         """valle.py:1287-1302 topk_sampling with torch's own RNG stream (so a fixed torch seed gives
         the reference's draws), then the stop rule + append on the device."""
         if forced_step is not None:  # teacher forcing (test hook): the given ids instead of a draw
@@ -904,10 +985,10 @@ class ValleEngine:
         logits = buf.logits[:, : self.n_vocab].clone()
         if self.sample_on_host:
             host = logits.cpu()
-            samp = torch.cat([topk_sampling(host[b:b + 1], top_k=top_k, top_p=1.0, temperature=temperature).view(-1)
+            samp = torch.cat([topk_sampling(host[b:b + 1], top_k=top_k, top_p=top_p, temperature=temperature).view(-1)
                               for b in range(host.shape[0])]).to(self.device)
         else:
-            samp = topk_sampling(logits, top_k=top_k, top_p=1.0, temperature=temperature).view(-1).contiguous()
+            samp = topk_sampling(logits, top_k=top_k, top_p=top_p, temperature=temperature).view(-1).contiguous()
         L.check(self.lib.vb_ar_push_tokens(C.byref(head), C.byref(buf.st), samp.data_ptr(), self.d,
                                            L.stream_ptr()), "vb_ar_push_tokens")
 

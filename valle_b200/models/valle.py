@@ -211,11 +211,14 @@ class VALLE(nn.Module):
     @torch.no_grad()
     def inference(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor,
                   enroll_x_lens: Optional[torch.Tensor] = None, top_k: int = -100,
-                  temperature: float = 1.0, max_new_tokens: Optional[int] = None, seed: Optional[int] = None) -> torch.Tensor:
+                  temperature: float = 1.0, max_new_tokens: Optional[int] = None, seed: Optional[int] = None,
+                  top_p: float = 1.0, ras=None) -> torch.Tensor:
         """x: (1, S) phoneme ids, x_lens: (1,), y: (1, T, 8) acoustic prompt.
         Returns the predicted audio code matrix (1, T', 8) -- same contract as the reference.
         seed: None samples with torch's generator as the reference does; an int in [0, 2**64) draws with the seeded
-        device sampler inside the CUDA-graph decode step (ValleEngine.generate), reproducible from the seed alone."""
+        device sampler inside the CUDA-graph decode step (ValleEngine.generate), reproducible from the seed alone.
+        top_p: nucleus filtering after top-k, in (0, 1]; ras: repetition-aware sampling, a (window, threshold) pair
+        (needs seed); see ValleEngine.generate."""
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
@@ -225,7 +228,7 @@ class VALLE(nn.Module):
         enroll = [int(enroll_x_lens.max())] if (self.prefix_mode in (2, 4) and enroll_x_lens is not None) else None
         out = self.engine().generate([x[0, :S]], [y[0]], enroll_lens=enroll, top_k=top_k,
                                      temperature=temperature, max_new_tokens=max_new_tokens,
-                                     return_device=True, seed=seed)
+                                     return_device=True, seed=seed, top_p=top_p, ras=ras)
         return out[0].unsqueeze(0).to(y.device)
 
     @torch.no_grad()
@@ -233,21 +236,22 @@ class VALLE(nn.Module):
                         enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1,
                         temperature: float = 1.0, max_new_tokens=None,
                         dtype: Optional[torch.dtype] = None, return_device: bool = False,
-                        seed=None) -> List[torch.Tensor]:
+                        seed=None, top_p=1.0, ras=None) -> List[torch.Tensor]:
         """Engine feature (the reference asserts batch 1, valle.py:989): B independent utterances
         decoded together; result[b] equals `inference()` on utterance b alone.  Codes come back on the host, or
         (return_device=True) stay on the GPU, e.g. for the data-parallel gather of valle_b200.dist.
         Sampling (top_k != 1) keeps that promise with `seed` (an int s, or B ints): utterance b then equals
-        `inference(..., seed=s + b)`; top_k and temperature may be per-utterance sequences.  max_new_tokens: one int
-        or one per utterance."""
+        `inference(..., seed=s + b)`; top_k, temperature and top_p may be per-utterance sequences, and ras one
+        (window, threshold) pair or one per utterance (ValleEngine.generate).  max_new_tokens: one int or one per
+        utterance."""
         return self.engine(dtype).generate(texts, prompts, enroll_lens=enroll_lens, top_k=top_k,
                                            temperature=temperature, max_new_tokens=max_new_tokens,
-                                           return_device=return_device, seed=seed)
+                                           return_device=return_device, seed=seed, top_p=top_p, ras=ras)
 
     def inference_stream(self, requests, slots: Optional[int] = None, max_context: Optional[int] = None,
                          poll: int = 32, nar_batch: Optional[int] = None, dtype: Optional[torch.dtype] = None):
         """Engine feature: continuous batching (ValleEngine.generate_stream).  requests: StreamRequest records
-        (text, prompt, enroll_len, seed, top_k, temperature, max_new_tokens), a sequence or a lazy iterator; yields
+        (text, prompt, enroll_len, seed, top_k, temperature, max_new_tokens, top_p, ras), a sequence or a lazy iterator; yields
         (index, codes [Tgen, 8] on the GPU) as each utterance completes, codes equal to `inference()` of that request
         alone.  Decodes in `engine_dtype` (or `dtype`) with the model's `kv_cache_dtype`."""
         return self.engine(dtype).generate_stream(requests, slots=slots, max_context=max_context, poll=poll,

@@ -224,10 +224,13 @@ def cross_entropy_rows(logits: torch.Tensor, targets: torch.Tensor, ignore_index
 
 
 @_dev_guard
-def sample_logits(logits: torch.Tensor, top_k, temperature, seeds, steps) -> torch.Tensor:
+def sample_logits(logits: torch.Tensor, top_k, temperature, seeds, steps, top_p=None, ras_window=None, ras_max=None,
+                  tokens: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Seeded top-k / temperature draw per row of fp32 logits [R, V] (V <= 1280; a row stride of 0, e.g. from
     `expand`, draws R times from one row), vb_sample_logits: top_k / temperature / seeds / steps are one value or one
-    per row; seeds are uint64 values (int64 bit patterns accepted).  Returns int64 ids [R]."""
+    per row; seeds are uint64 values (int64 bit patterns accepted).  Returns int64 ids [R].
+    top_p, ras_window / ras_max (one value or one per row) and tokens (int32 [R, >= max step] history, row stride
+    free) select vb_sample_logits_ex: nucleus filtering and repetition-aware sampling."""
     _req_cuda(logits)
     assert logits.dtype == torch.float32 and logits.dim() == 2 and logits.stride(1) == 1
     R, V = logits.shape
@@ -243,6 +246,20 @@ def sample_logits(logits: torch.Tensor, top_k, temperature, seeds, steps) -> tor
     sd, st = rows(seeds, torch.int64), rows(steps, torch.int32)
     k, t = rows(top_k, torch.int32), rows(temperature, torch.float32)
     out = torch.empty(R, dtype=torch.int64, device=dev)
+    if top_p is not None or ras_window is not None:
+        p = rows(top_p, torch.float32) if top_p is not None else None
+        rw = rm = None
+        tok_ld = 0
+        if ras_window is not None:
+            rw, rm = rows(ras_window, torch.int32), rows(ras_max, torch.int32)
+            assert tokens is not None and tokens.dtype == torch.int32 and tokens.dim() == 2 and tokens.stride(1) == 1
+            tokens = tokens.to(dev)
+            tok_ld = tokens.stride(0)
+        L.check(L.load().vb_sample_logits_ex(logits.data_ptr(), logits.stride(0), R, V, sd.data_ptr(), st.data_ptr(),
+                                             k.data_ptr(), t.data_ptr(), L.ptr(p), L.ptr(rw), L.ptr(rm),
+                                             L.ptr(tokens if rw is not None else None), tok_ld, out.data_ptr(),
+                                             _stream()), "vb_sample_logits_ex")
+        return out
     L.check(L.load().vb_sample_logits(logits.data_ptr(), logits.stride(0), R, V, sd.data_ptr(), st.data_ptr(),
                                       k.data_ptr(), t.data_ptr(), out.data_ptr(), _stream()), "vb_sample_logits")
     return out
