@@ -1,8 +1,13 @@
 """Host-side logic of the batched engine that needs no GPU: the packed index maps (rows / positions of the
-text and audio segments of every utterance) that generate() / _nar() ship to the device in one copy."""
-import numpy as np
+text and audio segments of every utterance) that generate() / _nar() ship to the device in one copy, the validated
+per-utterance draws of the seeded sampler, and the checks of an utterance's inputs."""
+import math
 
-from valle_b200.engine import _seg_ranges
+import numpy as np
+import pytest
+import torch
+
+from valle_b200.engine import _check_utt, _draws, _seg_ranges
 
 
 def _naive(starts, lens):
@@ -34,6 +39,83 @@ def test_seg_ranges_empty_and_packed_layout():
     assert trow.tolist() == [0, 1, 2, 7, 8] and tpos.tolist() == [0, 1, 2, 0, 1]
     assert arow.tolist() == [3, 4, 5, 6, 9] and apos.tolist() == [0, 1, 2, 3, 0]
     assert sorted(trow.tolist() + arow.tolist()) == list(range(int(cu[-1])))
+
+
+def test_draws_expand_one_seed_and_keep_per_utterance_values():
+    d = _draws(3, 5, 8, 0.7, 0.9)
+    assert [x.seed for x in d] == [5, 6, 7]   # utterance b draws from s + b, as it would alone with seed s + b
+    assert {(x.top_k, x.temperature, x.top_p, x.ras_window, x.ras_max) for x in d} == {(8, 0.7, 0.9, 0, 0)}
+    d = _draws(3, [9, 0, 2 ** 64 - 1], [1, 5, 1], [1.0, 0.8, 1.3], [1.0, 0.5, 0.95], [None, (4, 0.3), None])
+    assert [x.seed for x in d] == [9, 0, 2 ** 64 - 1] and [x.top_k for x in d] == [1, 5, 1]
+    assert [x.temperature for x in d] == [1.0, 0.8, 1.3] and [x.top_p for x in d] == [1.0, 0.5, 0.95]
+    assert [(x.ras_window, x.ras_max) for x in d] == [(0, 0), (4, 1), (0, 0)]
+    t = torch.tensor([3, 4])
+    assert [x.seed for x in _draws(2, t, t, 1.0)] == [3, 4]   # tensors of values, one per utterance
+
+
+def test_draw_seeds_map_to_their_int64_bit_patterns():
+    for s in (0, 1, 2 ** 63 - 1, 2 ** 63, 2 ** 63 + 5, 2 ** 64 - 1):
+        d = _draws(1, s, 5, 1.0)[0]
+        assert d.seed == s
+        want = int(np.array([s], dtype=np.uint64).view(np.int64)[0])
+        assert d.seed_i64 == want and -2 ** 63 <= d.seed_i64 < 2 ** 63
+    assert _draws(1, 2 ** 63, 5, 1.0)[0].seed_i64 == -2 ** 63
+    assert _draws(1, 2 ** 64 - 1, 5, 1.0)[0].seed_i64 == -1
+
+
+def test_draw_ras_max_is_the_python_count_test():
+    for (w, t), want in (((100, 0.29), 29), ((3, 1 / 3), 1), ((7, 0.5), 3), ((10, 0.0), 0)):
+        assert _draws(1, 0, 5, 1.0, ras=(w, t))[0].ras_max == want, (w, t)
+    for w in (1, 2, 3, 7, 10, 64, 100, 256):   # count > ras_max exactly when count / K > t
+        for t in (0.0, 0.1, 0.29, 1 / 3, 0.5, 0.7, 0.999):
+            d = _draws(1, 0, 5, 1.0, ras=(w, t))[0]
+            assert d.ras_window == w
+            assert all((c > d.ras_max) == (c / w > t) for c in range(w + 1)), (w, t)
+
+
+def test_draw_greedy_is_top_k_1_without_ras():
+    assert _draws(1, 0, 1, 0.5, 0.3)[0].greedy
+    assert not _draws(1, 0, 1, 1.0, ras=(8, 0.1))[0].greedy
+    assert not _draws(1, 0, 5, 1.0)[0].greedy
+    assert not _draws(1, 0, -100, 1.0)[0].greedy
+    assert [x.greedy for x in _draws(2, 0, [1, 1], 1.0, ras=[None, (4, 0.5)])] == [True, False]
+
+
+@pytest.mark.parametrize("kw, match", [
+    (dict(seed=-1), "seed"), (dict(seed=2 ** 64), "seed"), (dict(seed=2 ** 64 - 2), "seed"),
+    (dict(seed=[1, 2]), "seed"), (dict(top_k=[5, 5]), "top_k"),
+    (dict(temperature=0.0), "temperature"), (dict(temperature=-1.0), "temperature"),
+    (dict(temperature=math.inf), "temperature"), (dict(temperature=math.nan), "temperature"),
+    (dict(temperature=[1.0, 1.0, 0.5]), "temperature"),
+    (dict(top_p=0.0), "top_p"), (dict(top_p=1.01), "top_p"), (dict(top_p=-1.0), "top_p"),
+    (dict(top_p=math.nan), "top_p"), (dict(top_p=[0.5, 0.5, 0.5, 2.0]), "top_p"),
+    (dict(ras=(0, 0.1)), "window"), (dict(ras=(257, 0.1)), "window"), (dict(ras=(8.0, 0.1)), "window"),
+    (dict(ras=(True, 0.1)), "window"), (dict(ras=(8, 1.0)), "threshold"), (dict(ras=(8, -0.1)), "threshold"),
+    (dict(ras=(8, math.nan)), "threshold"), (dict(ras=[(8, 0.1)] * 3), "ras"), (dict(ras=(8, 0.1, 2)), "pair"),
+])
+def test_draw_argument_errors(kw, match):
+    args = dict(seed=1, top_k=5, temperature=1.0, top_p=1.0, ras=None)
+    args.update(kw)
+    with pytest.raises(ValueError, match=match):
+        _draws(2 if "ras" in kw else 4, **args)
+
+
+def test_utterance_checks():
+    text, prompt = torch.tensor([3, 4, 5]), torch.zeros((6, 8), dtype=torch.int64)
+    _check_utt("utterance 0", text, prompt, 8)
+    for t, p in ((text[None], prompt), (text[:0], prompt), (text, prompt[:, :7]), (text, prompt[0])):
+        with pytest.raises(ValueError, match="utterance 0"):
+            _check_utt("utterance 0", t, p, 8)
+    bad_first = prompt.clone()
+    bad_first[2, 0] = 1025
+    bad_rest = prompt.clone()
+    bad_rest[2, 3] = 1024
+    for t, p, what in ((torch.tensor([3, 512]), prompt, "phoneme"), (torch.tensor([-1]), prompt, "phoneme"),
+                       (text, bad_first, "first codebook"), (text, bad_rest, "prompt code id 1024")):
+        with pytest.raises(IndexError, match=what):
+            _check_utt("utterance 0", t, p, 8)
+    prompt[:, 0] = 1024                       # <BOS> row of the first codebook's tables
+    _check_utt("utterance 0", text, prompt, 8)
 
 
 def test_layernorm_fold_identity_of_the_decode_chain():

@@ -16,7 +16,7 @@ from conftest import load_golden
 from test_sampling_gpu import _batch, _model, _rows
 from test_stream_gpu import _check_equal, _requests, _stream, tuned
 from test_stream_gpu import _model as _stream_model
-from valle_b200.engine import StreamRequest, _ras_arrays
+from valle_b200.engine import StreamRequest, _draws
 
 pytestmark = pytest.mark.gpu
 
@@ -165,7 +165,7 @@ def test_traced_native_decode_matches_the_restatement(chain, monkeypatch):
     eng = m.engine(dtype)
     x, y = g["x"][0], g["y"][0]
     seed, k, T, p, ras = 4242, 8, 1.0, 0.7, (6, 0.2)
-    rmax = _ras_arrays([ras])[1][0]
+    rmax = _draws(1, seed, k, T, p, ras)[0].ras_max
     tr = {"steps": "all"}
     out = eng.generate([x], [y], top_k=k, temperature=T, top_p=p, ras=ras, trace=tr, seed=seed)[0].cpu()
     n = out.shape[0]

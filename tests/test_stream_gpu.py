@@ -14,7 +14,7 @@ import torch
 from conftest import build_model, load_golden
 from test_post_ln import postln_model
 from valle_b200 import _lib as L
-from valle_b200.engine import StreamRequest, _ArBuffers
+from valle_b200.engine import StreamRequest, _ArBuffers, _draws
 
 pytestmark = pytest.mark.gpu
 
@@ -175,14 +175,9 @@ def _rand_utts(n, seed, S=(4, 12), Tp=(8, 30)):
     return out
 
 
-def _set_rows(buf, p, idx, greedy, seeds):
-    buf.text_len.index_copy_(0, idx, p.S_d)
-    buf.prompt_len.index_copy_(0, idx, p.Tp_d)
-    buf.max_new.index_copy_(0, idx, p.capn_d)
-    if greedy == 2:
-        buf.sample_seed.index_copy_(0, idx, torch.tensor(seeds, dtype=torch.int64, device=DEV))
-        buf.top_k.index_copy_(0, idx, torch.tensor([7 + i for i in range(len(seeds))], dtype=torch.int32, device=DEV))
-        buf.temperature.index_copy_(0, idx, torch.tensor([0.9] * len(seeds), dtype=torch.float32, device=DEV))
+def _seeded(greedy, seeds):
+    """the draws of the seeded head (greedy == 2): top_k 7, 8, ... and temperature 0.9"""
+    return _draws(len(seeds), seeds, [7 + i for i in range(len(seeds))], 0.9) if greedy == 2 else None
 
 
 STATE = ["n_gen", "finished", "tokens", "x_cur", "logits", "kcache", "vcache"]
@@ -205,7 +200,7 @@ def test_admit_rows_into_running_state(lib, chain, greedy, monkeypatch):
     old, new = _rand_utts(8, 1), _rand_utts(3, 2)
     buf = _ArBuffers(eng, 8, cap, ts)
     p = eng._prefill_inputs([u[0] for u in old], [u[1] for u in old], [100] * 8)
-    _set_rows(buf, p, torch.arange(8, device=DEV), greedy, list(range(8)))
+    buf.load_rows(p, _seeded(greedy, list(range(8))))
     h = eng._prefill(buf, p, pe_a)
     L.check(lib.vb_ar_head_step(eng.ar.handle, C.byref(head), h.data_ptr(), C.byref(buf.st), buf.ws.data_ptr(),
                                 buf.ws.numel(), L.stream_ptr()))
@@ -217,7 +212,7 @@ def test_admit_rows_into_running_state(lib, chain, greedy, monkeypatch):
     slots = [5, 0, 3]
     sl = torch.tensor(slots, dtype=torch.int32, device=DEV)
     pn = eng._prefill_inputs([u[0] for u in new], [u[1] for u in new], [100] * 3, slots=slots)
-    _set_rows(buf, pn, sl.long(), greedy, [50, 51, 52])
+    buf.load_rows(pn, _seeded(greedy, [50, 51, 52]))   # rows 5, 0, 3
     before = {n: getattr(buf, n).clone() for n in STATE}
     hn = eng._prefill(buf, pn, pe_a)
     ws = torch.empty(lib.vb_ar_admit_workspace(C.byref(eng.ar.desc), 3, nv), dtype=torch.uint8, device=DEV)
@@ -226,7 +221,7 @@ def test_admit_rows_into_running_state(lib, chain, greedy, monkeypatch):
     # the reference: the same 3 utterances as a fresh 3-row state
     fresh = _ArBuffers(eng, 3, cap, ts)
     pf = eng._prefill_inputs([u[0] for u in new], [u[1] for u in new], [100] * 3)
-    _set_rows(fresh, pf, torch.arange(3, device=DEV), greedy, [50, 51, 52])
+    fresh.load_rows(pf, _seeded(greedy, [50, 51, 52]))
     hf = eng._prefill(fresh, pf, pe_a)
     assert torch.equal(hf, hn)
     L.check(lib.vb_ar_head_step(eng.ar.handle, C.byref(head), hf.data_ptr(), C.byref(fresh.st), fresh.ws.data_ptr(),

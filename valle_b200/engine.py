@@ -47,10 +47,16 @@ def _on_device(fn):
     return wrapper
 
 
-def _check_ids(tensors, hi: int, what: str):
-    """nn.Embedding raises IndexError for ids outside the table (valle/modules/embedding.py:46).  Host tensors are
-    checked here before the copy; device tensors are checked by the kernels (clamped read + flag, ops.check_oob)."""
-    for t in tensors:
+def _check_utt(who: str, text: torch.Tensor, codes: torch.Tensor, Q: int, name: str = "prompt code"):
+    """One utterance's inputs: text [S > 0] phoneme ids and codes [T, Q] codec ids (the prompt, or continual()'s
+    codes); ValueError for a shape.  nn.Embedding raises IndexError for ids outside the table
+    (valle/modules/embedding.py:46): host tensors are checked here before the copy, device tensors by the kernels
+    (clamped read + flag, ops.check_oob).  The first codebook's tables have 1025 rows (+ <BOS>)."""
+    if text.ndim != 1 or text.numel() == 0 or codes.ndim != 2 or codes.shape[1] != Q:
+        raise ValueError(f"{who}: expected text ids [S > 0] and {name}s [T, {Q}]")
+    for t, hi, what in ((text, NUM_TEXT_TOKENS, "phoneme"),
+                        (codes[:, :1], NUM_AUDIO_TOKENS + 1, f"{name} (first codebook)"),
+                        (codes[:, 1:], NUM_AUDIO_TOKENS, name)):
         if not t.is_cuda and t.numel() > 0:
             lo_v, hi_v = int(t.min()), int(t.max())
             if lo_v < 0 or hi_v >= hi:
@@ -135,13 +141,74 @@ class _ArBuffers:
         self.graphs: Dict[tuple, Tuple[torch.cuda.CUDAGraph, int, L.ArHead]] = {}
         self.eng = eng
 
+    def load_rows(self, p: _Prefill, draws: Optional[Sequence[_Draw]] = None):
+        """Write the lengths and token caps of prefill block p's utterances into their rows (0..B-1, or p.slots_d)
+        and, given their draws, the sampler columns, all six from one host -> device copy"""
+        rows = None if p.slots_d is None else p.slots_d.long()
 
-class _Prefill:
-    """the device-side inputs of one packed AR prefill (ValleEngine._prefill_inputs)"""
+        def put(col, v):
+            if rows is None:
+                col[:len(p.S)].copy_(v)
+            else:
+                col.index_copy_(0, rows, v)
+        put(self.text_len, p.S_d)
+        put(self.prompt_len, p.Tp_d)
+        put(self.max_new, p.capn_d)
+        if draws is None:
+            return
+        # _Draw's fields in order; the int64 seeds first, so that every column starts aligned to its element size
+        cols = (self.sample_seed, self.top_k, self.temperature, self.top_p, self.ras_window, self.ras_max)
+        vals = zip(*(d._replace(seed=d.seed_i64) for d in draws))
+        block = torch.cat([torch.tensor(v, dtype=c.dtype).view(torch.uint8) for c, v in zip(cols, vals)])
+        block = block.to(self.text_len.device, non_blocking=True).split([len(draws) * c.element_size() for c in cols])
+        for c, v in zip(cols, block):
+            put(c, v.view(c.dtype))
+
+
+class _Utt(NamedTuple):
+    """One utterance on its way to the NAR: its index in the call, device text ids [S] and prompt codes [Tp, Q], the
+    prompt length the AR saw (Tp + 1 with <BOS>), and the enrolled phonemes the NAR text leaves out in prefix modes
+    2 / 4 (None: the whole text)"""
+    index: int
+    text: torch.Tensor
+    prompt: torch.Tensor
+    Tp_ar: int
+    enroll_len: Optional[int] = None
+
+
+class _Prefill(NamedTuple):
+    """The device-side inputs of one packed AR prefill of B utterances (ValleEngine._prefill_inputs)"""
+    S: List[int]                    # text lengths
+    Tp: List[int]                   # prompt lengths the AR sees (+1 for <BOS> with prepend_bos)
+    Tp_nar: List[int]               # prompt lengths the NAR sees
+    text_all: torch.Tensor          # int64 [sum S] phoneme ids
+    prm_all: torch.Tensor           # int64 [sum Tp_nar, Q] prompt codes
+    ar_tok: Optional[torch.Tensor]  # prepend_bos: int64 [sum Tp], <BOS> and the first codebook of every prompt
+    # int32 views of one device block: the packed layout (cu_seqlens, lengths, rows / positions of the text and
+    # prompt rows, the last row of every utterance), the token caps and the decode slots (None: rows 0..B-1)
+    cu_d: torch.Tensor
+    S_d: torch.Tensor
+    Tp_d: torch.Tensor
+    capn_d: torch.Tensor
+    trow_d: torch.Tensor
+    tpos_d: torch.Tensor
+    arow_d: torch.Tensor
+    apos_d: torch.Tensor
+    last_d: torch.Tensor
+    slots_d: Optional[torch.Tensor]
+
+    def utts(self, index: Sequence[int], enroll_lens: Sequence[Optional[int]]) -> List[_Utt]:
+        return [_Utt(i, t, pr, tp, None if e is None else int(e)) for i, t, pr, tp, e in
+                zip(index, self.text_all.split(self.S), self.prm_all.split(self.Tp_nar), self.Tp, enroll_lens)]
 
 
 def _is_seq(v) -> bool:
     return isinstance(v, (list, tuple)) or (isinstance(v, (torch.Tensor, np.ndarray)) and v.ndim > 0)
+
+
+def _offsets(lens) -> np.ndarray:
+    """[0, l0, l0 + l1, ..., sum]: where each ragged segment starts, then the total (int64)"""
+    return np.concatenate([[0], np.cumsum(lens, dtype=np.int64)]).astype(np.int64)
 
 
 def _check_top_p(ps):
@@ -149,36 +216,32 @@ def _check_top_p(ps):
         raise ValueError("top_p must lie in (0, 1]")
 
 
-def _ras_rows(B: int, ras) -> List[Optional[Tuple[int, float]]]:
-    """Validated per-utterance repetition-aware sampling settings: None (off), one (window, threshold) pair for every
-    utterance, or a sequence of B pairs / Nones.  window: an int in [1, 256]; threshold in [0, 1)."""
-    if ras is None:
-        return [None] * B
-    per = _is_seq(ras) and len(ras) > 0 and (ras[0] is None or _is_seq(ras[0]))
-    rows = list(ras) if per else [ras] * B
-    if len(rows) != B:
-        raise ValueError(f"ras: {len(rows)} values for {B} utterances")
-    out = []
-    for r in rows:
-        if r is None:
-            out.append(None)
-            continue
-        if not _is_seq(r) or len(r) != 2:
-            raise ValueError(f"ras: expected a (window, threshold) pair, got {r!r}")
-        w, t = r
-        if isinstance(w, bool) or not isinstance(w, (int, np.integer)) or not 1 <= int(w) <= 256:
-            raise ValueError(f"ras: the window must be an int in [1, 256] (got {w!r})")
-        t = float(t)
-        if not 0.0 <= t < 1.0:
-            raise ValueError(f"ras: the threshold must lie in [0, 1) (got {t!r})")
-        out.append((int(w), t))
-    return out
+class _Draw(NamedTuple):
+    """One utterance's seeded device draw, the sampler columns of vb_ar_state: top-k, temperature and top-p, then
+    repetition-aware sampling over the last ras_window codes (0: off), which draws again when the draw occurs there
+    more than ras_max times"""
+    seed: int
+    top_k: int
+    temperature: float
+    top_p: float
+    ras_window: int
+    ras_max: int
+
+    @property
+    def greedy(self) -> bool:
+        """argmax: the seed draws nothing"""
+        return self.top_k == 1 and self.ras_window == 0
+
+    @property
+    def seed_i64(self) -> int:
+        """the uint64 seed as the int64 bit pattern the device column holds"""
+        return self.seed - (1 << 64) if self.seed >= 1 << 63 else self.seed
 
 
 def _ras_arrays(rows) -> Tuple[List[int], List[int]]:
-    """(ras_window, ras_max) of vb_ar_state per utterance: ras_max = floor(t K), the largest count c with c / K <= t, so
-    that the device's integer test count > ras_max is exactly count / K > t as Python evaluates it (t K rounded to a
-    double can land just below an integer: 0.29 * 100 = 28.999...)"""
+    """(ras_window, ras_max) of validated (window K, threshold t) pairs / Nones (off): ras_max = floor(t K), the largest
+    count c with c / K <= t, so that the device's integer test count > ras_max is exactly count / K > t as Python
+    evaluates it (t K rounded to a double can land just below an integer: 0.29 * 100 = 28.999...)"""
     def ras_max(K, t):
         c = math.floor(t * K)
         while (c + 1) / K <= t:
@@ -189,10 +252,12 @@ def _ras_arrays(rows) -> Tuple[List[int], List[int]]:
     return [0 if r is None else r[0] for r in rows], [0 if r is None else ras_max(*r) for r in rows]
 
 
-def _sampler_args(B: int, seed, top_k, temperature, top_p=1.0, ras=None):
-    """Validated per-utterance (seeds, top_k, temperature, top_p, ras) lists of a seeded call: an int seed s stands for
-    s, s+1, ..., s+B-1 (so utterance b decoded alone with seed s+b draws what it draws in the batch); top_k /
-    temperature / top_p are one value or a sequence of B; ras as _ras_rows takes it."""
+def _draws(B: int, seed, top_k, temperature, top_p=1.0, ras=None) -> List[_Draw]:
+    """Validated draws of the B utterances of a seeded call.  An int seed s stands for s, s+1, ..., s+B-1 (so utterance
+    b decoded alone with seed s+b draws what it draws in the batch), or B seeds, each in [0, 2**64); top_k /
+    temperature / top_p: one value or a sequence of B; ras (repetition-aware sampling): None (off), one (window,
+    threshold) pair for every utterance, or a sequence of B pairs / Nones, window an int in [1, 256], threshold in
+    [0, 1)."""
     def per_row(v, what):
         if _is_seq(v):
             v = [x.item() if hasattr(x, "item") else x for x in v]
@@ -213,7 +278,22 @@ def _sampler_args(B: int, seed, top_k, temperature, top_p=1.0, ras=None):
         raise ValueError("temperature must be finite and > 0")
     ps = [float(x) for x in per_row(top_p, "top_p")]
     _check_top_p(ps)
-    return seeds, ks, ts, ps, _ras_rows(B, ras)
+    per = _is_seq(ras) and len(ras) > 0 and (ras[0] is None or _is_seq(ras[0]))
+    rr = list(ras) if per else [ras] * B
+    if len(rr) != B:
+        raise ValueError(f"ras: {len(rr)} values for {B} utterances")
+    for i, r in enumerate(rr):
+        if r is not None:
+            if not _is_seq(r) or len(r) != 2:
+                raise ValueError(f"ras: expected a (window, threshold) pair, got {r!r}")
+            w, t = r
+            if isinstance(w, bool) or not isinstance(w, (int, np.integer)) or not 1 <= int(w) <= 256:
+                raise ValueError(f"ras: the window must be an int in [1, 256] (got {w!r})")
+            t = float(t)
+            if not 0.0 <= t < 1.0:
+                raise ValueError(f"ras: the threshold must lie in [0, 1) (got {t!r})")
+            rr[i] = (int(w), t)
+    return [_Draw(*v) for v in zip(seeds, ks, ts, ps, *_ras_arrays(rr))]
 
 
 def _seg_ranges(starts, lens):
@@ -341,8 +421,7 @@ class ValleEngine:
         utterance is convolved on its own with zero padding, as the reference's batch-1 call does (valle.py:995-996)"""
         convs, (wl, bl) = self.pre[which]
         R, d = x.shape
-        starts = np.cumsum([0] + list(S[:-1]), dtype=np.int64)
-        base, pos = _seg_ranges(starts, S)                   # row index, position inside its utterance
+        base, pos = _seg_ranges(_offsets(S)[:-1], S)         # row index, position inside its utterance
         lens = np.repeat(np.asarray(S, dtype=np.int64), S)
         idx = np.stack([np.where((pos + k - 2 >= 0) & (pos + k - 2 < lens), base + k - 2, -1) for k in range(5)])
         idx_d = torch.from_numpy(idx.astype(np.int32)).to(self.device)
@@ -425,19 +504,18 @@ class ValleEngine:
         teacher-forced with (every sampled id is replaced by the given one before it is appended, AR and NAR), so
         that per-step logits can be compared with a reference that took exactly those ids."""
         self._refresh()
-        m, dev, d, Q = self.model, self.device, self.d, self.Q
         B = len(texts)
-        assert B == len(prompts) and B >= 1
-        kv_dtype = self.kv_cache_dtype()
-        sampler = None
+        if B < 1 or len(prompts) != B:
+            raise ValueError(f"generate: {B} texts and {len(prompts)} prompts (one of each per utterance, >= 1)")
+        draws = None
         if ras is not None and self.sample_on_host:
             raise ValueError("ras draws on the device; it cannot be combined with sample_on_host = True")
         if seed is not None:
             if self.sample_on_host:
                 raise ValueError("seed= selects the device sampler; it cannot be combined with sample_on_host = True")
-            sampler = _sampler_args(B, seed, top_k, temperature, top_p, ras)
-            if all(k == 1 for k in sampler[1]) and all(r is None for r in sampler[4]):
-                sampler, top_k = None, 1          # greedy: the seed draws nothing
+            draws = _draws(B, seed, top_k, temperature, top_p, ras)
+            if all(dr.greedy for dr in draws):
+                draws, top_k = None, 1          # greedy: the seed draws nothing
         elif ras is not None:
             raise ValueError("ras needs seed= (the seeded device sampler)")
         elif _is_seq(top_k) or _is_seq(temperature) or _is_seq(top_p):
@@ -445,42 +523,49 @@ class ValleEngine:
         else:
             top_p = float(top_p)
             _check_top_p([top_p])
-        if B > self.max_tc_batch and self.dtype == torch.bfloat16 and trace is None and forced is None:
-            # the tensor-core decode projections take up to 64 rows (one UMMA N tile): a larger batch is decoded as
-            # consecutive groups of <= 64 utterances instead of falling onto the CUDA-core GEMV path
-            outs: List[torch.Tensor] = []
-            stats = EngineStats()
-            packed = []
-            for b0 in range(0, B, self.max_tc_batch):
-                b1 = min(B, b0 + self.max_tc_batch)
-                if sampler is None:
-                    kw = dict(top_k=top_k, temperature=temperature, top_p=top_p)
-                else:   # by absolute utterance index
-                    kw = dict(seed=sampler[0][b0:b1], top_k=sampler[1][b0:b1], temperature=sampler[2][b0:b1],
-                              top_p=sampler[3][b0:b1], ras=sampler[4][b0:b1])
-                mnt = max_new_tokens[b0:b1] if _is_seq(max_new_tokens) else max_new_tokens
-                outs += self.generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
-                                      max_new_tokens=mnt, poll=poll, return_device=return_device, **kw)
-                stats.ar_steps += self.stats.ar_steps
-                stats.ar_ms += self.stats.ar_ms
-                stats.prefill_ms += self.stats.prefill_ms
-                stats.nar_ms += self.stats.nar_ms
-                packed.append(self.last_packed)
-            self.stats = stats
-            self.last_packed = torch.cat(packed) if return_device else None
-            return outs
+        if not (B > self.max_tc_batch and self.dtype == torch.bfloat16 and trace is None and forced is None):
+            return self._generate(texts, prompts, enroll_lens, draws, top_k, temperature, top_p, max_new_tokens, poll,
+                                  return_device, trace, forced)
+        # the tensor-core decode projections take up to 64 rows (one UMMA N tile): a larger batch is decoded as
+        # consecutive groups of <= 64 utterances instead of falling onto the CUDA-core GEMV path
+        outs: List[torch.Tensor] = []
+        stats = EngineStats()
+        packed = []
+        for b0 in range(0, B, self.max_tc_batch):
+            b1 = min(B, b0 + self.max_tc_batch)
+            mnt = max_new_tokens[b0:b1] if _is_seq(max_new_tokens) else max_new_tokens
+            outs += self._generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
+                                   None if draws is None else draws[b0:b1], top_k, temperature, top_p, mnt, poll,
+                                   return_device)
+            stats.ar_steps += self.stats.ar_steps
+            stats.ar_ms += self.stats.ar_ms
+            stats.prefill_ms += self.stats.prefill_ms
+            stats.nar_ms += self.stats.nar_ms
+            packed.append(self.last_packed)
+        self.stats = stats
+        self.last_packed = torch.cat(packed) if return_device else None
+        return outs
+
+    def _generate(self, texts, prompts, enroll_lens, draws: Optional[List[_Draw]], top_k, temperature, top_p,
+                  max_new_tokens, poll: int, return_device: bool, trace: Optional[dict] = None,
+                  forced: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+        """generate() of one group of utterances with validated sampler arguments: draws (the seeded device sampler), or
+        None and top_k / temperature / top_p (greedy, or torch's sampler)"""
+        m, dev, Q = self.model, self.device, self.Q
+        B = len(texts)
+        kv_dtype = self.kv_cache_dtype()
+        for b in range(B):
+            _check_utt(f"utterance {b}", texts[b], prompts[b], Q)
+        if self.prefix_mode in (2, 4) and Q > 1 and enroll_lens is None:
+            raise ValueError(f"prefix_mode {self.prefix_mode} needs enroll_lens (the NAR text leaves them out)")
         S = [int(t.numel()) for t in texts]
         Tp = [int(p.shape[0]) for p in prompts]
-        assert all(s > 0 for s in S) and all(p.shape[1] == Q for p in prompts)
-        _check_ids(texts, NUM_TEXT_TOKENS, "phoneme")
-        _check_ids([p[:, :1] for p in prompts], NUM_AUDIO_TOKENS + 1, "prompt code (first codebook)")  # 1025-row tables
-        _check_ids([p[:, 1:] for p in prompts], NUM_AUDIO_TOKENS, "prompt code")
         cap_new = self._cap_new(S, max_new_tokens)
         tok_stride = (max(cap_new) + 2 + 7) // 8 * 8
         cap = (max(S[b] + Tp[b] + cap_new[b] + 2 for b in range(B)) + 63) // 64 * 64
-        greedy = sampler is None and top_k == 1 and forced is None
+        greedy = draws is None and top_k == 1 and forced is None
         # seeded draw in the decode step's tail (forced ids replace every draw: that runs the push path below)
-        native = sampler is not None and forced is None
+        native = draws is not None and forced is None
         forced_steps = None
         if forced is not None:  # [steps, B] first-codebook ids, EOS once an utterance's forced ids run out
             n_f = max(int(f.shape[0]) for f in forced) + 1
@@ -492,27 +577,16 @@ class ValleEngine:
 
         # ---- host -> device (once per batch) ----
         p = self._prefill_inputs(texts, prompts, cap_new)
-        Tp_nar, Tp, text_all, prm_all = p.Tp_nar, p.Tp, p.text_all, p.prm_all
+        utts = p.utts(range(B), [None] * B if enroll_lens is None else enroll_lens)
 
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         ev[0].record()
         # ---- AR prefill (valle.py:995-997,1013-1016) ----
         buf = self._buffers(B, cap, tok_stride, kv_dtype)
-        buf.text_len.copy_(p.S_d)
-        buf.prompt_len.copy_(p.Tp_d)
-        buf.max_new.copy_(p.capn_d)
+        buf.load_rows(p, draws if native else None)
         buf.n_gen.zero_()
         buf.finished.zero_()
-        if native:
-            seeds, ks, ts, ps, rr = sampler
-            buf.sample_seed.copy_(torch.tensor([x - (1 << 64) if x >= 1 << 63 else x for x in seeds], dtype=torch.int64))
-            buf.top_k.copy_(torch.tensor(ks, dtype=torch.int32))
-            buf.temperature.copy_(torch.tensor(ts, dtype=torch.float32))
-            buf.top_p.copy_(torch.tensor(ps, dtype=torch.float32))
-            rw, rm = _ras_arrays(rr)
-            buf.ras_window.copy_(torch.tensor(rw, dtype=torch.int32))
-            buf.ras_max.copy_(torch.tensor(rm, dtype=torch.int32))
-        pe_a = self._pe(m.ar_audio_position, max(Tp) + max(cap_new) + 2)
+        pe_a = self._pe(m.ar_audio_position, max(p.Tp) + max(cap_new) + 2)
         h_last = self._prefill(buf, p, pe_a)
         head = self._head(pe_a, 2 if native else int(greedy))
         self._head_ref = head
@@ -535,48 +609,38 @@ class ValleEngine:
         ev[1].record()
 
         # ---- AR decode loop (valle.py:1012-1057) ----
-        max_steps = max(cap_new) + 1
+        max_steps = max(cap_new) + 1     # the stop rule has fired in every row by then
         steps = 0
-        while steps < max_steps:
+        running = dict(enumerate(utts))
+        Tg = [0] * B
+        while running and steps < max_steps:
             n = min(poll, max_steps - steps)
             if (greedy or native) and self.use_cuda_graph:
                 self._device_steps(buf, head, n)
             else:
                 for _ in range(n):
-                    fs = None
-                    if forced_steps is not None:
-                        fs = forced_steps[min(steps + 1, forced_steps.shape[0] - 1)]
-                    self._decode_step(buf, head, greedy or native, top_k, temperature, fs, top_p)
+                    self._launch_step(buf, head)
+                    if not (greedy or native):   # draw on the host, or take the forced ids
+                        fs = None
+                        if forced_steps is not None:
+                            fs = forced_steps[min(steps + 1, forced_steps.shape[0] - 1)]
+                        self._sample_push(buf, head, top_k, temperature, fs, top_p)
             steps += n
             if trace is not None and want(steps):  # poll == 1 here: the logits row of iteration `steps`
                 trace["ar_logits"][steps] = buf.logits[:, : self.n_vocab].clone()
-            if bool((buf.finished != 0).all()):  # one D2H sync per `poll` steps
-                break
+            for b, n_b in self._stopped(buf, running).items():
+                Tg[b] = n_b
+                del running[b]
         self.stats.ar_steps = steps
         ev[2].record()
-        n_gen = buf.n_gen.cpu().tolist()
-        fin = buf.finished.cpu().tolist()
-        if any(f == 2 for f in fin):
-            raise SyntaxError("well trained model shouldn't reach here.")  # valle.py:1049-1052
-        if not self.quiet:
-            for b in range(B):
-                print(f"VALL-E EOS [{Tp_nar[b]} -> {Tp[b] + n_gen[b]}]")  # valle.py:1054
 
         # ---- NAR (valle.py:1059-1137) ----
-        Tg = n_gen
-        cu_g = [0]
-        for n in Tg:
-            cu_g.append(cu_g[-1] + n)
-        G = cu_g[-1]
-        codes = torch.empty((G, Q), dtype=torch.int64, device=dev)
         src = torch.from_numpy(_seg_ranges(np.arange(B, dtype=np.int64) * tok_stride, Tg)[0]).to(dev)
-        codes[:, 0] = buf.tokens.view(-1).index_select(0, src).to(torch.int64)
-        if Q > 1:
-            fc = None
-            if forced is not None:
-                fc = torch.cat([forced[b][: Tg[b]].to(torch.int64) for b in range(B)]).to(dev)
-            self._nar(texts, text_all, prm_all, S, Tp_nar, Tg, cu_g, codes, enroll_lens, forced_codes=fc,
-                      trace=trace if (trace is not None and trace.get("nar")) else None)
+        fc = None
+        if forced is not None:
+            fc = torch.cat([forced[b][: Tg[b]].to(torch.int64) for b in range(B)]).to(dev)
+        codes, cu_g = self._nar(utts, Tg, buf.tokens.view(-1).index_select(0, src).to(torch.int64), forced_codes=fc,
+                                trace=trace if (trace is not None and trace.get("nar")) else None)
         ev[3].record()
         ev[3].synchronize()
         if any(t.is_cuda for t in list(texts) + list(prompts)):
@@ -656,25 +720,20 @@ class ValleEngine:
         with torch.cuda.device(dev):
             buf = self._buffers(n_slots, cap, tok_stride, kv_dtype)
             buf.n_gen.zero_()
-            buf.finished.fill_(1)              # a slot that is never filled never runs
+            buf.finished.fill_(1)              # a slot that is never filled never runs, nor reads its sampler columns
             buf.x_cur.zero_()
-            buf.sample_seed.zero_()
-            buf.top_k.fill_(1)
-            buf.temperature.fill_(1.0)
-            buf.top_p.fill_(1.0)
-            buf.ras_window.zero_()
-            buf.ras_max.zero_()
             pe_a = self._pe(m.ar_audio_position, cap + 2)
             heads = {g: self._head(pe_a, g) for g in (1, 2)}
             ws = torch.empty(self.lib.vb_ar_admit_workspace(C.byref(self.ar.desc), n_slots, self.n_vocab),
                              dtype=torch.uint8, device=dev)
         mode = 1                               # 2 (the seeded sampler) from the first seeded request on
         free = list(range(n_slots))
-        active: Dict[int, tuple] = {}          # slot -> (index, S, Tp prompt, Tp AR, text ids, prompt ids, enroll_len)
-        pending: list = []                     # finished utterances waiting for the NAR
+        active: Dict[int, _Utt] = {}           # slot -> the utterance decoding in it
+        pending: List[Tuple[_Utt, torch.Tensor]] = []   # finished utterances and their codes, waiting for the NAR
         n_pulled, exhausted, device_ids = 0, False, False
 
         def pull(k):
+            """up to k validated requests: (index, request, draw)"""
             nonlocal n_pulled, exhausted, mode
             out = []
             while len(out) < k and not exhausted:
@@ -685,25 +744,20 @@ class ValleEngine:
                     break
                 idx = n_pulled
                 n_pulled += 1
-                if r.text.ndim != 1 or r.text.numel() == 0 or r.prompt.ndim != 2 or r.prompt.shape[1] != Q:
-                    raise ValueError(f"request {idx}: text must be [S > 0] ids and prompt [Tp, {Q}] codes")
+                _check_utt(f"request {idx}", r.text, r.prompt, Q)
                 seed, top_k = r.seed, r.top_k
                 if seed is None:
                     if top_k != 1 or r.ras is not None:
                         raise ValueError(f"request {idx}: top_k={top_k} / ras need a seed (the seeded device sampler)")
                     seed = 0
-                seeds, ks, ts, ps, rr = _sampler_args(1, seed, top_k, r.temperature, r.top_p,
-                                                      None if r.ras is None else [r.ras])
+                draw = _draws(1, seed, top_k, r.temperature, r.top_p, None if r.ras is None else [r.ras])[0]
                 if pm in (2, 4) and r.enroll_len is None:
                     raise ValueError(f"request {idx}: prefix_mode {pm} needs enroll_len")
                 if self._context(r) > max_context:
                     raise ValueError(f"request {idx} needs {self._context(r)} KV-cache rows > max_context={max_context}")
-                _check_ids([r.text], NUM_TEXT_TOKENS, "phoneme")
-                _check_ids([r.prompt[:, :1]], NUM_AUDIO_TOKENS + 1, "prompt code (first codebook)")
-                _check_ids([r.prompt[:, 1:]], NUM_AUDIO_TOKENS, "prompt code")
-                if ks[0] != 1 or rr[0] is not None:
+                if not draw.greedy:
                     mode = 2
-                out.append((idx, r, seeds[0], ks[0], ts[0], ps[0], rr[0]))
+                out.append((idx, r, draw))
             return out
 
         def admit(new):
@@ -711,55 +765,30 @@ class ValleEngine:
             k = len(new)
             sl = free[:k]
             del free[:k]
-            texts = [r.text for _, r, *_ in new]
-            prompts = [r.prompt for _, r, *_ in new]
-            S = [int(t.numel()) for t in texts]
-            cap_new = [self._cap_new([S[i]], new[i][1].max_new_tokens)[0] for i in range(k)]
+            texts = [r.text for _, r, _ in new]
+            prompts = [r.prompt for _, r, _ in new]
+            cap_new = [self._cap_new([int(r.text.numel())], r.max_new_tokens)[0] for _, r, _ in new]
             p = self._prefill_inputs(texts, prompts, cap_new, slots=sl)
             ev = timed("prefill_ms")
-            idx_d = p.slots_d.long()
-            buf.text_len.index_copy_(0, idx_d, p.S_d)
-            buf.prompt_len.index_copy_(0, idx_d, p.Tp_d)
-            buf.max_new.index_copy_(0, idx_d, p.capn_d)
-            seeds = [x - (1 << 64) if x >= 1 << 63 else x for x in (n[2] for n in new)]
-            buf.sample_seed.index_copy_(0, idx_d, torch.tensor(seeds, dtype=torch.int64).to(dev, non_blocking=True))
-            buf.top_k.index_copy_(0, idx_d, torch.tensor([n[3] for n in new], dtype=torch.int32).to(dev, non_blocking=True))
-            buf.temperature.index_copy_(0, idx_d, torch.tensor([n[4] for n in new], dtype=torch.float32).to(
-                dev, non_blocking=True))
-            buf.top_p.index_copy_(0, idx_d, torch.tensor([n[5] for n in new], dtype=torch.float32).to(dev, non_blocking=True))
-            rw, rm = _ras_arrays([n[6] for n in new])
-            buf.ras_window.index_copy_(0, idx_d, torch.tensor(rw, dtype=torch.int32).to(dev, non_blocking=True))
-            buf.ras_max.index_copy_(0, idx_d, torch.tensor(rm, dtype=torch.int32).to(dev, non_blocking=True))
+            buf.load_rows(p, [draw for *_, draw in new])
             h = self._prefill(buf, p, pe_a)
             L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), k, p.slots_d.data_ptr(),
                                          C.byref(buf.st), ws.data_ptr(), ws.numel(), L.stream_ptr()), "vb_ar_admit")
             e = torch.cuda.Event(enable_timing=True)
             e.record()
             ev.append(e)
-            to, po = 0, 0
-            for i, (idx, r, *_) in enumerate(new):
-                active[sl[i]] = (idx, S[i], p.Tp_nar[i], p.Tp[i], p.text_all[to:to + S[i]],
-                                 p.prm_all[po:po + p.Tp_nar[i]], r.enroll_len)
-                to += S[i]
-                po += p.Tp_nar[i]
+            active.update(zip(sl, p.utts([idx for idx, *_ in new], [r.enroll_len for _, r, _ in new])))
             device_ids |= any(t.is_cuda for t in texts + prompts)
             stats.admissions += k
 
         def nar(batch):
             ev = timed("nar_ms")
-            Tg = [int(c.shape[0]) for *_, c in batch]
-            cu_g = [0]
-            for n in Tg:
-                cu_g.append(cu_g[-1] + n)
-            codes = torch.empty((cu_g[-1], Q), dtype=torch.int64, device=dev)
-            codes[:, 0] = torch.cat([c for *_, c in batch])
-            if Q > 1:
-                self._nar(None, torch.cat([b[4] for b in batch]), torch.cat([b[5] for b in batch]),
-                          [b[1] for b in batch], [b[2] for b in batch], Tg, cu_g, codes, [b[6] for b in batch])
+            codes, cu_g = self._nar([u for u, _ in batch], [int(c.shape[0]) for _, c in batch],
+                                    torch.cat([c for _, c in batch]))
             e = torch.cuda.Event(enable_timing=True)
             e.record()
             ev.append(e)
-            return [(b[0], codes[cu_g[i]:cu_g[i + 1]]) for i, b in enumerate(batch)]
+            return [(u.index, codes[cu_g[i]:cu_g[i + 1]]) for i, (u, _) in enumerate(batch)]
 
         def advance():
             """admission, `poll` decode steps and the stop flags; returns the utterances whose codes are ready"""
@@ -779,18 +808,10 @@ class ValleEngine:
                 e.record()
                 ev.append(e)
                 stats.ar_steps += poll
-                fin, n_gen = torch.stack([buf.finished, buf.n_gen]).cpu().tolist()   # one D2H sync per `poll` steps
-                for s in sorted(active):
-                    if fin[s] == 0:
-                        continue
-                    if fin[s] == 2:
-                        raise SyntaxError("well trained model shouldn't reach here.")  # valle.py:1049-1052
-                    idx, S, Tp_nar, Tp, text_d, prm_d, enroll = active.pop(s)
-                    if not self.quiet:
-                        print(f"VALL-E EOS [{Tp_nar} -> {Tp + n_gen[s]}]")  # valle.py:1054
-                    pending.append((idx, S, Tp_nar, Tp, text_d, prm_d, enroll,
-                                    buf.tokens[s, :n_gen[s]].to(torch.int64)))
-                    stats.slot_steps += n_gen[s]
+                for s, n in self._stopped(buf, active).items():
+                    # copied out now: the slot may be refilled before the NAR batch runs
+                    pending.append((active.pop(s), buf.tokens[s, :n].to(torch.int64)))
+                    stats.slot_steps += n
                     free.append(s)
                 free.sort()
             ready = []
@@ -829,7 +850,23 @@ class ValleEngine:
             cap_new = [min(c, t - 1) for c, t in zip(cap_new, mnt)]
         return cap_new
 
-    def _prefill_inputs(self, texts, prompts, cap_new, slots: Optional[Sequence[int]] = None):
+    def _stopped(self, buf: _ArBuffers, rows: Dict[int, _Utt]) -> Dict[int, int]:
+        """The stop flags and n_gen of buf in one device -> host copy (one sync): of `rows` (row -> its utterance), the
+        ones whose utterance has stopped, in row order, with their n_gen.  Prints their EOS lines (valle.py:1054);
+        an utterance that stopped before its first code raises as the reference does (valle.py:1049-1052)."""
+        fin, n_gen = torch.stack([buf.finished, buf.n_gen]).cpu().tolist()
+        out = {}
+        for s in sorted(rows):
+            if fin[s] == 0:
+                continue
+            if fin[s] == 2:
+                raise SyntaxError("well trained model shouldn't reach here.")
+            if not self.quiet:
+                print(f"VALL-E EOS [{rows[s].prompt.shape[0]} -> {rows[s].Tp_ar + n_gen[s]}]")
+            out[s] = n_gen[s]
+        return out
+
+    def _prefill_inputs(self, texts, prompts, cap_new, slots: Optional[Sequence[int]] = None) -> _Prefill:
         """the host -> device copies of one packed AR prefill (ids, and one int32 block of lengths and row maps);
         slots: the decode slots the utterances go to (generate_stream)"""
         dev, Q = self.device, self.Q
@@ -844,38 +881,22 @@ class ValleEngine:
             ar_tok = torch.cat([torch.cat([bos, p[:, 0].to(torch.int64).cpu()]) for p in prompts]).to(dev, non_blocking=True)
             Tp = [t + 1 for t in Tp]
         seq_len = [S[b] + Tp[b] for b in range(B)]
-        cu = [0]
-        for n in seq_len:
-            cu.append(cu[-1] + n)
-        cu_np = np.asarray(cu, dtype=np.int64)
+        cu_np = _offsets(seq_len)
         text_rows, text_pos = _seg_ranges(cu_np[:-1], S)
         aud_rows, aud_pos = _seg_ranges(cu_np[:-1] + np.asarray(S, dtype=np.int64), Tp)
         meta = torch.from_numpy(np.concatenate([cu_np, S, Tp, cap_new, text_rows, text_pos, aud_rows, aud_pos,
                                                 cu_np[1:] - 1, [] if slots is None else slots]).astype(np.int32)
                                 ).to(dev, non_blocking=True)
-        o = 0
-        def take(n):
-            nonlocal o
-            v = meta[o:o + n]
-            o += n
-            return v
-        p = _Prefill()
-        p.B, p.S, p.Tp, p.Tp_nar, p.M, p.max_len = B, S, Tp, Tp_nar, cu[-1], max(seq_len)
-        p.text_all, p.prm_all, p.ar_tok = text_all, prm_all, ar_tok
-        p.cu_d, p.S_d, p.Tp_d, p.capn_d = take(B + 1), take(B), take(B), take(B)
-        p.trow_d, p.tpos_d = take(sum(S)), take(sum(S))
-        p.arow_d, p.apos_d = take(sum(Tp)), take(sum(Tp))
-        p.last_d = take(B)
-        p.slots_d = take(B) if slots is not None else None
-        return p
+        v = meta.split([B + 1, B, B, B, sum(S), sum(S), sum(Tp), sum(Tp), B, 0 if slots is None else B])
+        return _Prefill(S, Tp, Tp_nar, text_all, prm_all, ar_tok, *v[:-1], None if slots is None else v[-1])
 
-    def _prefill(self, buf: _ArBuffers, p: "_Prefill", pe_a: torch.Tensor) -> torch.Tensor:
+    def _prefill(self, buf: _ArBuffers, p: _Prefill, pe_a: torch.Tensor) -> torch.Tensor:
         """embedding (+ pre-net) + positions of every [text | prompt] row and the AR prefill (valle.py:995-997,
         1013-1016), which fills cache stream b of buf, or p.slots_d[b]; returns the last row of each utterance [B, d]"""
         m = self.model
         S, Tp = p.S, p.Tp
         pe_t = self._pe(m.ar_text_position, max(S))
-        x = torch.empty((p.M, self.d), dtype=torch.float32, device=self.device)
+        x = torch.empty((sum(S) + sum(Tp), self.d), dtype=torch.float32, device=self.device)
         self._embed_pe(p.text_all, 1, m.ar_text_embedding.weight, pe_t, m.ar_text_position.alpha, sum(S), x, p.trow_d,
                        p.tpos_d, prenet=("ar_text", S) if self.pre else None)
         if self.prepend_bos:
@@ -883,8 +904,8 @@ class ValleEngine:
         else:
             self._embed_pe(p.prm_all, self.Q, self.ar_audio_table, pe_a, m.ar_audio_position.alpha, sum(Tp), x, p.arow_d,
                            p.apos_d)
-        self.ar.forward(x, p.cu_d, p.B, p.max_len, L.VB_MASK_VALLE_AR, p.S_d, None, buf.kcache, buf.vcache, buf.cap,
-                        k_exp=buf.k_exp, v_exp=buf.v_exp, cache_slots=p.slots_d)
+        self.ar.forward(x, p.cu_d, len(S), max(s + t for s, t in zip(S, Tp)), L.VB_MASK_VALLE_AR, p.S_d, None,
+                        buf.kcache, buf.vcache, buf.cap, k_exp=buf.k_exp, v_exp=buf.v_exp, cache_slots=p.slots_d)
         return ops.gather_rows(x, p.last_d)
 
     def _device_steps(self, buf: _ArBuffers, head: L.ArHead, n: int):
@@ -904,21 +925,16 @@ class ValleEngine:
         self._refresh()
         dev, Q = self.device, self.Q
         B = len(texts)
-        S = [int(t.numel()) for t in texts]
+        for b in range(B):
+            _check_utt(f"utterance {b}", texts[b], ys[b], Q, "code")
         T = [int(y.shape[0]) for y in ys]
         Tp = [min(int(t * 0.5), 3 * 75) for t in T]
-        Tg = [T[b] - Tp[b] for b in range(B)]
-        _check_ids(texts, NUM_TEXT_TOKENS, "phoneme")
-        _check_ids([y_[:, :1] for y_ in ys], NUM_AUDIO_TOKENS + 1, "code (first codebook)")
-        _check_ids([y_[:, 1:] for y_ in ys], NUM_AUDIO_TOKENS, "code")
-        text_all = torch.cat([t.reshape(-1).to(torch.int64) for t in texts]).to(dev)
+        text_all = torch.cat([t.to(torch.int64) for t in texts]).to(dev)
         prm_all = torch.cat([ys[b][:Tp[b]].to(torch.int64) for b in range(B)]).contiguous().to(dev)
-        cu_g = [0]
-        for n in Tg:
-            cu_g.append(cu_g[-1] + n)
-        codes = torch.empty((cu_g[-1], Q), dtype=torch.int64, device=dev)
-        codes[:, 0] = torch.cat([ys[b][Tp[b]:, 0].to(torch.int64) for b in range(B)]).to(dev)
-        self._nar(texts, text_all, prm_all, S, Tp, Tg, cu_g, codes, None, trim_text=False)
+        utts = [_Utt(b, t, pr, Tp[b]) for b, (t, pr) in
+                enumerate(zip(text_all.split([int(t.numel()) for t in texts]), prm_all.split(Tp)))]
+        codes, cu_g = self._nar(utts, [T[b] - Tp[b] for b in range(B)],
+                                torch.cat([ys[b][Tp[b]:, 0].to(torch.int64) for b in range(B)]).to(dev))
         if any(t.is_cuda for t in list(texts) + list(ys)):
             ops.check_oob(dev)
         return [codes[cu_g[b]:cu_g[b + 1]] for b in range(B)]
@@ -936,14 +952,6 @@ class ValleEngine:
         if prenet is not None:
             tmp = self._text_prenet(tmp, prenet[1], prenet[0])
         ops.add_pe(tmp, pe, alpha.detach(), x, n, positions=pos, out_rows=rows)
-
-    def _decode_step(self, buf: _ArBuffers, head: L.ArHead, greedy: bool, top_k: int, temperature: float,
-                     forced_step: Optional[torch.Tensor] = None, top_p: float = 1.0):
-        """one decode step without a graph; greedy: the step draws on the device (argmax, or the seeded sampler when
-        head.greedy == 2), else on the host"""
-        self._launch_step(buf, head)
-        if not greedy:
-            self._sample_push(buf, head, top_k, temperature, forced_step, top_p)
 
     def _replay_steps(self, buf: _ArBuffers, head: L.ArHead, k: int):
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
@@ -976,57 +984,47 @@ class ValleEngine:
                      forced_step: Optional[torch.Tensor] = None, top_p: float = 1.0):
         """valle.py:1287-1302 topk_sampling with torch's own RNG stream (so a fixed torch seed gives
         the reference's draws), then the stop rule + append on the device."""
+        from .models.valle import topk_sampling
         if forced_step is not None:  # teacher forcing (test hook): the given ids instead of a draw
             samp = forced_step.contiguous()
-            L.check(self.lib.vb_ar_push_tokens(C.byref(head), C.byref(buf.st), samp.data_ptr(), self.d,
-                                               L.stream_ptr()), "vb_ar_push_tokens")
-            return
-        from .models.valle import topk_sampling
-        logits = buf.logits[:, : self.n_vocab].clone()
-        if self.sample_on_host:
-            host = logits.cpu()
+        elif self.sample_on_host:
+            host = buf.logits[:, : self.n_vocab].cpu()
             samp = torch.cat([topk_sampling(host[b:b + 1], top_k=top_k, top_p=top_p, temperature=temperature).view(-1)
                               for b in range(host.shape[0])]).to(self.device)
         else:
-            samp = topk_sampling(logits, top_k=top_k, top_p=top_p, temperature=temperature).view(-1).contiguous()
+            samp = topk_sampling(buf.logits[:, : self.n_vocab].clone(), top_k=top_k, top_p=top_p,
+                                 temperature=temperature).view(-1).contiguous()
         L.check(self.lib.vb_ar_push_tokens(C.byref(head), C.byref(buf.st), samp.data_ptr(), self.d,
                                            L.stream_ptr()), "vb_ar_push_tokens")
 
-    def _nar(self, texts, text_all, prm_all, S, Tp, Tg, cu_g, codes, enroll_lens, trim_text: bool = True,
-             forced_codes: Optional[torch.Tensor] = None, trace: Optional[dict] = None):
+    def _nar(self, utts: Sequence[_Utt], Tg: Sequence[int], first_codes: torch.Tensor,
+             forced_codes: Optional[torch.Tensor] = None,
+             trace: Optional[dict] = None) -> Tuple[torch.Tensor, np.ndarray]:
+        """The NAR stages (valle.py:1059-1137) over utts, packed [text | prompt | generated]: first_codes, int64
+        [sum(Tg)], holds the first codebook of the Tg[b] generated frames of every utterance in turn.  Returns the
+        codes [sum(Tg), Q], packed the same way, and _offsets(Tg)."""
         m, dev, d, Q = self.model, self.device, self.d_nar, self.Q
-        B = len(S)
+        cu_g = _offsets(Tg)
+        G = int(cu_g[-1])
+        codes = torch.empty((G, Q), dtype=torch.int64, device=dev)
+        codes[:, 0] = first_codes
+        if Q == 1:
+            return codes, cu_g
+        B = len(utts)
         pm = self.prefix_mode
-        # text seen by the NAR decoder (valle.py:1068-1079)
-        if pm in (2, 4) and trim_text:
-            assert enroll_lens is not None
-            keep = []
-            off = 0
-            S2 = []
-            for b in range(B):
-                e = int(enroll_lens[b])
-                idx = [off] + list(range(off + e - 1, off + S[b]))
-                keep += idx
-                S2.append(len(idx))
-                off += S[b]
-            text_nar = text_all.index_select(0, torch.tensor(keep, dtype=torch.int64, device=dev))
-        else:
-            text_nar, S2 = text_all, list(S)
+
+        def nar_text(u):   # valle.py:1068-1079: prefix modes 2 / 4 keep the first phoneme and those after the enrolled
+            return (u.text[:1], u.text[u.enroll_len - 1:]) if pm in (2, 4) and u.enroll_len is not None else (u.text,)
+        pieces = [nar_text(u) for u in utts]
+        S2 = [sum(int(t.shape[0]) for t in ps) for ps in pieces]
+        text_nar = torch.cat([t for ps in pieces for t in ps])
+        prm_all = torch.cat([u.prompt for u in utts])
+        Tp = [int(u.prompt.shape[0]) for u in utts]
         T = [Tp[b] + Tg[b] for b in range(B)]
         Ltot = [S2[b] + T[b] for b in range(B)]
-        cu = [0]
-        for n in Ltot:
-            cu.append(cu[-1] + n)
-        M = cu[-1]
-        cu_t = [0]
-        for n in T:
-            cu_t.append(cu_t[-1] + n)
-        NT = cu_t[-1]
-        cu_p = [0]
-        for n in Tp:
-            cu_p.append(cu_p[-1] + n)
         # index maps (host-built with numpy, one H2D)
-        cu_np, cut_np = np.asarray(cu, dtype=np.int64), np.asarray(cu_t, dtype=np.int64)
+        cu_np, cut_np = _offsets(Ltot), _offsets(T)
+        M, NT = int(cu_np[-1]), int(cut_np[-1])
         S2_np, Tp_np = np.asarray(S2, dtype=np.int64), np.asarray(Tp, dtype=np.int64)
         trow, tpos = _seg_ranges(cu_np[:-1], S2)
         yrow, ypos = _seg_ranges(cu_np[:-1] + S2_np, T)
@@ -1035,17 +1033,8 @@ class ValleEngine:
         tgt_rows = _seg_ranges(cu_np[:-1] + S2_np + Tp_np, Tg)[0]
         meta = torch.from_numpy(np.concatenate([cu_np, trow, tpos, yrow, ypos, y_prompt_rows, y_gen_rows,
                                                 tgt_rows]).astype(np.int32)).to(dev)
-        o = 0
-        def take(n):
-            nonlocal o
-            v = meta[o:o + n]
-            o += n
-            return v
-        cu_d = take(B + 1)
-        trow_d, tpos_d = take(sum(S2)), take(sum(S2))
-        yrow_d, ypos_d = take(NT), take(NT)
-        yp_d, yg_d, tgt_d = take(sum(Tp)), take(sum(Tg)), take(sum(Tg))
-        G = sum(Tg)
+        cu_d, trow_d, tpos_d, yrow_d, ypos_d, yp_d, yg_d, tgt_d = meta.split(
+            [B + 1, sum(S2), sum(S2), NT, NT, sum(Tp), G, G])
 
         emb = [e.weight.detach() for e in m.nar_audio_embeddings]
         # y_emb = nar_audio_embeddings[0](y)  (valle.py:1064); rows packed [prompt_b | generated_b]
@@ -1092,3 +1081,4 @@ class ValleEngine:
                                           y_emb if nxt is not None else None, yg_d)
             if pm == 0 and i < Q - 2:  # valle.py:1104-1107
                 ops.embed_sum(prm_all[:, i + 1:], Q, 0, [emb[i + 1]], sum(Tp), y_emb, out_rows=yp_d, accumulate=True)
+        return codes, cu_g
