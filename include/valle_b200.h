@@ -25,11 +25,11 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 11
+#define VB_ABI_VERSION 12
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
- * bf16 AR decoding only (vb_decoder_forward_kv8, vb_ar_state.kv_dtype), never a weight or activation type. */
+ * bf16 AR decoding only ("FP8 (e4m3) KV cache" below), never a weight or activation type. */
 enum vb_dtype { VB_F32 = 0, VB_BF16 = 1, VB_E4M3 = 2 };
 enum vb_epilogue { VB_EPI_NONE = 0, VB_EPI_RELU = 1, VB_EPI_RESIDUAL = 2 };
 /* attention visibility rule */
@@ -158,21 +158,8 @@ void vb_decoder_destroy(vb_decoder_t dec);
 /* bytes of scratch vb_decoder_forward needs for M rows */
 size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t M);
 
-/* a5/a6  TransformerEncoder.forward WITHOUT the final norm over packed ragged sequences
- *   (prefill of the AR decoder, a NAR pass, the training forward).
- *   x: fp32 [M, d] residual stream, updated in place (post-LN: the output of the last layer's norm2).
- *   ada_wb: NULL (LayerNorm) or fp32 AdaLN (weight|bias) rows for the current stage, [(2*n_layer+1), 2d] for a
- *   stack with a final norm, [2*n_layer, 2d] without one: row 2l = layer l norm1, 2l+1 = layer l norm2, row 2*n_layer
- *   (if present) = final norm (read by the caller's final-norm call, not here).
- *   kcache/vcache: NULL or [n_layer, B, H, cache_cap, hd] caches filled for later decoding. */
-int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                       const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                       int mask_mode, const float *ada_wb,
-                       void *kcache, void *vcache, int64_t cache_layer_stride,
-                       int64_t cache_seq_stride, int cache_cap, void *workspace,
-                       size_t workspace_bytes, vb_stream_t stream);
-
-/* FP8 (e4m3) KV cache, one power-of-two scale per cached row.
+/* ------------------------------------------------------------------------------------------
+ * FP8 (e4m3) KV cache: the opt-in cache of bf16 AR decoding, one power-of-two scale per cached row.
  *   kcache / vcache: uint8 e4m3 [n_layer, B, H, cache_cap, 64] (the bf16 cache's layout with 1-byte elements);
  *   k_exp / v_exp:   uint8 [n_layer, B, H, cache_cap], the biased exponent e + 127 of each row (element offset / 64
  *                    of the row's first cache element: the strides are the cache's strides divided by 64).
@@ -181,31 +168,34 @@ int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32
  * all-zero row gets e = -127.  Stored bytes: cvt.rn.satfinite.e4m3(r * 2^-e) (= torch.float8_e4m3fn rounding of the
  * exactly scaled row); the row reads back as fp8 * 2^e, exact in fp32.
  * The AR decode step attends to the CURRENT token's k / v as the unquantized bf16 row it has just computed and appends
- * the quantized row: an FP8-cache step is the bf16 step run on the dequantized cache.  bf16 decoders only, on the
- * tensor-core decode chains (B <= 64, not VB_DECODE_SIMT, not VB_ATTN_DECODE_1PASS) and the wgmma prefill attention
- * (not VB_ATTN_SIMT); everything else returns VB_ERR_UNSUPPORTED. */
-/* vb_decoder_forward that fills an FP8 cache (kcache / vcache / k_exp / v_exp all non-NULL; strides in elements of the
- * [n_layer, B, H, cache_cap, 64] cache).  The FP8 cache requires (here and in vb_ar_decode_step, VB_ERR_ARG otherwise):
- * cache_layer_stride and cache_seq_stride multiples of 1024, cache_cap a multiple of 16, k_exp / v_exp 16-byte
- * aligned -- the decode attention reads the exponent rows 16 bytes at a time. */
-int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                           const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                           int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
-                           uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
-                           void *workspace, size_t workspace_bytes, vb_stream_t stream);
+ * the quantized row: an FP8-cache step is the bf16 step run on the dequantized cache.
+ * Layout (vb_decoder_forward and vb_ar_decode_step, VB_ERR_ARG otherwise): cache_layer_stride and cache_seq_stride
+ * multiples of 1024, cache_cap a multiple of 16, k_exp / v_exp both set and 16-byte aligned -- the decode attention
+ * reads the exponent rows 16 bytes at a time.
+ * bf16 decoders only, on the tensor-core decode chains (B <= 64, not VB_DECODE_SIMT, not VB_ATTN_DECODE_1PASS) and the
+ * wgmma prefill attention (not VB_ATTN_SIMT); everything else returns VB_ERR_UNSUPPORTED.
+ * ---------------------------------------------------------------------------------------- */
 
-/* Prefill into chosen cache streams (ABI 10; continuous batching: new utterances refill the stopped slots of a running
- * batch).  vb_decoder_forward over the B packed sequences, except that sequence b fills cache stream cache_slots[b]
- * ([n_layer, <cache batch>, H, cache_cap, hd] caches; FP8: its exponent rows as well) instead of stream b.
- * cache_slots: device int32 [B] of distinct values in [0, cache batch), or NULL = identity (then the call computes what
- * vb_decoder_forward / vb_decoder_forward_kv8 computes).  Every other stream of the cache is left untouched; x is the
- * same as without the map.  kcache / vcache non-NULL; k_exp / v_exp both NULL (a cache of the decoder's wdtype) or both
- * set (the FP8 cache, under the layout rules of vb_decoder_forward_kv8). */
-int vb_decoder_forward_slots(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                             const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                             int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
-                             uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
-                             const int32_t *cache_slots, void *workspace, size_t workspace_bytes, vb_stream_t stream);
+/* a5/a6  TransformerEncoder.forward WITHOUT the final norm over packed ragged sequences
+ *   (prefill of the AR decoder, a NAR pass, the training forward).
+ *   x: fp32 [M, d] residual stream, updated in place (post-LN: the output of the last layer's norm2).
+ *   ada_wb: NULL (LayerNorm) or fp32 AdaLN (weight|bias) rows for the current stage, [(2*n_layer+1), 2d] for a
+ *   stack with a final norm, [2*n_layer, 2d] without one: row 2l = layer l norm1, 2l+1 = layer l norm2, row 2*n_layer
+ *   (if present) = final norm (read by the caller's final-norm call, not here).
+ *   kcache / vcache: both NULL (no cache) or both [n_layer, <cache batch>, H, cache_cap, hd] caches filled for later
+ *   decoding; strides in elements.
+ *   k_exp / v_exp: both NULL (a cache of the decoder's wdtype) or both set: kcache / vcache are the FP8 cache (see
+ *   "FP8 (e4m3) KV cache" above).  Only with a cache.
+ *   cache_slots: NULL (identity: sequence b fills cache stream b) or device int32 [B] of distinct values in
+ *   [0, cache batch): sequence b fills cache stream cache_slots[b], FP8 exponent rows included (continuous batching:
+ *   new utterances refill the stopped slots of a running batch).  Every other stream of the cache is left untouched;
+ *   x is the same as without the map.  Only with a cache.
+ *   Any other combination of NULLs returns VB_ERR_ARG. */
+int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                       const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                       int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
+                       uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
+                       const int32_t *cache_slots, void *workspace, size_t workspace_bytes, vb_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * a2 / f2  Training: VALLE.forward with gradients (valle/models/valle.py:762-959; loss.backward() at
@@ -341,7 +331,7 @@ typedef struct vb_ar_state {
   const uint64_t *sample_seed; /* [B] seed of each utterance */
   const int32_t *top_k;        /* [B] <= 0 or >= n_vocab: no filter; 1: argmax */
   const float *temperature;    /* [B] finite, > 0 */
-  /* KV cache type (ABI 9): VB_E4M3 selects the FP8 cache (see vb_decoder_forward_kv8) with its exponent arrays
+  /* KV cache type (ABI 9): VB_E4M3 selects the FP8 cache ("FP8 (e4m3) KV cache" above) with its exponent arrays
    * k_exp / v_exp [n_layer, B, H, cache_cap]; any other value (0 in a zero-initialised state) = the decoder's wdtype */
   int32_t kv_dtype;
   int32_t kv_pad_unused;
@@ -385,9 +375,9 @@ int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb
 size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab);
 
 /* Admit k new utterances into rows slots[0..k) (device int32 [k], distinct, in [0, st->B)) of a running state (ABI 10;
- * after their prefill through vb_decoder_forward_slots).  h: fp32 [k, d], the last prefill row of each.  On entry the
- * slots' text_len, prompt_len, max_new (and, for head->greedy == 2, the sampler arrays, top_p / ras_* included) hold the new
- * utterances' values.  The call runs vb_ar_head_step on a k-row state built from those rows, with n_gen = 0 and
+ * after their prefill through vb_decoder_forward with cache_slots).  h: fp32 [k, d], the last prefill row of each.
+ * On entry the slots' text_len, prompt_len, max_new (and, for head->greedy == 2, the sampler arrays, top_p / ras_*
+ * included) hold the new utterances' values.  The call runs vb_ar_head_step on a k-row state built from those rows, with n_gen = 0 and
  * finished = 0, so admitted row i gets exactly what vb_ar_head_step on a fresh k-row state gives its row i.
  * Writes, for the slots only: n_gen, finished, tokens[slot, 0], x_cur[slot, :] and logits[slot, 0:n_vocab].  Every other
  * row of every array, the slots' other entries and the KV cache are left unchanged.  No host reads: safe to capture in

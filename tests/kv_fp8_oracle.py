@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY -- the FP8 (e4m3) KV-cache row format of include/valle_b200.h (vb_decoder_forward_kv8),
+"""TEST INFRASTRUCTURE ONLY -- the FP8 (e4m3) KV-cache row format of include/valle_b200.h ("FP8 (e4m3) KV cache"),
 restated with torch on the CPU.
 
 A cached row r is 64 values (the bf16 row the bf16 cache would hold).  a = max |r|; e = the smallest integer with

@@ -66,8 +66,8 @@ def _launches(fn):
 
 
 def _forward(name):
-    """fwd_{pre,post}_{ln_prefill,adaln_nar}_{f32,bf16}: one vb_decoder_forward call; fwd_{pre,post}_ln_prefill_f8: one
-    vb_decoder_forward_kv8 call (bf16 stack, FP8 cache)"""
+    """fwd_{pre,post}_{ln_prefill,adaln_nar}_{f32,bf16}: one vb_decoder_forward call; fwd_{pre,post}_ln_prefill_f8: the
+    same call with the exponent rows (bf16 stack, FP8 cache)"""
     from valle_b200 import _lib as L
     _, order, norm, shape, dt = name.split("_")
     f8 = dt == "f8"

@@ -1,4 +1,4 @@
-"""CPU checks of the FP8 KV-cache row format (tests/kv_fp8_oracle.py, include/valle_b200.h vb_decoder_forward_kv8):
+"""CPU checks of the FP8 KV-cache row format (tests/kv_fp8_oracle.py, include/valle_b200.h "FP8 (e4m3) KV cache"):
 the exponent rule puts every row's scaled maximum in (224, 448], the edge rows behave, and quantization is
 torch.float8_e4m3fn rounding of the exactly scaled row."""
 import torch

@@ -1,5 +1,5 @@
 """The opt-in FP8 (e4m3) KV cache of bf16 AR decoding (`VALLE.kv_cache_dtype = torch.float8_e4m3fn`, include/valle_b200.h
-vb_decoder_forward_kv8 / vb_ar_state.kv_dtype), on the GPU.
+"FP8 (e4m3) KV cache", vb_ar_state.kv_dtype), on the GPU.
 
   * prefill: the FP8 cache the prefill writes is, byte for byte and exponent for exponent, tests/kv_fp8_oracle.py applied
     to the bf16 cache the bf16 prefill writes; rows outside the sequences keep their sentinel;
@@ -320,7 +320,7 @@ def test_teacher_forced_logits_stay_within_the_e4m3_bar_big_short():
 
 
 # ---- errors and sizes ------------------------------------------------------------------------------------------------
-def test_errors():
+def test_forward_and_step_argument_errors():
     from valle_b200 import _lib as L
     m = _tiny()
     utts = _utts(1)
@@ -342,12 +342,15 @@ def test_errors():
     ke = torch.zeros(shape[:-1], dtype=torch.uint8, device=DEV)
     x = torch.zeros(4, nd.desc.d_model, device=DEV)
     cu = torch.tensor([0, 4], dtype=torch.int32, device=DEV)
-    ws = torch.zeros(nd.lib.vb_decoder_forward_workspace(C.byref(nd.desc), 4), dtype=torch.uint8, device=DEV)
-    st = nd.lib.vb_decoder_forward_kv8(nd.handle, x.data_ptr(), 4, B, cu.data_ptr(), cu.data_ptr(), None, 0, 4,
-                                       L.VB_MASK_VALLE_AR, None, k8.data_ptr(), k8.data_ptr(), ke.data_ptr(),
-                                       ke.data_ptr(), k8.stride(0), k8.stride(1), cap, ws.data_ptr(), ws.numel(),
-                                       L.stream_ptr())
-    assert st == 3, st
+
+    def forward(nd, kc, vc, ke, ve, slots=None):
+        ws = torch.zeros(nd.lib.vb_decoder_forward_workspace(C.byref(nd.desc), 4), dtype=torch.uint8, device=DEV)
+        return nd.lib.vb_decoder_forward(nd.handle, x.data_ptr(), 4, B, cu.data_ptr(), cu.data_ptr(), None, 0, 4,
+                                         L.VB_MASK_VALLE_AR, None, kc, vc, ke, ve, k8.stride(0), k8.stride(1), cap,
+                                         slots, ws.data_ptr(), ws.numel(), L.stream_ptr())
+
+    k, e = k8.data_ptr(), ke.data_ptr()
+    assert forward(nd, k, k, e, e) == 3
     s = L.ArState()
     s.B, s.cache_cap = B, cap
     s.kcache = s.vcache = k8.data_ptr()
@@ -365,12 +368,13 @@ def test_errors():
     s.k_exp = ke.data_ptr() + 1
     assert nd.lib.vb_ar_decode_step(nd.handle, C.byref(h), C.byref(s), w3.data_ptr(), nbytes, L.stream_ptr()) == 1
     assert b"16-byte" in nd.lib.vb_last_error()
-    ws = torch.zeros(nd.lib.vb_decoder_forward_workspace(C.byref(nd.desc), 4), dtype=torch.uint8, device=DEV)
-    st = nd.lib.vb_decoder_forward_kv8(nd.handle, x.data_ptr(), 4, B, cu.data_ptr(), cu.data_ptr(), None, 0, 4,
-                                       L.VB_MASK_VALLE_AR, None, k8.data_ptr(), k8.data_ptr(), ke.data_ptr(),
-                                       ke.data_ptr() + 1, k8.stride(0), k8.stride(1), cap, ws.data_ptr(), ws.numel(),
-                                       L.stream_ptr())
-    assert st == 1, st
+    assert forward(nd, k, k, e, e + 1) == 1
+    assert b"16-byte" in nd.lib.vb_last_error()
+    # exponent rows and a slot map need a cache, and the cache and the exponent rows come in pairs
+    assert forward(nd, None, None, None, None, cu.data_ptr()) == 1
+    assert forward(nd, None, None, e, e) == 1
+    assert forward(nd, k, k, e, None) == 1
+    assert forward(nd, k, None, None, None) == 1
 
 
 def test_fp8_buffers_take_half_the_cache_bytes():

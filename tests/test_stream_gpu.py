@@ -1,6 +1,6 @@
 """GPU checks of continuous batching (ValleEngine.generate_stream / VALLE.inference_stream) on an H100: the slot-mapped
-prefill (vb_decoder_forward_slots) and the admission of rows into a running decode state (vb_ar_admit) at the kernel
-level, then the streaming engine against solo decodes of every request, bit for bit.
+prefill (vb_decoder_forward with cache_slots) and the admission of rows into a running decode state (vb_ar_admit) at
+the kernel level, then the streaming engine against solo decodes of every request, bit for bit.
 
 Solo and streamed decodes run with different batch sizes and cache capacities.  The decode attention's KV split
 count follows both (decode_nsplit), and its partial results are combined in split order, so the module pins
@@ -96,25 +96,17 @@ def _check_equal(outs, solos):
 
 
 # ---------------------------------------------------------------- kernel level: slot-mapped prefill
-def _forward(lib, nd, x, cu, S, B, maxlen, kc, vc, ke, ve, slots, entry):
+def _forward(lib, nd, x, cu, S, B, maxlen, kc, vc, ke, ve, slots):
     ws = torch.empty(lib.vb_decoder_forward_workspace(C.byref(nd.desc), x.shape[0]), dtype=torch.uint8, device=DEV)
     ls, ss, cap = kc.stride(0), kc.stride(1), kc.shape[3]
-    common = (nd.handle, x.data_ptr(), x.shape[0], B, cu.data_ptr(), S.data_ptr(), None, 0, maxlen, L.VB_MASK_VALLE_AR,
-              None, kc.data_ptr(), vc.data_ptr())
-    if entry == "slots":
-        st = lib.vb_decoder_forward_slots(*common, L.ptr(ke), L.ptr(ve), ls, ss, cap, L.ptr(slots), ws.data_ptr(),
-                                          ws.numel(), L.stream_ptr())
-    elif ke is not None:
-        st = lib.vb_decoder_forward_kv8(*common, ke.data_ptr(), ve.data_ptr(), ls, ss, cap, ws.data_ptr(), ws.numel(),
-                                        L.stream_ptr())
-    else:
-        st = lib.vb_decoder_forward(*common, ls, ss, cap, ws.data_ptr(), ws.numel(), L.stream_ptr())
-    L.check(st, entry)
+    L.check(lib.vb_decoder_forward(nd.handle, x.data_ptr(), x.shape[0], B, cu.data_ptr(), S.data_ptr(), None, 0, maxlen,
+                                   L.VB_MASK_VALLE_AR, None, kc.data_ptr(), vc.data_ptr(), L.ptr(ke), L.ptr(ve), ls, ss,
+                                   cap, L.ptr(slots), ws.data_ptr(), ws.numel(), L.stream_ptr()), "vb_decoder_forward")
 
 
 @pytest.mark.parametrize("kind", ["f32", "bf16", "fp8"])
 @pytest.mark.parametrize("slots", [[5, 0, 3], [7, 2, 6, 1, 4]])
-def test_slot_mapped_prefill_equals_identity_prefill(lib, kind, slots):
+def test_slot_mapped_prefill_equals_unmapped_prefill(lib, kind, slots):
     dtype = torch.float32 if kind == "f32" else torch.bfloat16
     _, m = _model("tiny_pm1.pt", dtype)
     nd = m.ar_decoder.native(dtype)
@@ -142,17 +134,17 @@ def test_slot_mapped_prefill_equals_identity_prefill(lib, kind, slots):
 
     ident = caches(B, 0x5A)
     xi = x0.clone()
-    _forward(lib, nd, xi, cu, S, B, max(Ls), *ident, None, "plain")
-    xn, null = x0.clone(), caches(B, 0x5A)
-    _forward(lib, nd, xn, cu, S, B, max(Ls), *null, None, "slots")
-    assert torch.equal(xn, xi)
-    for a, b in zip(null, ident):
+    _forward(lib, nd, xi, cu, S, B, max(Ls), *ident, None)
+    xe, explicit = x0.clone(), caches(B, 0x5A)
+    _forward(lib, nd, xe, cu, S, B, max(Ls), *explicit, torch.arange(B, dtype=torch.int32, device=DEV))
+    assert torch.equal(xe, xi)
+    for a, b in zip(explicit, ident):
         if a is not None:
             assert torch.equal(raw(a), raw(b))
     sl = torch.tensor(slots, dtype=torch.int32, device=DEV)
     xs, mapped = x0.clone(), caches(8, 0x5A)
     before = [None if t is None else raw(t).clone() for t in mapped]
-    _forward(lib, nd, xs, cu, S, B, max(Ls), *mapped, sl, "slots")
+    _forward(lib, nd, xs, cu, S, B, max(Ls), *mapped, sl)
     torch.cuda.synchronize()
     assert torch.equal(xs, xi), "the residual rows depend on the slot map"
     for a, b, pre in zip(mapped, ident, before):

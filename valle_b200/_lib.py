@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 11
+ABI_VERSION = 12
 VB_F32, VB_BF16, VB_E4M3 = 0, 1, 2
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -132,11 +132,7 @@ PROTOTYPES = {
     "vb_decoder_destroy": (None, [vp]),
     "vb_decoder_forward_workspace": (C.c_size_t, [C.POINTER(DecoderDesc), C.c_int64]),
     "vb_decoder_forward": (C.c_int, [vp, vp, C.c_int64, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp,
-                                     C.c_int64, C.c_int64, C.c_int, vp, C.c_size_t, vp]),
-    "vb_decoder_forward_kv8": (C.c_int, [vp, vp, C.c_int64, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp,
-                                         vp, vp, C.c_int64, C.c_int64, C.c_int, vp, C.c_size_t, vp]),
-    "vb_decoder_forward_slots": (C.c_int, [vp, vp, C.c_int64, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp,
-                                           vp, vp, vp, C.c_int64, C.c_int64, C.c_int, vp, vp, C.c_size_t, vp]),
+                                     vp, vp, C.c_int64, C.c_int64, C.c_int, vp, vp, C.c_size_t, vp]),
     "vb_decoder_train_save_bytes": (C.c_size_t, [C.POINTER(DecoderDesc), C.c_int64]),
     "vb_decoder_forward_train": (C.c_int, [vp, vp, C.c_int64, C.c_int, vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp,
                                            C.c_size_t, C.c_float, C.c_uint64, vp]),

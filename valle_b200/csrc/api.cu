@@ -345,82 +345,46 @@ VB_API size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t 
   return carved_bytes(carve_forward_ws, *desc, M);
 }
 
-// the body of vb_decoder_forward and vb_decoder_forward_kv8 (fn: the entry point's name, for the error message)
-static int decoder_forward(const char *fn, vb_decoder_t dec, float *x, int64_t M, const Packed &pk, const float *ada_wb,
-                           const KvCache &cache, int64_t cache_layer_stride, void *workspace, size_t workspace_bytes,
-                           vb_stream_t stream) {
-  const vb_decoder_desc &D = dec->desc;
-  VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M), "%s: workspace too small (%zu < %zu)", fn,
-               workspace_bytes, vb_decoder_forward_workspace(&D, M));
-  if (M == 0) return VB_OK;
-  Carve c(workspace);
-  const LayerSave ws = carve_forward_ws(c, D, M);
-  return stack_forward(dec, x, M, pk, ada_wb, [&](int) { return ws; }, cache, cache_layer_stride, nullptr, 0.f, 0,
-                       (cudaStream_t)stream);
-}
-
-VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                                  const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start,
-                                  int max_seqlen, int mask_mode,
-                                  const float *ada_wb, void *kcache, void *vcache,
-                                  int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
-                                  void *workspace, size_t workspace_bytes, vb_stream_t stream) {
-  VB_CHECK_ARG(dec && x && cu_seqlens, "vb_decoder_forward: null argument");
-  const KvCache cache{kcache, vcache, nullptr, nullptr, cache_seq_stride, cache_cap, (int)elem_size(dec->desc.wdtype)};
-  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
-  return decoder_forward("vb_decoder_forward", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
-                         workspace_bytes, stream);
-}
-
-// the FP8 cache's exponent rows are read 16 bytes at a time (cp.async in the decode attention): every (layer, utterance,
-// head) stream of k_exp / v_exp, at offset stride / 64, and every 16-key chunk of it must start 16-byte aligned
-static bool kv8_layout_ok(const void *k_exp, const void *v_exp, int64_t layer_stride, int64_t seq_stride, int cap) {
-  return layer_stride % 1024 == 0 && seq_stride % 1024 == 0 && cap % 16 == 0 &&
-         (reinterpret_cast<uintptr_t>(k_exp) & 15) == 0 && (reinterpret_cast<uintptr_t>(v_exp) & 15) == 0;
-}
-
-// the FP8 cache's requirements (fn: the entry point's name, for the message)
-static int check_kv8(const char *fn, const vb_decoder_t dec, const uint8_t *k_exp, const uint8_t *v_exp,
+// The one check of an FP8 cache against a decoder (fn: the entry point's name, for the message): a bf16 decoder, both
+// exponent arrays, and their layout.  The exponent rows are read 16 bytes at a time (cp.async in the decode attention):
+// every (layer, utterance, head) stream of k_exp / v_exp, at offset stride / 64, and every 16-key chunk of it must
+// start 16-byte aligned.
+static int check_kv8(const char *fn, const vb_decoder_desc &D, const uint8_t *k_exp, const uint8_t *v_exp,
                      int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap) {
-  if (dec->desc.wdtype != VB_BF16) {
+  if (D.wdtype != VB_BF16) {
     set_error("%s: the FP8 KV cache needs a bf16 decoder", fn);
     return VB_ERR_UNSUPPORTED;
   }
-  VB_CHECK_ARG(kv8_layout_ok(k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap),
+  VB_CHECK_ARG(k_exp && v_exp, "%s: FP8 cache: k_exp / v_exp missing", fn);
+  VB_CHECK_ARG(cache_layer_stride % 1024 == 0 && cache_seq_stride % 1024 == 0 && cache_cap % 16 == 0 &&
+                   (reinterpret_cast<uintptr_t>(k_exp) & 15) == 0 && (reinterpret_cast<uintptr_t>(v_exp) & 15) == 0,
                "%s: FP8 cache: strides must be multiples of 1024, cache_cap a multiple of 16 and "
                "k_exp / v_exp 16-byte aligned", fn);
   return VB_OK;
 }
 
-VB_API int vb_decoder_forward_kv8(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                                  const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                                  int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
-                                  uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
-                                  void *workspace, size_t workspace_bytes, vb_stream_t stream) {
-  VB_CHECK_ARG(dec && x && cu_seqlens && kcache && vcache && k_exp && v_exp, "vb_decoder_forward_kv8: null argument");
-  VB_TRY(check_kv8("vb_decoder_forward_kv8", dec, k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap));
-  const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap, (int)elem_size(VB_E4M3)};
-  const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode};
-  return decoder_forward("vb_decoder_forward_kv8", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
-                         workspace_bytes, stream);
-}
-
-VB_API int vb_decoder_forward_slots(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
-                                    const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
-                                    int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
-                                    uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
-                                    const int32_t *cache_slots, void *workspace, size_t workspace_bytes,
-                                    vb_stream_t stream) {
-  VB_CHECK_ARG(dec && x && cu_seqlens && kcache && vcache, "vb_decoder_forward_slots: null argument");
-  VB_CHECK_ARG(!k_exp == !v_exp, "vb_decoder_forward_slots: k_exp / v_exp: both or neither");
+VB_API int vb_decoder_forward(vb_decoder_t dec, float *x, int64_t M, int B, const int32_t *cu_seqlens,
+                              const int32_t *text_lens, const int32_t *seg1_lens, int seg1_start, int max_seqlen,
+                              int mask_mode, const float *ada_wb, void *kcache, void *vcache, uint8_t *k_exp,
+                              uint8_t *v_exp, int64_t cache_layer_stride, int64_t cache_seq_stride, int cache_cap,
+                              const int32_t *cache_slots, void *workspace, size_t workspace_bytes, vb_stream_t stream) {
+  VB_CHECK_ARG(dec && x && cu_seqlens, "vb_decoder_forward: null argument");
+  VB_CHECK_ARG(!kcache == !vcache, "vb_decoder_forward: kcache / vcache: both or neither");
+  VB_CHECK_ARG(!k_exp == !v_exp, "vb_decoder_forward: k_exp / v_exp: both or neither");
+  VB_CHECK_ARG(kcache || (!k_exp && !cache_slots), "vb_decoder_forward: k_exp / v_exp and cache_slots need a cache");
+  const vb_decoder_desc &D = dec->desc;
   const bool f8 = k_exp != nullptr;
-  if (f8)
-    VB_TRY(check_kv8("vb_decoder_forward_slots", dec, k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap));
-  const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap,
-                      (int)elem_size(f8 ? VB_E4M3 : dec->desc.wdtype)};
+  if (f8) VB_TRY(check_kv8("vb_decoder_forward", D, k_exp, v_exp, cache_layer_stride, cache_seq_stride, cache_cap));
+  VB_CHECK_ARG(workspace_bytes >= vb_decoder_forward_workspace(&D, M),
+               "vb_decoder_forward: workspace too small (%zu < %zu)", workspace_bytes,
+               vb_decoder_forward_workspace(&D, M));
+  if (M == 0) return VB_OK;
+  const KvCache cache{kcache, vcache, k_exp, v_exp, cache_seq_stride, cache_cap, (int)elem_size(f8 ? VB_E4M3 : D.wdtype)};
   const Packed pk{cu_seqlens, text_lens, seg1_lens, B, max_seqlen, seg1_start, mask_mode, cache_slots};
-  return decoder_forward("vb_decoder_forward_slots", dec, x, M, pk, ada_wb, cache, cache_layer_stride, workspace,
-                         workspace_bytes, stream);
+  Carve c(workspace);
+  const LayerSave ws = carve_forward_ws(c, D, M);
+  return stack_forward(dec, x, M, pk, ada_wb, [&](int) { return ws; }, cache, cache_layer_stride, nullptr, 0.f, 0,
+                       (cudaStream_t)stream);
 }
 
 VB_API size_t vb_decoder_train_save_bytes(const vb_decoder_desc *desc, int64_t M) {
@@ -730,10 +694,9 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     set_error("vb_ar_decode_step: the FP8 KV cache runs on the bf16 tensor-core chains only (bf16, B <= 64, not VB_DECODE_SIMT)");
     return VB_ERR_UNSUPPORTED;
   }
-  VB_CHECK_ARG(!f8 || (st->k_exp && st->v_exp &&
-                       kv8_layout_ok(st->k_exp, st->v_exp, st->cache_layer_stride, st->cache_seq_stride, st->cache_cap)),
-               "vb_ar_decode_step: FP8 cache: exponent arrays missing, strides not multiples of 1024, cache_cap %% 16 != 0 "
-               "or k_exp / v_exp not 16-byte aligned");
+  if (f8)
+    VB_TRY(check_kv8("vb_ar_decode_step", D, st->k_exp, st->v_exp, st->cache_layer_stride, st->cache_seq_stride,
+                     st->cache_cap));
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model, dff = D.d_ff, B = st->B, dt = D.wdtype, hd = d / D.n_head;
   const size_t ts = elem_size(dt);

@@ -102,7 +102,7 @@ __device__ __forceinline__ void online_softmax(float (&s)[32], int j0, int t, co
   l_b = l_b * corr_b + rs_b;
 }
 
-// kF8: the KV cache is the FP8 one (include/valle_b200.h, vb_decoder_forward_kv8): e4m3 rows and their exponents;
+// kF8: the KV cache is the FP8 one (include/valle_b200.h, "FP8 (e4m3) KV cache"): e4m3 rows and their exponents;
 // the attention itself computes on the bf16 tiles either way
 template <bool kF8>
 __global__ void __launch_bounds__(kThreads, 2)

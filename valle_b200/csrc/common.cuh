@@ -125,7 +125,7 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ---- FP8 (e4m3) KV cache rows, one power-of-two scale per 64-element row (include/valle_b200.h,
-//      vb_decoder_forward_kv8).  Exponents travel biased: eb = e + 127, eb in [0, 254].
+//      "FP8 (e4m3) KV cache").  Exponents travel biased: eb = e + 127, eb in [0, 254].
 // eb of a row with max |r| = a: the smallest integer e with a <= 448 * 2^e (frexpf: a = m 2^x, m in [0.5, 1); e = x - 9
 // when m <= 0.875 = 448 / 2^9, else x - 8), clamped to [-127, 127]; an all-zero row gets e = -127
 __device__ __forceinline__ int kv8_exp_biased(float a) {

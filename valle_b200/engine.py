@@ -93,7 +93,7 @@ class StreamRequest(NamedTuple):
 class _ArBuffers:
     """Persistent device state for the AR loop at one (B, cache_cap, tok_stride, cache dtype) shape, plus the CUDA
     graphs of decode steps captured on it.  kv_dtype torch.float8_e4m3fn: the FP8 cache (e4m3 rows and one exponent
-    byte per cached row, include/valle_b200.h vb_decoder_forward_kv8); None: the engine dtype."""
+    byte per cached row, include/valle_b200.h "FP8 (e4m3) KV cache"); None: the engine dtype."""
 
     def __init__(self, eng: "ValleEngine", B: int, cap: int, tok_stride: int, kv_dtype: Optional[torch.dtype] = None):
         dev, d = eng.device, eng.d

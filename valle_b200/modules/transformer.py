@@ -405,34 +405,18 @@ class NativeDecoder:
                 vcache: Optional[Tensor] = None, cache_cap: int = 0, seg1_lens: Optional[Tensor] = None,
                 seg1_start: int = 0, k_exp: Optional[Tensor] = None, v_exp: Optional[Tensor] = None,
                 cache_slots: Optional[Tensor] = None) -> Tensor:
-        """In-place stack forward over packed rows x [M, d] fp32 (no final norm).  k_exp / v_exp (uint8 [n_layer, B, H,
-        cap]) given: kcache / vcache are the FP8 cache (torch.float8_e4m3fn, vb_decoder_forward_kv8).  cache_slots
-        (device int32 [B]) given: sequence b fills cache stream cache_slots[b] (vb_decoder_forward_slots)."""
+        """In-place stack forward over packed rows x [M, d] fp32 (no final norm): one vb_decoder_forward call.
+        kcache / vcache ([n_layer, B, H, cap, hd]) given: the attention fills them.  k_exp / v_exp (uint8 [n_layer, B,
+        H, cap]) given: kcache / vcache are the FP8 cache (torch.float8_e4m3fn, include/valle_b200.h "FP8 (e4m3) KV
+        cache").  cache_slots (device int32 [B]) given: sequence b fills cache stream cache_slots[b]."""
         M = x.shape[0]
-        nbytes = self.lib.vb_decoder_forward_workspace(C.byref(self.desc), M)
-        ws = self.workspace(nbytes)
-        ls = ss = 0
-        if kcache is not None:  # [n_layer, B, H, cap, hd]
-            ls, ss = kcache.stride(0), kcache.stride(1)
-        if cache_slots is not None:
-            L.check(self.lib.vb_decoder_forward_slots(self.handle, x.data_ptr(), M, B, cu_seqlens.data_ptr(),
-                                                      L.ptr(text_lens), L.ptr(seg1_lens), seg1_start, max_seqlen,
-                                                      mask_mode, L.ptr(ada), L.ptr(kcache), L.ptr(vcache), L.ptr(k_exp),
-                                                      L.ptr(v_exp), ls, ss, cache_cap, cache_slots.data_ptr(),
-                                                      ws.data_ptr(), ws.numel(), L.stream_ptr()),
-                    "vb_decoder_forward_slots")
-            return x
-        if k_exp is not None:
-            L.check(self.lib.vb_decoder_forward_kv8(self.handle, x.data_ptr(), M, B, cu_seqlens.data_ptr(),
-                                                    L.ptr(text_lens), L.ptr(seg1_lens), seg1_start, max_seqlen, mask_mode,
-                                                    L.ptr(ada), L.ptr(kcache), L.ptr(vcache), L.ptr(k_exp), L.ptr(v_exp),
-                                                    ls, ss, cache_cap, ws.data_ptr(), ws.numel(), L.stream_ptr()),
-                    "vb_decoder_forward_kv8")
-            return x
-        L.check(self.lib.vb_decoder_forward(self.handle, x.data_ptr(), M, B, cu_seqlens.data_ptr(),
-                                            L.ptr(text_lens), L.ptr(seg1_lens), seg1_start, max_seqlen, mask_mode, L.ptr(ada),
-                                            L.ptr(kcache), L.ptr(vcache), ls, ss, cache_cap,
-                                            ws.data_ptr(), ws.numel(), L.stream_ptr()), "vb_decoder_forward")
+        ws = self.workspace(self.lib.vb_decoder_forward_workspace(C.byref(self.desc), M))
+        ls, ss = (kcache.stride(0), kcache.stride(1)) if kcache is not None else (0, 0)
+        L.check(self.lib.vb_decoder_forward(self.handle, x.data_ptr(), M, B, cu_seqlens.data_ptr(), L.ptr(text_lens),
+                                            L.ptr(seg1_lens), seg1_start, max_seqlen, mask_mode, L.ptr(ada),
+                                            L.ptr(kcache), L.ptr(vcache), L.ptr(k_exp), L.ptr(v_exp), ls, ss, cache_cap,
+                                            L.ptr(cache_slots), ws.data_ptr(), ws.numel(), L.stream_ptr()),
+                "vb_decoder_forward")
         return x
 
     def final_norm(self, x: Tensor, ada: Optional[Tensor], rows: Optional[Tensor] = None,
