@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 12
+#define VB_ABI_VERSION 13
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
@@ -343,6 +343,22 @@ typedef struct vb_ar_state {
   const float *top_p;          /* [B] in (0, 1] */
   const int32_t *ras_window;   /* [B] in [0, 256] */
   const int32_t *ras_max;      /* [B] >= 0: fall back when the draw's count in the window exceeds it */
+  /* best-of-n decoding (ABI 13): n candidates of one utterance decode side by side and read one copy of their shared
+   * prompt prefix.  NULL means off, so a zero-initialised tail decodes as before.  vb_ar_admit does not use either
+   * field (it admits rows through a state of its own), and continuous batching does not set them. */
+  const int32_t *kv_parent;    /* [B] or NULL (vb_ar_decode_step).  Row b reads its cache rows below
+                                  P_b = 16 * floor((text_len[b] + prompt_len[b]) / 16) from row kv_parent[b]'s streams,
+                                  and every other row from its own.  Not checked (the step reads no host values): the
+                                  caller guarantees that kv_parent[kv_parent[b]] == kv_parent[b], that the parent has
+                                  row b's text_len and prompt_len, and that its streams hold those rows (its prefill
+                                  wrote them, and a finished row leaves its cache untouched).  The result is bitwise
+                                  the step in which row b reads the same rows from its own streams.  bf16 and fp32
+                                  caches only: with kv_dtype == VB_E4M3 the step returns VB_ERR_UNSUPPORTED. */
+  float *logprob;              /* [B] or NULL (vb_ar_head.greedy == 2 only: vb_ar_head_step, vb_ar_decode_step).  Each
+                                  token the seeded sampler appends to row b adds log_softmax(l)[token] to logprob[b],
+                                  l = the step's raw fp32 logits over all n_vocab ids (before temperature, top-k and
+                                  top-p), in fp32: logsumexp = max + logf(sum expf(l_i - max)).  A step that stops the
+                                  row adds nothing.  The caller zeroes the array. */
 } vb_ar_state;
 
 typedef struct vb_ar_head {

@@ -697,6 +697,10 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
   if (f8)
     VB_TRY(check_kv8("vb_ar_decode_step", D, st->k_exp, st->v_exp, st->cache_layer_stride, st->cache_seq_stride,
                      st->cache_cap));
+  if (f8 && st->kv_parent) {
+    set_error("vb_ar_decode_step: kv_parent (shared prompt prefixes) is not supported on the FP8 KV cache");
+    return VB_ERR_UNSUPPORTED;
+  }
   cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model, dff = D.d_ff, B = st->B, dt = D.wdtype, hd = d / D.n_head;
   const size_t ts = elem_size(dt);
@@ -735,7 +739,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     auto kv_slice = [&](int layer, int quarter) {
       if (pf_rows <= 0) return KvPrefetch{};
       const QkvScatter kv = layer_kv(D, st, layer % D.n_layer, w.q);
-      return KvPrefetch{kv.kv, kv.rows, B, D.n_head, pf_rows * quarter / 4, pf_rows * (quarter + 1) / 4};
+      return KvPrefetch{kv.kv, kv.rows, B, D.n_head, pf_rows * quarter / 4, pf_rows * (quarter + 1) / 4, st->kv_parent};
     };
     SplitK pend;  // the last FFN2's partial sums, for the next LayerNorm to add
     if (post) VB_TRY(launch_cast_from_f32(x, w.xn16, VB_BF16, (int64_t)B * d, s));
@@ -763,7 +767,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
                                     nullptr, nullptr, d, &kv, P, w.gemm_ws_bytes, &qkv, &pf_qkv, pdl, s));
         }
       }
-      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, kv_dt, w.att, w.att16, w.attn_ws, pdl, s));
+      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, kv_dt, w.att, w.att16, w.attn_ws, pdl, s, st->kv_parent));
       VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, sp.out, L.out_proj_b, DG_RESIDUAL, x,
                                 nullptr, d, nullptr, P, w.gemm_ws_bytes, &out, &pf_out, pdl, s, fold));
       if (fold) {
@@ -792,7 +796,7 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     const QkvScatter kv = layer_kv(D, st, l, w.q);
     LnParams ln1{P.norm1_w, P.norm1_b, nullptr, 1e-5f};
     VB_TRY(launch_gemv(x, d, B, P.in_proj_w, dt, P.in_proj_b, 3 * d, d, nullptr, 0, post ? nullptr : &ln1, 3, &kv, s));
-    VB_TRY(launch_attn_decode(kv, SplitK{}, B, D.n_head, dt, w.att, nullptr, w.attn_ws, false, s));
+    VB_TRY(launch_attn_decode(kv, SplitK{}, B, D.n_head, dt, w.att, nullptr, w.attn_ws, false, s, st->kv_parent));
     VB_TRY(launch_gemv(w.att, d, B, P.out_proj_w, dt, P.out_proj_b, d, d, x, d, nullptr, 2, nullptr, s));
     if (post) VB_TRY(launch_post_norm(x, B, d, P.norm1_w, P.norm1_b, nullptr, 1e-5f, nullptr, VB_F32, s));
     LnParams ln2{P.norm2_w, P.norm2_b, nullptr, 1e-5f};

@@ -218,6 +218,8 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int n_head, i
 // ------------------------------------------------------------------------------------------
 // Single-query decode attention over the KV cache.
 //   grid (H, B, nsplit), 128 threads.  kv_len[b] = S_b + Tp_b + n_gen[b].
+//   kShared (kv_parent != NULL, best-of-n decoding; bf16 and fp32 caches): the rows below P_b come from the parent
+//   row's streams (KvStreamRows); the same values in the same order as from the row's own copy of them.
 // ------------------------------------------------------------------------------------------
 static constexpr int kDecMaxChunk = 4096;
 
@@ -267,11 +269,12 @@ __device__ __forceinline__ bool decode_row_finished(const int32_t *finished, int
 // the chunk, streams the K row and the V row of its keys together (4 keys = 8 x 16-byte loads in
 // flight per lane), and keeps its OWN online-softmax state (m, l, 8 output elements per lane).  The 16
 // groups are merged once at the end (flash-decoding style).
-template <typename T>
+template <typename T, bool kShared = false>
 __global__ void __launch_bounds__(128)
 attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
                    float *__restrict__ out, bf16 *__restrict__ out16,
-                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit) {
+                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
+                   const int32_t *__restrict__ kv_parent) {
   __shared__ __align__(16) float qs[HD];
   __shared__ __align__(16) float knew[HD];
   __shared__ __align__(16) float vnew[HD];
@@ -290,6 +293,7 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
   const int n = max(0, c1 - c0);
   T *kb = (T *)kv.k + kv.row(b, h, 0);
   T *vb_ = (T *)kv.v + kv.row(b, h, 0);
+  const KvStreamRows<kShared> sr(kv_parent, rows, kv, b);
   const bool has_new = qp.part != nullptr;
   if (tid < HD) {
     if (has_new) {
@@ -337,8 +341,8 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
     for (int u = 0; u < 4; ++u) {
       const int key = base + u * 16 + grp;
       const int kk = min(key, n - 1);
-      KvRow8<T>::load(kb + (int64_t)(c0 + kk) * HD + j8, kf[u]);
-      KvRow8<T>::load(vb_ + (int64_t)(c0 + kk) * HD + j8, vf[u]);
+      KvRow8<T>::load(kb + sr.row(c0 + kk) + j8, kf[u]);
+      KvRow8<T>::load(vb_ + sr.row(c0 + kk) + j8, vf[u]);
     }
     float s[4];
 #pragma unroll
@@ -423,11 +427,12 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
 // rows.  The exponents of the chunk come into shared memory by cp.async; 2^e is applied once per row: to the score
 // (K) and to p_j ahead of P.V (V).  The current token's k / v are the unquantized bf16 rows, served from shared
 // memory; split 0 appends their quantized rows.
-template <int U, typename CT>
+template <int U, typename CT, bool kShared = false>
 __global__ void __launch_bounds__(128, 8)
 attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
                    float *__restrict__ out, bf16 *__restrict__ out16,
-                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit) {
+                   float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
+                   const int32_t *__restrict__ kv_parent) {
   constexpr bool kF8 = sizeof(CT) == 1;
   using Raw = typename std::conditional<kF8, uint2, uint4>::type;
   auto ld_raw = [](const CT *p) -> Raw {
@@ -461,6 +466,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
   using T = bf16;
   CT *kb = (CT *)kv.k + kv.row(b, h, 0);
   CT *vb_ = (CT *)kv.v + kv.row(b, h, 0);
+  const KvStreamRows<kShared> sr(kv_parent, rows, kv, b);
   const bool has_new = qp.part != nullptr;
   const int g = lane >> 3, j8 = (lane & 7) * 8;
   // The K rows of earlier tokens and the lengths do not depend on the kernels of THIS step that precede the
@@ -479,7 +485,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
     if (n > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        kraw[u] = ld_raw(kb + (int64_t)(c0 + min(u * 16 + warp * 4 + g, n - 1)) * HD + j8);
+        kraw[u] = ld_raw(kb + sr.row(c0 + min(u * 16 + warp * 4 + g, n - 1)) + j8);
     }
   };
   // (only with the fused QKV prologue: there the current token's row is served from shared memory; without it the
@@ -593,7 +599,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
     if (base > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        kraw[u] = ld_raw(kb + (int64_t)(c0 + min(base + u * 16 + warp * 4 + g, n - 1)) * HD + j8);
+        kraw[u] = ld_raw(kb + sr.row(c0 + min(base + u * 16 + warp * 4 + g, n - 1)) + j8);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
@@ -617,7 +623,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
   Raw vraw[U];
   if (n > 0) {
 #pragma unroll
-    for (int u = 0; u < U; ++u) vraw[u] = ld_raw(vb_ + (int64_t)(c0 + min(u * 16 + jl, n - 1)) * HD + eg);
+    for (int u = 0; u < U; ++u) vraw[u] = ld_raw(vb_ + sr.row(c0 + min(u * 16 + jl, n - 1)) + eg);
   }
   if (new_here && warp == 0) {  // score of the current token from the shared-memory key (never from the cache)
     float dot = 0.f;
@@ -667,7 +673,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
     if (base > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
-        vraw[u] = ld_raw(vb_ + (int64_t)(c0 + min(base + u * 16 + jl, n - 1)) * HD + eg);
+        vraw[u] = ld_raw(vb_ + sr.row(c0 + min(base + u * 16 + jl, n - 1)) + eg);
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
@@ -771,7 +777,7 @@ static int set_attn_carveout() {
 }
 
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
-                       void *workspace, bool pdl, cudaStream_t s) {
+                       void *workspace, bool pdl, cudaStream_t s, const int32_t *kv_parent) {
   VB_CHECK_ARG(kv.head_dim == HD, "attn_decode: head_dim=%d, only 64 is built", kv.head_dim);
   const int cache_cap = kv.kv.cap;
   const int ns = decode_nsplit(B, n_head, cache_cap);
@@ -792,18 +798,21 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
     constexpr auto k = attn_decode_2phase_pf_kernel<8, uint8_t>;
     VB_TRY(set_attn_carveout<k>());
     VB_CUDA(launch_kernel(k, grid, dim3(128), smem, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
-                          (bf16 *)out16, part_o, part_ml, ns));
+                          (bf16 *)out16, part_o, part_ml, ns, nullptr));   // no shared prefixes (vb_ar_decode_step)
   } else if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
-    VB_CUDA(launch_kernel(dtype == VB_F32 ? attn_decode_kernel<float> : attn_decode_kernel<bf16>, grid, dim3(128), 0, s,
-                          pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml,
-                          ns));
+    const auto k = dtype == VB_F32 ? (kv_parent ? attn_decode_kernel<float, true> : attn_decode_kernel<float>)
+                                   : (kv_parent ? attn_decode_kernel<bf16, true> : attn_decode_kernel<bf16>);
+    VB_CUDA(launch_kernel(k, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
+                          (bf16 *)out16, part_o, part_ml, ns, kv_parent));
   } else {
     // score buffer: the chunk of one split, rounded as the kernel rounds it (+16), in 1 KB steps
     const size_t sc_bytes = align_up((size_t)((cache_cap + ns - 1) / ns + 32) * sizeof(float), 1024);
     constexpr auto k = attn_decode_2phase_pf_kernel<4, bf16>;
-    VB_TRY(set_attn_carveout<k>());
-    VB_CUDA(launch_kernel(k, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
-                          (bf16 *)out16, part_o, part_ml, ns));
+    constexpr auto k_sh = attn_decode_2phase_pf_kernel<4, bf16, true>;
+    if (kv_parent) VB_TRY(set_attn_carveout<k_sh>());
+    else VB_TRY(set_attn_carveout<k>());
+    VB_CUDA(launch_kernel(kv_parent ? k_sh : k, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q, qkv, n_head,
+                          kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml, ns, kv_parent));
   }
   count_launch();
   if (ns > 1) {

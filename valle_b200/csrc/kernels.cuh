@@ -156,18 +156,50 @@ struct KvRows {
     return max(0, min(text_len[b] + prompt_len[b] + n_gen_b - 1, cap - 1));
   }
 };
+// Shared prompt prefix of best-of-n decoding (vb_ar_state.kv_parent): row b reads its cache rows below
+// P_b = 16 floor((text_len[b] + prompt_len[b]) / 16) from the streams of row parent[b], which holds the same text and
+// prompt, and every other row from its own streams.  A row that is its own parent shares nothing (P = 0).  P_b is a
+// multiple of 16, as is every KV split boundary; the current token's row is always >= S_b + Tp_b >= P_b, so every write
+// goes to the row's own streams.  bf16 and fp32 caches only: on the FP8 cache the shared read was measured slower than
+// every row reading its own copy (DESIGN section 7), so vb_ar_decode_step refuses it there.
+__device__ __forceinline__ int kv_shared_rows(const int32_t *parent, const KvRows &rows, int b, int &par) {
+  par = parent[b];
+  return par == b ? 0 : (rows.text_len[b] + rows.prompt_len[b]) & ~15;
+}
+// The rows of one (utterance, head) stream as a decode kernel reads them: element offset of row `pos` from the
+// stream's row 0.  kShared = false: the stream's own rows, nothing else is
+// computed.  kShared: rows below `shared` are the parent's, `poff` elements away (the parent's stream minus the own).
+template <bool kShared>
+struct KvStreamRows {
+  int64_t poff = 0;
+  int shared = 0;
+  __device__ __forceinline__ KvStreamRows() {}
+  __device__ __forceinline__ KvStreamRows(const int32_t *parent, const KvRows &rows, const KvCache &kv, int b) {
+    if constexpr (kShared) {
+      int par;
+      shared = kv_shared_rows(parent, rows, b, par);
+      poff = (int64_t)(par - b) * kv.seq_stride;
+    }
+  }
+  __device__ __forceinline__ int64_t row(int pos) const {
+    if constexpr (kShared) return (int64_t)pos * 64 + (pos < shared ? poff : 0);
+    else return (int64_t)pos * 64;
+  }
+};
 
 // L2 prefetch of a slice of an upcoming layer's K and V cache, issued by the otherwise idle warps of the
 // split-K decode projections (gemm_decode.cu) while their weight tiles stream: the projection chain is latency
 // bound and leaves HBM mostly idle, the KV-cache attention that follows is HBM bound -- rows [row_lo, row_hi) of
 // every (utterance, head) stream (the leading rows, where every CTA of the attention starts) are pulled into L2
 // ahead of it.  Only a hint: the lengths may be one step stale (read before the dependency wait),
-// which changes what is prefetched, never what is computed.
+// which changes what is prefetched, never what is computed.  A row whose parent (kv_parent) is another row skips the
+// shared rows: its parent's streams hold them and its parent fetches them.
 struct KvPrefetch {
   KvCache kv;   // the target layer (kv.k == nullptr: nothing to prefetch)
   KvRows rows;
   int B, H;
   int row_lo, row_hi;
+  const int32_t *kv_parent = nullptr;   // vb_ar_state.kv_parent, or nullptr
 };
 // worker = one warp; `n_workers` warps of the grid share the streams.  Lane i of a warp fetches the lengths of the
 // warp's i-th stream up front (the three dependent global loads per stream would otherwise serialise the loop).
@@ -194,7 +226,12 @@ __device__ __forceinline__ void kv_prefetch(const KvPrefetch &pf, int worker, in
     }
     const int pair = sidx >> 1;
     const int b = pair / pf.H, h = pair - b * pf.H;
-    const int r_lo = min(kv, pf.row_lo), r_hi = min(kv, pf.row_hi);
+    int lo = pf.row_lo;
+    if (pf.kv_parent != nullptr) {
+      int par;
+      lo = max(lo, kv_shared_rows(pf.kv_parent, pf.rows, b, par));
+    }
+    const int r_lo = min(kv, lo), r_hi = min(kv, pf.row_hi);
     const char *p = (const char *)((sidx & 1) ? pf.kv.v : pf.kv.k) + pf.kv.row(b, h, r_lo) * pf.kv.elem;
     const int lines = ((r_hi - r_lo) * row_bytes) >> 7;  // 128-byte lines
     for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + ((int64_t)l << 7)));
@@ -304,9 +341,9 @@ int launch_attention_wgmma(const bf16 *qkv, int64_t M, int n_head, const Packed 
                            cudaStream_t s);
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
 // the current token's q, k, v (kv.q, or pending in qkv) against the layer's cache kv.kv.  dtype VB_E4M3: the FP8
-// cache; q, k, v must then be pending in qkv
+// cache; q, k, v must then be pending in qkv.  kv_parent: vb_ar_state.kv_parent (NULL: every row reads its own streams)
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
-                       void *workspace, bool pdl, cudaStream_t s);
+                       void *workspace, bool pdl, cudaStream_t s, const int32_t *kv_parent);
 
 // decode_fused.cu
 int launch_relu_reduce(const SplitK &in, int B, int N, bf16 *out16, int64_t ldo, bool pdl, cudaStream_t s);

@@ -3,7 +3,8 @@
 //     (argmax==EOS or sample==EOS or n_new > 16*S), the append of :1057 and the embedding + sine PE
 //     of the appended token (:1013-1015) so the next decode step needs no host round trip
 //     (the reference syncs to the host once per token).
-//     ar_sample_kernel<true> draws the token with the seeded sampler (sample_row) instead of taking the argmax.
+//     ar_sample_kernel<true> draws the token with the seeded sampler (sample_row) instead of taking the argmax;
+//     ar_sample_kernel<true, true> also adds the drawn token's log-probability under the raw logits to the row's score.
 //   * sample_logits_kernel: the same sampler on caller-given logits (vb_sample_logits, vb_sample_logits_ex).
 //   * nar_argmax_accumulate_kernel: samples = argmax(logits) (:1130) and
 //     y_emb[:, Tp:] += nar_audio_embeddings[i+1](samples) (:1133-1134).
@@ -261,7 +262,7 @@ __device__ int sample_row(const float (&l)[5], int n, int amax, const RowSampler
   return d;
 }
 
-template <bool kSample>
+template <bool kSample, bool kScore = false>
 __global__ void __launch_bounds__(256)
 ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__restrict__ partials, int splits,
                  int ldp, int n_vocab, int eos_id,
@@ -271,7 +272,7 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
                  int32_t *__restrict__ n_gen, int32_t *__restrict__ finished,
                  int32_t *__restrict__ tokens, int tok_stride, float *__restrict__ x_cur, int d,
                  const int64_t *__restrict__ forced, int reduce_only, LnFoldStats fold, const float *__restrict__ fold_d,
-                 SamplerArgs sa) {
+                 SamplerArgs sa, float *__restrict__ logprob) {
   __shared__ ArgMax wbest[8];
   __shared__ int s_tok, s_pos;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -346,10 +347,25 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
     if (reduce_only) return;
   }
   int draw = -1;
+  float lse = 0.f;   // kScore: logsumexp of the raw logits
   if constexpr (kSample) {
     __shared__ SamplerSmem smp;
     best = block_argmax(best, wbest);
     draw = sample_row(lv, n_vocab, best.i, rs, smp);
+    if constexpr (kScore) {
+      // sum of expf(l_i - max) (a padding entry is -inf: 0), the 8 warps' sums added in order
+      __shared__ float wz[8];
+      float z = 0.f;
+#pragma unroll
+      for (int j = 0; j < 5; ++j) z += expf(lv[j] - best.v);
+      z = warp_sum(z);
+      if (lane == 0) wz[warp] = z;
+      __syncthreads();
+      z = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) z += wz[w];
+      lse = best.v + logf(z);
+    }
   } else {
     best = warp_argmax(best);
     if (lane == 0) wbest[warp] = best;
@@ -366,6 +382,7 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
       s_tok = -1;
     } else {
       tokens[(int64_t)b * tok_stride + n_new] = samp;
+      if constexpr (kScore) logprob[b] += row[samp] - lse;
       n_gen[b] = n_new + 1;
       s_tok = samp;
       s_pos = min(p_len + n_new, pe_rows - 1);
@@ -397,17 +414,20 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
 int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const vb_ar_head *head, vb_ar_state *st,
                      int d, const int64_t *forced, int reduce_only, bool pdl, cudaStream_t s) {
   const bool sample = head->greedy == 2 && forced == nullptr && !reduce_only;
+  const bool score = sample && st->logprob != nullptr;
   SamplerArgs sa{};
   if (sample) {
     VB_CHECK_ARG(st->sample_seed && st->top_k && st->temperature, "vb_ar_head.greedy == 2: sampler arrays not set");
     VB_CHECK_ARG(head->n_vocab <= 5 * 256, "device sampler: n_vocab %d > 1280", head->n_vocab);
     sa = SamplerArgs{st->sample_seed, st->top_k, st->temperature, st->top_p, st->ras_window, st->ras_max};
   }
-  VB_CUDA(launch_kernel(sample ? ar_sample_kernel<true> : ar_sample_kernel<false>, dim3(st->B), dim3(256), 0, s, pdl,
+  const auto k = score ? ar_sample_kernel<true, true> : sample ? ar_sample_kernel<true> : ar_sample_kernel<false>;
+  VB_CUDA(launch_kernel(k, dim3(st->B), dim3(256), 0, s, pdl,
                         logits, ld_logits, in.part, in.splits, in.ldp, head->n_vocab, head->eos_id, head->audio_emb,
                         head->alpha, head->pe, head->pe_rows, (const int32_t *)st->text_len,
                         (const int32_t *)st->prompt_len, (const int32_t *)st->max_new, st->n_gen, st->finished,
-                        st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, in.fold, in.bias, sa));
+                        st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, in.fold, in.bias, sa,
+                        score ? st->logprob : nullptr));
   count_launch();
   return VB_OK;
 }

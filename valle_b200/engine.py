@@ -122,6 +122,10 @@ class _ArBuffers:
         self.top_p = torch.ones(B, dtype=torch.float32, device=dev)
         self.ras_window = torch.zeros(B, **i32)
         self.ras_max = torch.zeros(B, **i32)
+        #: best-of-n: each row's parent row (the shared prompt prefix of its cache) and its AR log-likelihood; the
+        #: state points at them only in calls that use them (set_best_of)
+        self.kv_parent = torch.zeros(B, **i32)
+        self.logprob = torch.zeros(B, dtype=torch.float32, device=dev)
         st = L.ArState()
         st.B, st.tok_stride = B, tok_stride
         st.text_len, st.prompt_len, st.max_new = self.text_len.data_ptr(), self.prompt_len.data_ptr(), self.max_new.data_ptr()
@@ -140,6 +144,21 @@ class _ArBuffers:
         #: (head tables, draw mode, steps) -> (graph of that many decode steps, kernels per replay, head struct)
         self.graphs: Dict[tuple, Tuple[torch.cuda.CUDAGraph, int, L.ArHead]] = {}
         self.eng = eng
+
+    def set_best_of(self, n_rows: int, n: int, scores: bool):
+        """Point the state at kv_parent when n > 1 (row r of the first n_rows reads its parent r - r % n's prompt
+        prefix) and at logprob, zeroed, with scores; leave either NULL otherwise.  The FP8 cache keeps kv_parent NULL:
+        there the shared read is slower than every row reading its own copy (DESIGN section 7), and the codes are
+        the same either way."""
+        self.st.kv_parent = None
+        if n > 1 and self.kv_dtype is None:
+            r = torch.arange(n_rows, dtype=torch.int32)
+            self.kv_parent[:n_rows].copy_(r - r % n)
+            self.st.kv_parent = self.kv_parent.data_ptr()
+        self.st.logprob = None
+        if scores:
+            self.logprob.zero_()
+            self.st.logprob = self.logprob.data_ptr()
 
     def load_rows(self, p: _Prefill, draws: Optional[Sequence[_Draw]] = None):
         """Write the lengths and token caps of prefill block p's utterances into their rows (0..B-1, or p.slots_d)
@@ -294,6 +313,48 @@ def _draws(B: int, seed, top_k, temperature, top_p=1.0, ras=None) -> List[_Draw]
                 raise ValueError(f"ras: the threshold must lie in [0, 1) (got {t!r})")
             rr[i] = (int(w), t)
     return [_Draw(*v) for v in zip(seeds, ks, ts, ps, *_ras_arrays(rr))]
+
+
+def _check_num_samples(n, seed, return_scores: bool, trace, forced, sample_on_host: bool, bf16_rows: Optional[int]):
+    """Validated best-of-n arguments of generate(): n, an int >= 1.  n > 1 and return_scores need a seed (the seeded
+    device sampler); n > 1 excludes the trace / forced test hooks; bf16_rows: the rows of one bf16 decode group, which
+    must hold all n candidates of an utterance (None: no limit)"""
+    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 1:
+        raise ValueError(f"num_samples must be an int >= 1 (got {n!r})")
+    n = int(n)
+    if (n > 1 or return_scores) and seed is None:
+        raise ValueError("num_samples > 1 and return_scores need seed= (the seeded device sampler)")
+    if (n > 1 or return_scores) and sample_on_host:
+        raise ValueError("num_samples > 1 and return_scores draw on the device; they cannot be combined with "
+                         "sample_on_host = True")
+    if n > 1 and (trace is not None or forced is not None):
+        raise ValueError("num_samples > 1 cannot be combined with the trace / forced test hooks")
+    if return_scores and forced is not None:
+        raise ValueError("return_scores scores the seeded draws; forced ids replace them")
+    if bf16_rows is not None and n > bf16_rows:
+        raise ValueError(f"num_samples={n}: a bf16 decode group holds at most {bf16_rows} candidates of one utterance")
+    return n
+
+
+def _candidates(B: int, n: int, seed, per_utt: Dict[str, object], ras):
+    """The arguments of the repeated list that candidate j of utterance b stands for, row b * n + j: every
+    per-utterance sequence (checked to hold B values) repeated n times, and the seeds s + b * n + j for an int s, or
+    seed[b] + j for B seeds"""
+    def rep(v, what):
+        v = list(v)
+        if len(v) != B:
+            raise ValueError(f"{what}: {len(v)} values for {B} utterances")
+        return [x for x in v for _ in range(n)]
+    if _is_seq(seed):
+        if len(seed) != B:
+            raise ValueError(f"seed: {len(seed)} values for {B} utterances")
+        seeds = [int(s) + j for s in seed for j in range(n)]
+    else:
+        seeds = int(seed)        # s + r for row r = b * n + j, as the repeated list draws
+    out = {k: rep(v, k) if _is_seq(v) else v for k, v in per_utt.items()}
+    if _is_seq(ras) and len(ras) > 0 and (ras[0] is None or _is_seq(ras[0])):
+        ras = rep(ras, "ras")
+    return seeds, out, ras
 
 
 def _seg_ranges(starts, lens):
@@ -482,7 +543,7 @@ class ValleEngine:
                  max_new_tokens=None, poll: int = 32,
                  return_device: bool = False, trace: Optional[dict] = None,
                  forced: Optional[Sequence[torch.Tensor]] = None, seed=None, top_p=1.0,
-                 ras=None) -> List[torch.Tensor]:
+                 ras=None, num_samples: int = 1, return_scores: bool = False):
         """texts[b]: int64 [S_b] phoneme ids; prompts[b]: int64 [Tp_b, Q] codec ids (host or device).
         Returns codes[b]: int64 [Tgen_b, Q] -- per utterance exactly what VALLE.inference returns.
 
@@ -499,6 +560,18 @@ class ValleEngine:
         in [1, 256], threshold in [0, 1)) is replaced by a draw from the unfiltered distribution; see
         include/valle_b200.h vb_sample_logits_ex.
 
+        Best-of-n (seeded calls only): num_samples=n > 1 draws n candidates per utterance and returns codes[b][j], B
+        lists of n [T, Q] tensors.  Candidate j of utterance b draws from seed s + b * n + j (int s) or seed[b] + j (B
+        seeds), and its codes are bit for bit those of generate() on the list with every utterance repeated n times;
+        on the bf16 and fp32 caches the n candidates' decode steps read one copy of their shared prompt prefix from the
+        KV cache.  One caveat, the batch-size caveat every batched call carries: in bf16 a decode group holds
+        floor(64 / n) whole utterances, so with B * n > 64 and n not dividing 64 the groups differ from the repeated
+        list's groups of 64 rows, and the default KV split count (which depends on the group's size) may then round a
+        row's attention differently.  With VB_DECODE_NSPLIT fixed the codes are the repeated list's in every case.
+        return_scores=True (any seeded call) returns (codes, scores): scores [B, n] fp32, the AR log-likelihood of each
+        candidate, the sum over its first-codebook codes of log_softmax(raw logits)[code] (before temperature, top-k
+        and top-p), accumulated in fp32 on the device.
+
         Test hooks: `trace` collects AR logits (trace["steps"] = set of iterations or "all") and, with
         trace["nar"] = True, the NAR logits / argmax of every stage; `forced[b]` = int64 [T_b, Q] codes the decode is
         teacher-forced with (every sampled id is replaced by the given one before it is appended, AR and NAR), so
@@ -507,15 +580,26 @@ class ValleEngine:
         B = len(texts)
         if B < 1 or len(prompts) != B:
             raise ValueError(f"generate: {B} texts and {len(prompts)} prompts (one of each per utterance, >= 1)")
+        bf16 = self.dtype == torch.bfloat16
+        n = _check_num_samples(num_samples, seed, return_scores, trace, forced, self.sample_on_host,
+                               self.max_tc_batch if bf16 else None)
+        if n > 1:
+            seed, per, ras = _candidates(B, n, seed, dict(texts=texts, prompts=prompts, enroll_lens=enroll_lens,
+                                                          max_new_tokens=max_new_tokens, top_k=top_k,
+                                                          temperature=temperature, top_p=top_p), ras)
+            texts, prompts, enroll_lens, max_new_tokens = (per[k] for k in ("texts", "prompts", "enroll_lens",
+                                                                            "max_new_tokens"))
+            top_k, temperature, top_p = per["top_k"], per["temperature"], per["top_p"]
+        rows = B * n
         draws = None
         if ras is not None and self.sample_on_host:
             raise ValueError("ras draws on the device; it cannot be combined with sample_on_host = True")
         if seed is not None:
             if self.sample_on_host:
                 raise ValueError("seed= selects the device sampler; it cannot be combined with sample_on_host = True")
-            draws = _draws(B, seed, top_k, temperature, top_p, ras)
-            if all(dr.greedy for dr in draws):
-                draws, top_k = None, 1          # greedy: the seed draws nothing
+            draws = _draws(rows, seed, top_k, temperature, top_p, ras)
+            if all(dr.greedy for dr in draws) and not return_scores:
+                draws, top_k = None, 1          # greedy: the seed draws nothing (scores keep the seeded sampler)
         elif ras is not None:
             raise ValueError("ras needs seed= (the seeded device sampler)")
         elif _is_seq(top_k) or _is_seq(temperature) or _is_seq(top_p):
@@ -523,20 +607,26 @@ class ValleEngine:
         else:
             top_p = float(top_p)
             _check_top_p([top_p])
-        if not (B > self.max_tc_batch and self.dtype == torch.bfloat16 and trace is None and forced is None):
-            return self._generate(texts, prompts, enroll_lens, draws, top_k, temperature, top_p, max_new_tokens, poll,
-                                  return_device, trace, forced)
+        if not (rows > self.max_tc_batch and bf16 and trace is None and forced is None):
+            outs, scores = self._generate(texts, prompts, enroll_lens, draws, top_k, temperature, top_p,
+                                          max_new_tokens, poll, return_device, trace, forced, n, return_scores)
+            return self._best_of(outs, scores, B, n, return_scores, return_device)
         # the tensor-core decode projections take up to 64 rows (one UMMA N tile): a larger batch is decoded as
-        # consecutive groups of <= 64 utterances instead of falling onto the CUDA-core GEMV path
+        # consecutive groups of <= 64 rows instead of falling onto the CUDA-core GEMV path; a group holds whole
+        # utterances, all n candidates of each
+        group = self.max_tc_batch // n * n
         outs: List[torch.Tensor] = []
+        scores = []
         stats = EngineStats()
         packed = []
-        for b0 in range(0, B, self.max_tc_batch):
-            b1 = min(B, b0 + self.max_tc_batch)
+        for b0 in range(0, rows, group):
+            b1 = min(rows, b0 + group)
             mnt = max_new_tokens[b0:b1] if _is_seq(max_new_tokens) else max_new_tokens
-            outs += self._generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
+            o, sc = self._generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
                                    None if draws is None else draws[b0:b1], top_k, temperature, top_p, mnt, poll,
-                                   return_device)
+                                   return_device, num_samples=n, scores=return_scores)
+            outs += o
+            scores.append(sc)
             stats.ar_steps += self.stats.ar_steps
             stats.ar_ms += self.stats.ar_ms
             stats.prefill_ms += self.stats.prefill_ms
@@ -544,13 +634,27 @@ class ValleEngine:
             packed.append(self.last_packed)
         self.stats = stats
         self.last_packed = torch.cat(packed) if return_device else None
-        return outs
+        return self._best_of(outs, torch.cat(scores) if return_scores else None, B, n, return_scores, return_device)
+
+    @staticmethod
+    def _best_of(outs: List[torch.Tensor], scores: Optional[torch.Tensor], B: int, n: int, return_scores: bool,
+                 return_device: bool):
+        """generate()'s result from the codes of its B * n rows and their scores: the rows grouped per utterance when
+        n > 1, and (codes, scores [B, n]) with return_scores"""
+        codes = outs if n == 1 else [outs[b * n:(b + 1) * n] for b in range(B)]
+        if not return_scores:
+            return codes
+        scores = scores.view(B, n)
+        return codes, scores if return_device else scores.cpu()
 
     def _generate(self, texts, prompts, enroll_lens, draws: Optional[List[_Draw]], top_k, temperature, top_p,
                   max_new_tokens, poll: int, return_device: bool, trace: Optional[dict] = None,
-                  forced: Optional[Sequence[torch.Tensor]] = None) -> List[torch.Tensor]:
+                  forced: Optional[Sequence[torch.Tensor]] = None, num_samples: int = 1,
+                  scores: bool = False) -> Tuple[List[torch.Tensor], Optional[torch.Tensor]]:
         """generate() of one group of utterances with validated sampler arguments: draws (the seeded device sampler), or
-        None and top_k / temperature / top_p (greedy, or torch's sampler)"""
+        None and top_k / temperature / top_p (greedy, or torch's sampler).  num_samples > 1: the rows are the
+        candidates of B / num_samples utterances, num_samples consecutive rows each, which decode reading their first row's prompt prefix.  Returns the
+        codes and, with scores (seeded draws only), the rows' AR log-likelihoods on the device."""
         m, dev, Q = self.model, self.device, self.Q
         B = len(texts)
         kv_dtype = self.kv_cache_dtype()
@@ -586,6 +690,7 @@ class ValleEngine:
         buf.load_rows(p, draws if native else None)
         buf.n_gen.zero_()
         buf.finished.zero_()
+        buf.set_best_of(B, num_samples, scores)
         pe_a = self._pe(m.ar_audio_position, max(p.Tp) + max(cap_new) + 2)
         h_last = self._prefill(buf, p, pe_a)
         head = self._head(pe_a, 2 if native else int(greedy))
@@ -632,6 +737,7 @@ class ValleEngine:
                 Tg[b] = n_b
                 del running[b]
         self.stats.ar_steps = steps
+        logprob = buf.logprob[:B].clone() if scores else None
         ev[2].record()
 
         # ---- NAR (valle.py:1059-1137) ----
@@ -652,9 +758,9 @@ class ValleEngine:
         #: as is instead of re-packing the views)
         self.last_packed = codes
         if return_device:
-            return [codes[cu_g[b]:cu_g[b + 1]] for b in range(B)]
+            return [codes[cu_g[b]:cu_g[b + 1]] for b in range(B)], logprob
         host = codes.cpu()
-        return [host[cu_g[b]:cu_g[b + 1]] for b in range(B)]
+        return [host[cu_g[b]:cu_g[b + 1]] for b in range(B)], logprob
 
     def generate_stream(self, requests: Iterable, slots: Optional[int] = None, max_context: Optional[int] = None,
                         poll: int = 32, nar_batch: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor]]:
@@ -722,6 +828,7 @@ class ValleEngine:
             buf.n_gen.zero_()
             buf.finished.fill_(1)              # a slot that is never filled never runs, nor reads its sampler columns
             buf.x_cur.zero_()
+            buf.set_best_of(n_slots, 1, False)   # no shared prefixes or scores: slots are refilled one by one
             pe_a = self._pe(m.ar_audio_position, cap + 2)
             heads = {g: self._head(pe_a, g) for g in (1, 2)}
             ws = torch.empty(self.lib.vb_ar_admit_workspace(C.byref(self.ar.desc), n_slots, self.n_vocab),
@@ -955,8 +1062,9 @@ class ValleEngine:
 
     def _replay_steps(self, buf: _ArBuffers, head: L.ArHead, k: int):
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
-        draw mode, k))"""
-        key = (head.pe, head.predict_w, head.audio_emb, head.greedy, buf.kv_dtype, k)
+        draw mode, shared prefixes, scores, k))"""
+        key = (head.pe, head.predict_w, head.audio_emb, head.greedy, buf.kv_dtype, bool(buf.st.kv_parent),
+               bool(buf.st.logprob), k)
         graphs = buf.graphs
         ent = graphs.get(key)
         if ent is None:

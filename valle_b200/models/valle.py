@@ -236,17 +236,19 @@ class VALLE(nn.Module):
                         enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1,
                         temperature: float = 1.0, max_new_tokens=None,
                         dtype: Optional[torch.dtype] = None, return_device: bool = False,
-                        seed=None, top_p=1.0, ras=None) -> List[torch.Tensor]:
+                        seed=None, top_p=1.0, ras=None, num_samples: int = 1, return_scores: bool = False):
         """Engine feature (the reference asserts batch 1, valle.py:989): B independent utterances
         decoded together; result[b] equals `inference()` on utterance b alone.  Codes come back on the host, or
         (return_device=True) stay on the GPU, e.g. for the data-parallel gather of valle_b200.dist.
         Sampling (top_k != 1) keeps that promise with `seed` (an int s, or B ints): utterance b then equals
         `inference(..., seed=s + b)`; top_k, temperature and top_p may be per-utterance sequences, and ras one
         (window, threshold) pair or one per utterance (ValleEngine.generate).  max_new_tokens: one int or one per
-        utterance."""
+        utterance.  Best-of-n (seeded calls): num_samples=n draws n candidates per utterance, result[b][j], and
+        return_scores=True returns (codes, [B, n] AR log-likelihoods) (ValleEngine.generate)."""
         return self.engine(dtype).generate(texts, prompts, enroll_lens=enroll_lens, top_k=top_k,
                                            temperature=temperature, max_new_tokens=max_new_tokens,
-                                           return_device=return_device, seed=seed, top_p=top_p, ras=ras)
+                                           return_device=return_device, seed=seed, top_p=top_p, ras=ras,
+                                           num_samples=num_samples, return_scores=return_scores)
 
     def inference_stream(self, requests, slots: Optional[int] = None, max_context: Optional[int] = None,
                          poll: int = 32, nar_batch: Optional[int] = None, dtype: Optional[torch.dtype] = None):
