@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 13
+#define VB_ABI_VERSION 14
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
@@ -359,6 +359,27 @@ typedef struct vb_ar_state {
                                   l = the step's raw fp32 logits over all n_vocab ids (before temperature, top-k and
                                   top-p), in fp32: logsumexp = max + logf(sum expf(l_i - max)).  A step that stops the
                                   row adds nothing.  The caller zeroes the array. */
+  /* beam search (ABI 14).  beam_width <= 1 and NULL pointers mean off, so a zero-initialised tail decodes as before.
+   * With beam_width = n, the B rows are B / n groups of n consecutive rows, each group one utterance (the same
+   * text_len, prompt_len and max_new, its rows' caches prefilled alike), row j of a group holding beam j.  Generated
+   * position t of a hypothesis is a token tokens[r, t] and the cache rows S_b + Tp_b + t of row r's streams, r being the
+   * group's row named by the hypothesis's ancestry entry for t; each such entry is written once, by the beam that held
+   * row r at step t.  vb_ar_admit and continuous batching use none of these fields.
+   *   Decode attention (beam_width > 1, vb_ar_decode_step): row b reads its generated cache rows
+   *   [S_b + Tp_b, current row) from the streams of row b - b % n + beam_anc[b, row - S_b - Tp_b], the rows below P_b
+   *   from kv_parent (when set), every other row from its own streams; bitwise the step whose rows sit in row b's own
+   *   streams.  bf16 and fp32 caches only: with kv_dtype == VB_E4M3 the step returns VB_ERR_UNSUPPORTED.
+   *   Beam tail (vb_ar_head.greedy == 3, vb_ar_head_step and vb_ar_decode_step; beam_width in [1, 16]): see "Beam
+   *   search" below vb_ar_head. */
+  int32_t beam_width;          /* n, or 0 */
+  int32_t beam_pad_unused;
+  uint8_t *beam_anc;           /* [B, tok_stride] ancestry: beam_anc[b, t] in [0, n) = the group row holding position t */
+  float *beam_score;           /* [B] score s_j of each live beam; after the stop, the first row of the group holds the
+                                  result's score */
+  float *beam_fin_score;       /* [B / n, 2] the finished hypothesis: its ranking score c (-inf: none yet) and the
+                                  score over its codes */
+  int32_t *beam_fin_len;       /* [B / n] the finished hypothesis's length */
+  uint8_t *beam_fin_anc;       /* [B / n, tok_stride] the finished hypothesis's ancestry */
 } vb_ar_state;
 
 typedef struct vb_ar_head {
@@ -372,9 +393,30 @@ typedef struct vb_ar_head {
   int32_t greedy;             /* 1: argmax + stop rule + append on device; 0: logits only (the caller draws and
                                  calls vb_ar_push_tokens); 2: seeded draw on the device from the state's sampler
                                  arrays (vb_sample_logits_ex, with the row's n_gen as step and its tokens row as
-                                 history), then the stop rule + append as for 1 */
+                                 history), then the stop rule + append as for 1; 3: one beam-search step (below) */
   vb_ln_fold fold;            /* final LayerNorm folded into predict_w (all-NULL: separate LayerNorm launch) */
 } vb_ar_head;
+
+/* Beam search (vb_ar_head.greedy == 3, ABI 14), one step of one group of n = beam_width rows, all with n_gen = t.
+ * The caller sets, after the prefill: beam_score = 0 for the first row of each group and -inf for the others (so the
+ * first step expands beam 0 only), beam_fin_score[g, 0] = -inf, n_gen = finished = 0.  No host reads: capturable.
+ *   Candidates: every pair (j, v), j in [0, n), v in [0, n_vocab), scored c = fl(s_j + fl(l_jv - lse_j)), l the row's
+ *   raw fp32 logits and lse_j = max + logf(sum expf(l - max)) summed exactly as vb_ar_state.logprob sums it.
+ *   Ranking: c descending, then l_jv descending, then j ascending, then v ascending (a total order; the raw-logit key
+ *   makes n = 1 pick the greedy argmax when two logits round to the same c).
+ *   Cap: if t > max_new or t >= tok_stride, no candidate is taken and the group stops with the better of the finished
+ *   hypothesis (when it exists; it wins ties) and beam 0.
+ *   Selection: walking the ranking from the top, an EOS candidate at rank < n is offered to the finished hypothesis
+ *   (beam j's tokens, ranking score c, score s_j) and replaces it if c is strictly larger; EOS candidates never become
+ *   beams; the first n non-EOS candidates become beams 0..n-1 in rank order (token v appended at position t, score c,
+ *   the parent's ancestry plus their own row for t, x_cur = audio_emb[v] + alpha * pe[min(Tp + t, pe_rows - 1)]).
+ *   Stop: the group stops after a step in which the finished hypothesis's c >= beam 0's score.  Every increment
+ *   fl(l - lse) is <= 0 (lse >= max >= l), so no continuation can overtake it: the stop is exact, and scores are not
+ *   length-normalised.
+ *   On the stop, the result's tokens are gathered into tokens[first row, 0..len), its length into that row's n_gen
+ *   and its score (the sum over its codes: the EOS term ranks but is not part of it, so n = 1 reports what greedy == 2
+ *   with logprob reports) into beam_score[first row]; every row of the group gets finished = 1 (2 for a result of
+ *   length 0). */
 
 /* bytes of scratch for vb_ar_head_step / vb_ar_decode_step.  The buffer must not be shared between
  * concurrently running streams. */
@@ -416,6 +458,11 @@ int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st,
  * (valle.py:1040-1057 with torch's own RNG), applying the same stop rule. */
 int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int64_t *sampled, int d,
                       vb_stream_t stream);
+
+/* one beam-search step (head->greedy == 3, "Beam search" above) on the logits already in st->logits, as the decode
+ * step's tail runs it.  lse: NULL or [B], receives each row's log-sum-exp (written unless the step is a cap step), so
+ * that a caller can restate the ranking exactly. */
+int vb_ar_beam_step(const vb_ar_head *head, vb_ar_state *st, int d, float *lse, vb_stream_t stream);
 
 /* Seeded top-k / temperature draw (valle.py:1040-1043,1287-1302 with top_p = 1), one row r of logits[r * ld ...]
  * (ld may be 0: every row reads the same logits) with V <= 1280 entries:

@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 13
+ABI_VERSION = 14
 VB_F32, VB_BF16, VB_E4M3 = 0, 1, 2
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -47,7 +47,9 @@ class ArState(C.Structure):
                 ("cache_cap", C.c_int32), ("_unused", C.c_int32),
                 ("sample_seed", vp), ("top_k", vp), ("temperature", vp),
                 ("kv_dtype", C.c_int32), ("_kv_pad", C.c_int32), ("k_exp", vp), ("v_exp", vp),
-                ("top_p", vp), ("ras_window", vp), ("ras_max", vp), ("kv_parent", vp), ("logprob", vp)]
+                ("top_p", vp), ("ras_window", vp), ("ras_max", vp), ("kv_parent", vp), ("logprob", vp),
+                ("beam_width", C.c_int32), ("_beam_pad", C.c_int32), ("beam_anc", vp), ("beam_score", vp),
+                ("beam_fin_score", vp), ("beam_fin_len", vp), ("beam_fin_anc", vp)]
 
 
 class LnFold(C.Structure):
@@ -163,6 +165,7 @@ PROTOTYPES = {
     "vb_ar_admit": (C.c_int, [vp, C.POINTER(ArHead), vp, C.c_int, vp, C.POINTER(ArState), vp, C.c_size_t, vp]),
     "vb_ar_decode_step": (C.c_int, [vp, C.POINTER(ArHead), C.POINTER(ArState), vp, C.c_size_t, vp]),
     "vb_ar_push_tokens": (C.c_int, [C.POINTER(ArHead), C.POINTER(ArState), vp, C.c_int, vp]),
+    "vb_ar_beam_step": (C.c_int, [C.POINTER(ArHead), C.POINTER(ArState), C.c_int, vp, vp]),
     "vb_sample_logits": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp, vp]),
     "vb_sample_logits_ex": (C.c_int, [vp, C.c_int64, C.c_int64, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int64,
                                       vp, vp]),

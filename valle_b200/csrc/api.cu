@@ -552,6 +552,31 @@ QkvScatter layer_kv(const vb_decoder_desc &D, const vb_ar_state *st, int l, floa
                     KvRows{st->text_len, st->prompt_len, st->n_gen, st->finished}};
 }
 
+// the beam ancestry the decode attention follows (beam_width > 1), or none
+BeamAnc beam_anc(const vb_ar_state *st) {
+  return st->beam_width > 1 ? BeamAnc{st->beam_anc, st->tok_stride, st->beam_width} : BeamAnc{};
+}
+// the beam-search fields a step with this head reads (include/valle_b200.h "Beam search")
+int check_beam(const char *fn, const vb_ar_head *head, const vb_ar_state *st) {
+  if (head->greedy == 3 || st->beam_width > 1) {
+    VB_CHECK_ARG(st->beam_width >= 1 && st->beam_width <= 16 && st->B % st->beam_width == 0,
+                 "%s: beam_width %d not in [1, 16] or not dividing B = %d", fn, st->beam_width, st->B);
+    VB_CHECK_ARG(st->beam_anc != nullptr, "%s: beam search needs beam_anc", fn);
+  }
+  if (head->greedy == 3)
+    VB_CHECK_ARG(st->beam_score && st->beam_fin_score && st->beam_fin_len && st->beam_fin_anc,
+                 "%s: vb_ar_head.greedy == 3: beam arrays not set", fn);
+  return VB_OK;
+}
+// the step's tail on the head's logits (in: their pending partials): the argmax / seeded draw, the reduce alone
+// (greedy == 0), or the reduce and the beam step (greedy == 3)
+int ar_tail(int ldl, const SplitK &in, const vb_ar_head *head, vb_ar_state *st, int d, bool pdl, cudaStream_t s) {
+  if (head->greedy != 3)
+    return launch_ar_sample(st->logits, ldl, in, head, st, d, nullptr, head->greedy ? 0 : 1, pdl, s);
+  if (in.part) VB_TRY(launch_ar_sample(st->logits, ldl, in, head, st, d, nullptr, 1, pdl, s));
+  return launch_beam_tail(head, st, d, pdl, s);
+}
+
 // final LayerNorm (adding the pending partials of the last FFN2) + ar_predict_layer + sampler on the tensor-core
 // path.  fold: the final norm is folded into ar_predict_layer, the projection reads the fp32 rows and the sampler
 // applies the moments.  A stack without a final norm (post-LN) feeds the head the bf16 rows of x: w.xn16 as the
@@ -565,7 +590,7 @@ int tc_head(const vb_decoder_desc &D, const vb_ar_head *head, float *x, vb_ar_st
   if (fold) {
     VB_TRY(launch_gemm_decode_x(x, B, d, head->fold, head->n_vocab, d, 0, (float *)w.gemm_ws, w.gemm_ws_bytes, w.stats,
                                 &logits, nullptr, pdl, s));
-    return launch_ar_sample(st->logits, ldl, logits, head, st, d, nullptr, head->greedy ? 0 : 1, pdl, s);
+    return ar_tail(ldl, logits, head, st, d, pdl, s);
   }
   if (D.final_norm_w)
     VB_TRY(launch_ln_reduce(x, d, B, d, pend, D.final_norm_w, D.final_norm_b, 1e-5f, w.xn16, pdl, s));
@@ -575,8 +600,7 @@ int tc_head(const vb_decoder_desc &D, const vb_ar_head *head, float *x, vb_ar_st
                             st->logits, nullptr, ldl, nullptr, (float *)w.gemm_ws, w.gemm_ws_bytes, &logits, nullptr,
                             pdl, s));
   // logits only (host-side sampling follows) and split: just reduce the partials
-  if (head->greedy || logits.part)
-    VB_TRY(launch_ar_sample(st->logits, ldl, logits, head, st, d, nullptr, head->greedy ? 0 : 1, pdl, s));
+  if (head->greedy || logits.part) VB_TRY(ar_tail(ldl, logits, head, st, d, pdl, s));
   return VB_OK;
 }
 }  // namespace
@@ -588,7 +612,8 @@ VB_API size_t vb_ar_step_workspace(const vb_decoder_desc *desc, int B, int cache
 VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
                            void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && head && h && st, "vb_ar_head_step: null argument");
-  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_head_step: greedy %d not in {0, 1, 2}", head->greedy);
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 3, "vb_ar_head_step: greedy %d not in {0, 1, 2, 3}", head->greedy);
+  VB_TRY(check_beam("vb_ar_head_step", head, st));
   const vb_decoder_desc &D = dec->desc;
   VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_head_step: a pre-LN decoder needs its final norm");
   cudaStream_t s = (cudaStream_t)stream;
@@ -604,7 +629,7 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
   LnParams ln{D.final_norm_w, D.final_norm_b, nullptr, 1e-5f};
   VB_TRY(launch_gemv(h, d, st->B, head->predict_w, D.wdtype, nullptr, head->n_vocab, d, st->logits, ldl,
                      D.final_norm_w ? &ln : nullptr, 0, nullptr, s));
-  if (head->greedy) VB_TRY(launch_ar_sample(st->logits, ldl, SplitK{}, head, st, d, nullptr, 0, false, s));
+  if (head->greedy) VB_TRY(ar_tail(ldl, SplitK{}, head, st, d, false, s));
   return VB_OK;
 }
 
@@ -680,10 +705,19 @@ VB_API int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int6
   return launch_ar_sample(st->logits, ldl, SplitK{}, head, st, d, sampled, 0, false, (cudaStream_t)stream);
 }
 
+VB_API int vb_ar_beam_step(const vb_ar_head *head, vb_ar_state *st, int d, float *lse, vb_stream_t stream) {
+  VB_CHECK_ARG(head && st, "vb_ar_beam_step: null argument");
+  VB_CHECK_ARG(head->greedy == 3, "vb_ar_beam_step: vb_ar_head.greedy %d != 3", head->greedy);
+  VB_TRY(check_beam("vb_ar_beam_step", head, st));
+  return launch_beam_tail(head, st, d, false, (cudaStream_t)stream, lse);
+}
+
 VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st, void *workspace,
                              size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && head && st, "vb_ar_decode_step: null argument");
-  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_decode_step: greedy %d not in {0, 1, 2}", head->greedy);
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 3, "vb_ar_decode_step: greedy %d not in {0, 1, 2, 3}",
+               head->greedy);
+  VB_TRY(check_beam("vb_ar_decode_step", head, st));
   const vb_decoder_desc &D = dec->desc;
   // the pre-LN chain leaves the last FFN2's partial sums to the final norm's reduce: without one they would be lost
   VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_decode_step: a pre-LN decoder needs its final norm");
@@ -699,6 +733,10 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
                      st->cache_cap));
   if (f8 && st->kv_parent) {
     set_error("vb_ar_decode_step: kv_parent (shared prompt prefixes) is not supported on the FP8 KV cache");
+    return VB_ERR_UNSUPPORTED;
+  }
+  if (f8 && st->beam_width > 1) {
+    set_error("vb_ar_decode_step: beam search (beam_width > 1) is not supported on the FP8 KV cache");
     return VB_ERR_UNSUPPORTED;
   }
   cudaStream_t s = (cudaStream_t)stream;
@@ -767,7 +805,8 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
                                     nullptr, nullptr, d, &kv, P, w.gemm_ws_bytes, &qkv, &pf_qkv, pdl, s));
         }
       }
-      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, kv_dt, w.att, w.att16, w.attn_ws, pdl, s, st->kv_parent));
+      VB_TRY(launch_attn_decode(kv, qkv, B, D.n_head, kv_dt, w.att, w.att16, w.attn_ws, pdl, s, st->kv_parent,
+                                beam_anc(st)));
       VB_TRY(launch_gemm_decode(w.att16, B, d, (const bf16 *)L.out_proj_w, d, d, sp.out, L.out_proj_b, DG_RESIDUAL, x,
                                 nullptr, d, nullptr, P, w.gemm_ws_bytes, &out, &pf_out, pdl, s, fold));
       if (fold) {
@@ -796,7 +835,8 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     const QkvScatter kv = layer_kv(D, st, l, w.q);
     LnParams ln1{P.norm1_w, P.norm1_b, nullptr, 1e-5f};
     VB_TRY(launch_gemv(x, d, B, P.in_proj_w, dt, P.in_proj_b, 3 * d, d, nullptr, 0, post ? nullptr : &ln1, 3, &kv, s));
-    VB_TRY(launch_attn_decode(kv, SplitK{}, B, D.n_head, dt, w.att, nullptr, w.attn_ws, false, s, st->kv_parent));
+    VB_TRY(launch_attn_decode(kv, SplitK{}, B, D.n_head, dt, w.att, nullptr, w.attn_ws, false, s, st->kv_parent,
+                              beam_anc(st)));
     VB_TRY(launch_gemv(w.att, d, B, P.out_proj_w, dt, P.out_proj_b, d, d, x, d, nullptr, 2, nullptr, s));
     if (post) VB_TRY(launch_post_norm(x, B, d, P.norm1_w, P.norm1_b, nullptr, 1e-5f, nullptr, VB_F32, s));
     LnParams ln2{P.norm2_w, P.norm2_b, nullptr, 1e-5f};

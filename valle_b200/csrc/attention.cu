@@ -220,6 +220,9 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int n_head, i
 //   grid (H, B, nsplit), 128 threads.  kv_len[b] = S_b + Tp_b + n_gen[b].
 //   kShared (kv_parent != NULL, best-of-n decoding; bf16 and fp32 caches): the rows below P_b come from the parent
 //   row's streams (KvStreamRows); the same values in the same order as from the row's own copy of them.
+//   kBeam (beam search; bf16 and fp32 caches): the generated rows below the current one come from the streams the
+//   beam ancestry names, every row through a table of stream offsets the CTA stages in shared memory behind its
+//   other buffers; again the same values in the same order as from a stream that holds them all.
 // ------------------------------------------------------------------------------------------
 static constexpr int kDecMaxChunk = 4096;
 
@@ -269,12 +272,12 @@ __device__ __forceinline__ bool decode_row_finished(const int32_t *finished, int
 // the chunk, streams the K row and the V row of its keys together (4 keys = 8 x 16-byte loads in
 // flight per lane), and keeps its OWN online-softmax state (m, l, 8 output elements per lane).  The 16
 // groups are merged once at the end (flash-decoding style).
-template <typename T, bool kShared = false>
+template <typename T, bool kShared = false, bool kBeam = false>
 __global__ void __launch_bounds__(128)
 attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
                    float *__restrict__ out, bf16 *__restrict__ out16,
                    float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
-                   const int32_t *__restrict__ kv_parent) {
+                   const int32_t *__restrict__ kv_parent, BeamAnc beam) {
   __shared__ __align__(16) float qs[HD];
   __shared__ __align__(16) float knew[HD];
   __shared__ __align__(16) float vnew[HD];
@@ -293,7 +296,11 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
   const int n = max(0, c1 - c0);
   T *kb = (T *)kv.k + kv.row(b, h, 0);
   T *vb_ = (T *)kv.v + kv.row(b, h, 0);
-  const KvStreamRows<kShared> sr(kv_parent, rows, kv, b);
+  KvStreamRows<kShared, kBeam> sr(kv_parent, rows, kv, b);
+  if constexpr (kBeam) {   // read after the __syncthreads below
+    extern __shared__ __align__(16) int16_t beam_dl[];
+    sr.stage_beam(beam_dl, kv_parent, rows, beam, b, c0, n, pos);
+  }
   const bool has_new = qp.part != nullptr;
   if (tid < HD) {
     if (has_new) {
@@ -427,12 +434,12 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
 // rows.  The exponents of the chunk come into shared memory by cp.async; 2^e is applied once per row: to the score
 // (K) and to p_j ahead of P.V (V).  The current token's k / v are the unquantized bf16 rows, served from shared
 // memory; split 0 appends their quantized rows.
-template <int U, typename CT, bool kShared = false>
+template <int U, typename CT, bool kShared = false, bool kBeam = false>
 __global__ void __launch_bounds__(128, 8)
 attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
                    float *__restrict__ out, bf16 *__restrict__ out16,
                    float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
-                   const int32_t *__restrict__ kv_parent) {
+                   const int32_t *__restrict__ kv_parent, BeamAnc beam) {
   constexpr bool kF8 = sizeof(CT) == 1;
   using Raw = typename std::conditional<kF8, uint2, uint4>::type;
   auto ld_raw = [](const CT *p) -> Raw {
@@ -466,7 +473,7 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
   using T = bf16;
   CT *kb = (CT *)kv.k + kv.row(b, h, 0);
   CT *vb_ = (CT *)kv.v + kv.row(b, h, 0);
-  const KvStreamRows<kShared> sr(kv_parent, rows, kv, b);
+  KvStreamRows<kShared, kBeam> sr(kv_parent, rows, kv, b);
   const bool has_new = qp.part != nullptr;
   const int g = lane >> 3, j8 = (lane & 7) * 8;
   // The K rows of earlier tokens and the lengths do not depend on the kernels of THIS step that precede the
@@ -482,6 +489,11 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
     c0 = sp * chunk;
     c1 = min(kv_len, c0 + chunk);
     n = max(0, c1 - c0);
+    if constexpr (kBeam) {   // the row table behind the score buffer (only after the dependency wait: see below)
+      const int sc_len = ((kv.cap + nsplit - 1) / nsplit + 32 + 15) & ~15;
+      sr.stage_beam(reinterpret_cast<int16_t *>(sc + sc_len), kv_parent, rows, beam, b, c0, n, pos);
+      __syncthreads();
+    }
     if (n > 0) {
 #pragma unroll
       for (int u = 0; u < U; ++u)
@@ -489,9 +501,10 @@ attn_decode_2phase_pf_kernel(const float *__restrict__ q, SplitK qp, int n_head,
     }
   };
   // (only with the fused QKV prologue: there the current token's row is served from shared memory; without it the
-  // row was written to the cache by the kernel this launch depends on and nothing may be read ahead of the wait)
-  const int n_gen_early = has_new ? rows.n_gen[b] : -1;
-  if (has_new) setup(n_gen_early);
+  // row was written to the cache by the kernel this launch depends on and nothing may be read ahead of the wait.
+  // kBeam: the ancestry is written by the previous step's tail, so the rows are located only after the wait.)
+  const int n_gen_early = (has_new && !kBeam) ? rows.n_gen[b] : -1;
+  if (has_new && !kBeam) setup(n_gen_early);
   float qbias[3] = {0.f, 0.f, 0.f}, qc[3] = {0.f, 0.f, 0.f};
   if (tid < HD && has_new) {
 #pragma unroll
@@ -777,7 +790,7 @@ static int set_attn_carveout() {
 }
 
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
-                       void *workspace, bool pdl, cudaStream_t s, const int32_t *kv_parent) {
+                       void *workspace, bool pdl, cudaStream_t s, const int32_t *kv_parent, const BeamAnc &beam) {
   VB_CHECK_ARG(kv.head_dim == HD, "attn_decode: head_dim=%d, only 64 is built", kv.head_dim);
   const int cache_cap = kv.kv.cap;
   const int ns = decode_nsplit(B, n_head, cache_cap);
@@ -785,6 +798,10 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
   float *part_o = (float *)workspace;
   float *part_ml = part_o + (size_t)B * n_head * ns * HD;
   dim3 grid(n_head, B, ns);
+  // beam search: the chunk's row table, int16 per row, behind the score buffer of the two-phase kernel (sized as the
+  // kernel sizes it) or alone (single-pass kernel); kBeam instantiations take kShared = true
+  const bool bm = beam.anc != nullptr;
+  const int dl_len = ((cache_cap + ns - 1) / ns + 32 + 15) & ~15;
   if (dtype == VB_E4M3) {
     if (tune("VB_ATTN_DECODE_1PASS", 0) != 0) {
       set_error("attn_decode: VB_ATTN_DECODE_1PASS has no FP8-cache variant");
@@ -798,12 +815,19 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
     constexpr auto k = attn_decode_2phase_pf_kernel<8, uint8_t>;
     VB_TRY(set_attn_carveout<k>());
     VB_CUDA(launch_kernel(k, grid, dim3(128), smem, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
-                          (bf16 *)out16, part_o, part_ml, ns, nullptr));   // no shared prefixes (vb_ar_decode_step)
+                          (bf16 *)out16, part_o, part_ml, ns, nullptr, BeamAnc{}));   // no shared rows (vb_ar_decode_step)
   } else if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
-    const auto k = dtype == VB_F32 ? (kv_parent ? attn_decode_kernel<float, true> : attn_decode_kernel<float>)
-                                   : (kv_parent ? attn_decode_kernel<bf16, true> : attn_decode_kernel<bf16>);
-    VB_CUDA(launch_kernel(k, grid, dim3(128), 0, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
-                          (bf16 *)out16, part_o, part_ml, ns, kv_parent));
+    const auto k = bm ? (dtype == VB_F32 ? attn_decode_kernel<float, true, true> : attn_decode_kernel<bf16, true, true>)
+                      : dtype == VB_F32 ? (kv_parent ? attn_decode_kernel<float, true> : attn_decode_kernel<float>)
+                                        : (kv_parent ? attn_decode_kernel<bf16, true> : attn_decode_kernel<bf16>);
+    VB_CUDA(launch_kernel(k, grid, dim3(128), bm ? dl_len * sizeof(int16_t) : 0, s, pdl, (const float *)kv.q, qkv,
+                          n_head, kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml, ns, kv_parent, beam));
+  } else if (bm) {
+    constexpr auto k_bm = attn_decode_2phase_pf_kernel<4, bf16, true, true>;
+    VB_TRY(set_attn_carveout<k_bm>());
+    VB_CUDA(launch_kernel(k_bm, grid, dim3(128), align_up((size_t)dl_len * (sizeof(float) + sizeof(int16_t)), 1024),
+                          s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml,
+                          ns, kv_parent, beam));
   } else {
     // score buffer: the chunk of one split, rounded as the kernel rounds it (+16), in 1 KB steps
     const size_t sc_bytes = align_up((size_t)((cache_cap + ns - 1) / ns + 32) * sizeof(float), 1024);
@@ -812,7 +836,7 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
     if (kv_parent) VB_TRY(set_attn_carveout<k_sh>());
     else VB_TRY(set_attn_carveout<k>());
     VB_CUDA(launch_kernel(kv_parent ? k_sh : k, grid, dim3(128), sc_bytes, s, pdl, (const float *)kv.q, qkv, n_head,
-                          kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml, ns, kv_parent));
+                          kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml, ns, kv_parent, beam));
   }
   count_launch();
   if (ns > 1) {

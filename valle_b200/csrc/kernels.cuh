@@ -166,23 +166,57 @@ __device__ __forceinline__ int kv_shared_rows(const int32_t *parent, const KvRow
   par = parent[b];
   return par == b ? 0 : (rows.text_len[b] + rows.prompt_len[b]) & ~15;
 }
+// Beam search (vb_ar_state.beam_width > 1): the ancestry table the decode attention follows.  Row b's generated cache
+// row S_b + Tp_b + t, below its current row, lives in the streams of row b - b % width + anc[b * ld + t].
+struct BeamAnc {
+  const uint8_t *anc = nullptr;  // [B, ld]
+  int ld = 0, width = 0;
+};
 // The rows of one (utterance, head) stream as a decode kernel reads them: element offset of row `pos` from the
 // stream's row 0.  kShared = false: the stream's own rows, nothing else is
 // computed.  kShared: rows below `shared` are the parent's, `poff` elements away (the parent's stream minus the own).
-template <bool kShared>
+// kBeam: every row of the CTA's chunk [c0, c0 + n) comes from the stream `dl[pos - c0]` rows away, a table the CTA
+// stages in shared memory once (stage_beam) from the prefix parent (when kv_parent is set) and the ancestry.
+template <bool kShared, bool kBeam = false>
 struct KvStreamRows {
   int64_t poff = 0;
   int shared = 0;
+  const int16_t *dl = nullptr;
+  int c0 = 0;
+  int64_t stride = 0;
   __device__ __forceinline__ KvStreamRows() {}
   __device__ __forceinline__ KvStreamRows(const int32_t *parent, const KvRows &rows, const KvCache &kv, int b) {
-    if constexpr (kShared) {
+    if constexpr (kBeam) {
+      stride = kv.seq_stride;
+    } else if constexpr (kShared) {
       int par;
       shared = kv_shared_rows(parent, rows, b, par);
       poff = (int64_t)(par - b) * kv.seq_stride;
     }
   }
+  // kBeam: row deltas of the chunk [c0, c0 + n) of row b, whose current row is `cur`, into dl_s (shared memory, n
+  // entries), by every thread of the CTA; the caller synchronises the CTA before the first row() call
+  __device__ __forceinline__ void stage_beam(int16_t *dl_s, const int32_t *parent, const KvRows &rows,
+                                             const BeamAnc &ba, int b, int c0_, int n, int cur) {
+    const int gen0 = rows.text_len[b] + rows.prompt_len[b];
+    int pre = 0, pd = 0;
+    if (parent != nullptr) {
+      int par;
+      pre = kv_shared_rows(parent, rows, b, par);
+      pd = par - b;
+    }
+    const int jb = b % ba.width;
+    const uint8_t *a = ba.anc + (int64_t)b * ba.ld;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const int p = c0_ + i;
+      dl_s[i] = (int16_t)(p < pre ? pd : (p >= gen0 && p < cur) ? (int)a[p - gen0] - jb : 0);
+    }
+    dl = dl_s;
+    c0 = c0_;
+  }
   __device__ __forceinline__ int64_t row(int pos) const {
-    if constexpr (kShared) return (int64_t)pos * 64 + (pos < shared ? poff : 0);
+    if constexpr (kBeam) return (int64_t)pos * 64 + (int64_t)dl[pos - c0] * stride;
+    else if constexpr (kShared) return (int64_t)pos * 64 + (pos < shared ? poff : 0);
     else return (int64_t)pos * 64;
   }
 };
@@ -342,8 +376,9 @@ int launch_attention_wgmma(const bf16 *qkv, int64_t M, int n_head, const Packed 
 size_t attn_decode_workspace(int B, int n_head, int head_dim, int cache_cap);
 // the current token's q, k, v (kv.q, or pending in qkv) against the layer's cache kv.kv.  dtype VB_E4M3: the FP8
 // cache; q, k, v must then be pending in qkv.  kv_parent: vb_ar_state.kv_parent (NULL: every row reads its own streams)
+// beam.anc != NULL: the generated rows follow the beam ancestry (bf16 and fp32 caches)
 int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_head, int dtype, float *out, void *out16,
-                       void *workspace, bool pdl, cudaStream_t s, const int32_t *kv_parent);
+                       void *workspace, bool pdl, cudaStream_t s, const int32_t *kv_parent, const BeamAnc &beam);
 
 // decode_fused.cu
 int launch_relu_reduce(const SplitK &in, int B, int N, bf16 *out16, int64_t ldo, bool pdl, cudaStream_t s);
@@ -375,6 +410,9 @@ int launch_cast_from_f32(const float *in, void *out, int dtype, int64_t n, cudaS
 // in: the head projection's pending partials (in.part == NULL: the logits are complete)
 int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const vb_ar_head *head, vb_ar_state *st,
                      int d, const int64_t *forced, int reduce_only, bool pdl, cudaStream_t s);
+// head->greedy == 3: one beam-search step (include/valle_b200.h "Beam search") over the complete logits st->logits,
+// one CTA per group of st->beam_width rows; lse: NULL or [B], each row's log-sum-exp (vb_ar_beam_step)
+int launch_beam_tail(const vb_ar_head *head, vb_ar_state *st, int d, bool pdl, cudaStream_t s, float *lse = nullptr);
 // vb_ar_admit: row i of the k-row state cs <-> row slots[i] of the running state st.  Gather (scatter = false): the
 // lengths and sampler parameters into cs, n_gen / finished / tokens of cs zeroed.  Scatter: n_gen, finished,
 // tokens[., 0], x_cur and logits[., 0:n_vocab] back into the slots

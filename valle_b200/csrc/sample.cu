@@ -262,6 +262,22 @@ __device__ int sample_row(const float (&l)[5], int n, int amax, const RowSampler
   return d;
 }
 
+// log-sum-exp of one row of logits as a 256-thread CTA holds it (element tid + 256 j, -inf padding), mx its maximum:
+// mx + logf(z), z = sum expf(l - mx), each thread's 5 terms in order, a warp sum, then the 8 warps' sums in order.
+// vb_ar_state.logprob and the beam scores both use it.  wz: 8 floats of shared memory.
+__device__ __forceinline__ float row_logsumexp(const float (&lv)[5], float mx, float *wz, int lane, int warp) {
+  float z = 0.f;
+#pragma unroll
+  for (int j = 0; j < 5; ++j) z += expf(lv[j] - mx);
+  z = warp_sum(z);
+  if (lane == 0) wz[warp] = z;
+  __syncthreads();
+  z = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) z += wz[w];
+  return mx + logf(z);
+}
+
 template <bool kSample, bool kScore = false>
 __global__ void __launch_bounds__(256)
 ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__restrict__ partials, int splits,
@@ -353,18 +369,8 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
     best = block_argmax(best, wbest);
     draw = sample_row(lv, n_vocab, best.i, rs, smp);
     if constexpr (kScore) {
-      // sum of expf(l_i - max) (a padding entry is -inf: 0), the 8 warps' sums added in order
       __shared__ float wz[8];
-      float z = 0.f;
-#pragma unroll
-      for (int j = 0; j < 5; ++j) z += expf(lv[j] - best.v);
-      z = warp_sum(z);
-      if (lane == 0) wz[warp] = z;
-      __syncthreads();
-      z = 0.f;
-#pragma unroll
-      for (int w = 0; w < 8; ++w) z += wz[w];
-      lse = best.v + logf(z);
+      lse = row_logsumexp(lv, best.v, wz, lane, warp);
     }
   } else {
     best = warp_argmax(best);
@@ -428,6 +434,241 @@ int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const v
                         (const int32_t *)st->prompt_len, (const int32_t *)st->max_new, st->n_gen, st->finished,
                         st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, in.fold, in.bias, sa,
                         score ? st->logprob : nullptr));
+  count_launch();
+  return VB_OK;
+}
+
+// ---- beam search tail (include/valle_b200.h "Beam search"), one CTA of 256 threads per group of n <= 16 rows.
+// The ranking (c desc, l desc, j asc, v asc) restricted to one row j is (l desc, v asc): c = fl(s_j + fl(l - lse_j)) is
+// non-decreasing in l.  So each row's 2n best by order_key (warp per row) hold the group's 2n best, which hold the n
+// first non-EOS candidates (a row has one EOS candidate) and every candidate of rank < n; warp 0 merges the rows'
+// sorted lists into the group's ranking.
+constexpr int kBeamMax = 16;
+struct BeamCand {
+  float c, l;
+  int v;
+};
+// -0 ranks as +0 (the ranking compares values)
+__device__ __forceinline__ uint32_t rank_key(float f) { return float_key(f == 0.f ? 0.f : f); }
+
+__global__ void __launch_bounds__(256)
+ar_beam_kernel(const float *__restrict__ logits, int64_t ld_logits, int n_vocab, int eos_id, int n,
+               const float *__restrict__ audio_emb, const float *__restrict__ alpha, const float *__restrict__ pe,
+               int pe_rows, const int32_t *__restrict__ prompt_len, const int32_t *__restrict__ max_new,
+               int32_t *__restrict__ n_gen, int32_t *__restrict__ finished, int32_t *__restrict__ tokens,
+               int tok_stride, float *__restrict__ x_cur, int d, uint8_t *__restrict__ anc,
+               float *__restrict__ score, float *__restrict__ fin_score, int32_t *__restrict__ fin_len,
+               uint8_t *__restrict__ fin_anc, float *__restrict__ lse_out) {
+  __shared__ ArgMax wbest[8];
+  __shared__ float wz[8];
+  __shared__ float lse[kBeamMax];
+  __shared__ BeamCand cand[kBeamMax][2 * kBeamMax];
+  __shared__ int ranked[2 * kBeamMax];                       // j * 2n + index in row j's list
+  __shared__ int npar[kBeamMax], ntok[kBeamMax];
+  __shared__ float nsc[kBeamMax];
+  __shared__ int s_stop, s_fpar, s_len, s_from_fin;
+  const int g = blockIdx.x, r0 = g * n, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int K = 2 * n;
+  pdl_launch_dependents();
+  pdl_wait();
+  if (finished[r0] != 0) {   // a stopped group rides along with fixed input rows, as ar_sample_kernel's rows do
+    for (int j = 0; j < n; ++j) {
+      float *xo = x_cur + (int64_t)(r0 + j) * d;
+      for (int c = tid * 4; c < d; c += 1024) *reinterpret_cast<float4 *>(xo + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    return;
+  }
+  const int t = n_gen[r0];
+  const bool cap = t > max_new[r0] || t >= tok_stride;
+  if (!cap) {
+    // every row's log-sum-exp, as the logprob path computes it
+    for (int j = 0; j < n; ++j) {
+      const float *row = logits + (int64_t)(r0 + j) * ld_logits;
+      float lv[5];
+      ArgMax best{-CUDART_INF_F, 0x7fffffff};
+#pragma unroll
+      for (int q = 0; q < 5; ++q) {
+        const int i = tid + q * 256;
+        lv[q] = i < n_vocab ? row[i] : -CUDART_INF_F;
+        if (i < n_vocab) best = better(best, ArgMax{lv[q], i});
+      }
+      best = block_argmax(best, wbest);
+      const float l = row_logsumexp(lv, best.v, wz, lane, warp);
+      if (tid == 0) {
+        lse[j] = l;
+        if (lse_out != nullptr) lse_out[r0 + j] = l;
+      }
+    }
+    __syncthreads();
+    // each row's K best (l desc, v asc), one warp per row, the row in registers (element lane + 32 q)
+    for (int j = warp; j < n; j += 8) {
+      const float *row = logits + (int64_t)(r0 + j) * ld_logits;
+      float x[40];
+#pragma unroll
+      for (int q = 0; q < 40; ++q) x[q] = lane + 32 * q < n_vocab ? row[lane + 32 * q] : 0.f;
+      uint64_t taken = 0;
+      auto mine = [&]() {
+        unsigned long long k = 0;
+#pragma unroll
+        for (int q = 0; q < 40; ++q) {
+          const int v = lane + 32 * q;
+          const unsigned long long kq = ((unsigned long long)rank_key(x[q]) << 32) | (0xFFFFFFFFu - (uint32_t)v);
+          if (v < n_vocab && !((taken >> q) & 1) && kq > k) k = kq;
+        }
+        return k;
+      };
+      unsigned long long km = mine();
+      const float sj = score[r0 + j], lj = lse[j];
+      for (int r = 0; r < K; ++r) {
+        unsigned long long w = km;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const unsigned long long ow = __shfl_xor_sync(0xffffffffu, w, o);
+          w = ow > w ? ow : w;
+        }
+        const int v = (int)(0xFFFFFFFFu - (uint32_t)w);
+        if (lane == (v & 31)) {
+          taken |= 1ull << (v >> 5);
+          km = mine();
+        }
+        if (lane == 0) {
+          const float l = key_float((uint32_t)(w >> 32));
+          cand[j][r] = BeamCand{__fadd_rn(sj, __fsub_rn(l, lj)), l, v};
+        }
+      }
+    }
+    __syncthreads();
+    // the group's K best: merge of the rows' sorted lists (c desc, l desc; ties to the smaller j)
+    if (warp == 0) {
+      int idx = 0;
+      for (int r = 0; r < K; ++r) {
+        unsigned long long w = 0;
+        if (lane < n && idx < K) {
+          const BeamCand &c = cand[lane][idx];
+          w = ((unsigned long long)rank_key(c.c) << 32) | rank_key(c.l);
+        }
+        int wl = lane;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const unsigned long long ow = __shfl_xor_sync(0xffffffffu, w, o);
+          const int ol = __shfl_xor_sync(0xffffffffu, wl, o);
+          if (ow > w || (ow == w && ol < wl)) {
+            w = ow;
+            wl = ol;
+          }
+        }
+        if (lane == wl) {
+          ranked[r] = lane * K + idx;
+          ++idx;
+        }
+      }
+    }
+    __syncthreads();
+  }
+  if (tid == 0) {
+    float fc = fin_score[2 * g], fo = fin_score[2 * g + 1];
+    int fpar = -1, stop = 1, from_fin = 0, len = t;
+    if (cap) {
+      from_fin = fc > -CUDART_INF_F && fc >= score[r0];
+    } else {
+      int live = 0;
+      for (int r = 0; r < K && live < n; ++r) {
+        const int j = ranked[r] / K;
+        const BeamCand c = cand[j][ranked[r] % K];
+        if (c.v == eos_id) {
+          if (r < n && c.c > fc) {
+            fc = c.c;
+            fo = score[r0 + j];
+            fpar = j;
+          }
+        } else {
+          npar[live] = j;
+          ntok[live] = c.v;
+          nsc[live] = c.c;
+          ++live;
+        }
+      }
+      if (fpar >= 0) {
+        fin_score[2 * g] = fc;
+        fin_score[2 * g + 1] = fo;
+        fin_len[g] = t;
+      }
+      stop = fc > -CUDART_INF_F && fc >= nsc[0];
+      from_fin = stop;
+    }
+    if (stop) {
+      len = from_fin ? (fpar >= 0 ? t : fin_len[g]) : t;
+      score[r0] = from_fin ? fo : score[r0];
+    }
+    s_stop = stop;
+    s_fpar = fpar;
+    s_len = len;
+    s_from_fin = from_fin;
+  }
+  __syncthreads();
+  const int stop = s_stop, fpar = s_fpar;
+  const int64_t ld = tok_stride;
+  // ancestry pass, thread per position: the n rows' old entries, then the finished hypothesis's copy and (going on)
+  // the new beams' entries
+  for (int i = tid; i < t && (fpar >= 0 || !stop); i += 256) {
+    unsigned long long lo = 0, hi = 0;
+    for (int j = 0; j < n; ++j) {
+      const unsigned long long a = anc[(r0 + j) * ld + i];
+      if (j < 8) lo |= a << (8 * j);
+      else hi |= a << (8 * (j - 8));
+    }
+    auto old = [&](int j) { return (uint8_t)(((j < 8) ? lo : hi) >> (8 * (j & 7))); };
+    if (fpar >= 0) fin_anc[g * ld + i] = old(fpar);
+    if (!stop)
+      for (int k = 0; k < n; ++k) anc[(r0 + k) * ld + i] = old(npar[k]);
+  }
+  if (stop) {
+    __syncthreads();   // fin_anc is complete
+    const int len = s_len;
+    const uint8_t *src = s_from_fin ? fin_anc + g * ld : anc + r0 * ld;
+    for (int i = tid; i < len; i += 256) tokens[r0 * ld + i] = tokens[(r0 + src[i]) * ld + i];
+    for (int j = 0; j < n; ++j) {
+      float *xo = x_cur + (int64_t)(r0 + j) * d;
+      for (int c = tid * 4; c < d; c += 1024) *reinterpret_cast<float4 *>(xo + c) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    if (tid < n) finished[r0 + tid] = len == 0 ? 2 : 1;
+    if (tid == 0) n_gen[r0] = len;
+    return;
+  }
+  if (tid < n) {
+    anc[(r0 + tid) * ld + t] = (uint8_t)tid;
+    tokens[(r0 + tid) * ld + t] = ntok[tid];
+    score[r0 + tid] = nsc[tid];
+    n_gen[r0 + tid] = t + 1;
+  }
+  // the new beams' input rows: embedding + alpha * PE, as ar_sample_kernel
+  const float a = alpha[0];
+  const float *p = pe + (int64_t)min(prompt_len[r0] + t, pe_rows - 1) * d;
+  for (int k = 0; k < n; ++k) {
+    const float *e = audio_emb + (int64_t)ntok[k] * d;
+    float *xo = x_cur + (int64_t)(r0 + k) * d;
+    for (int c = tid * 4; c < d; c += 1024) {
+      const float4 ev = *reinterpret_cast<const float4 *>(e + c);
+      const float4 pv = *reinterpret_cast<const float4 *>(p + c);
+      float4 o;
+      o.x = __fadd_rn(ev.x, __fmul_rn(a, pv.x));
+      o.y = __fadd_rn(ev.y, __fmul_rn(a, pv.y));
+      o.z = __fadd_rn(ev.z, __fmul_rn(a, pv.z));
+      o.w = __fadd_rn(ev.w, __fmul_rn(a, pv.w));
+      *reinterpret_cast<float4 *>(xo + c) = o;
+    }
+  }
+}
+
+int launch_beam_tail(const vb_ar_head *head, vb_ar_state *st, int d, bool pdl, cudaStream_t s, float *lse) {
+  const int n = st->beam_width;
+  VB_CHECK_ARG(head->n_vocab <= 40 * 32 && 2 * n <= head->n_vocab, "beam tail: n_vocab %d not in [2n, 1280]",
+               head->n_vocab);
+  const int64_t ldl = (head->n_vocab + 3) & ~3;
+  VB_CUDA(launch_kernel(ar_beam_kernel, dim3(st->B / n), dim3(256), 0, s, pdl, (const float *)st->logits, ldl,
+                        head->n_vocab, head->eos_id, n, head->audio_emb, head->alpha, head->pe, head->pe_rows,
+                        st->prompt_len, st->max_new, st->n_gen, st->finished, st->tokens, st->tok_stride, st->x_cur, d,
+                        st->beam_anc, st->beam_score, st->beam_fin_score, st->beam_fin_len, st->beam_fin_anc, lse));
   count_launch();
   return VB_OK;
 }

@@ -126,6 +126,13 @@ class _ArBuffers:
         #: state points at them only in calls that use them (set_best_of)
         self.kv_parent = torch.zeros(B, **i32)
         self.logprob = torch.zeros(B, dtype=torch.float32, device=dev)
+        #: beam search (include/valle_b200.h "Beam search"): each row's ancestry and score, and each group's finished
+        #: hypothesis (rows [0, B / n) of the fin arrays); the state points at them only in beam calls (set_best_of)
+        self.beam_anc = torch.zeros((B, tok_stride), dtype=torch.uint8, device=dev)
+        self.beam_score = torch.zeros(B, dtype=torch.float32, device=dev)
+        self.beam_fin_score = torch.zeros((B, 2), dtype=torch.float32, device=dev)
+        self.beam_fin_len = torch.zeros(B, **i32)
+        self.beam_fin_anc = torch.zeros((B, tok_stride), dtype=torch.uint8, device=dev)
         st = L.ArState()
         st.B, st.tok_stride = B, tok_stride
         st.text_len, st.prompt_len, st.max_new = self.text_len.data_ptr(), self.prompt_len.data_ptr(), self.max_new.data_ptr()
@@ -145,11 +152,23 @@ class _ArBuffers:
         self.graphs: Dict[tuple, Tuple[torch.cuda.CUDAGraph, int, L.ArHead]] = {}
         self.eng = eng
 
-    def set_best_of(self, n_rows: int, n: int, scores: bool):
+    def set_best_of(self, n_rows: int, n: int, scores: bool, beams: bool = False):
         """Point the state at kv_parent when n > 1 (row r of the first n_rows reads its parent r - r % n's prompt
         prefix) and at logprob, zeroed, with scores; leave either NULL otherwise.  The FP8 cache keeps kv_parent NULL:
         there the shared read is slower than every row reading its own copy (DESIGN section 7), and the codes are
-        the same either way."""
+        the same either way.  beams: the rows are groups of n beams (beam search), whose arrays the state then points
+        at, set to their starting values; otherwise beam search is off."""
+        st = self.st
+        st.beam_width, st.beam_anc, st.beam_score, st.beam_fin_score, st.beam_fin_len, st.beam_fin_anc = \
+            0, None, None, None, None, None
+        if beams:
+            r = torch.arange(n_rows, device=self.beam_score.device)
+            self.beam_score[:n_rows] = torch.where(r % n == 0, 0.0, float("-inf"))
+            self.beam_fin_score[:, 0] = float("-inf")
+            st.beam_width = n
+            st.beam_anc, st.beam_score = self.beam_anc.data_ptr(), self.beam_score.data_ptr()
+            st.beam_fin_score, st.beam_fin_len = self.beam_fin_score.data_ptr(), self.beam_fin_len.data_ptr()
+            st.beam_fin_anc = self.beam_fin_anc.data_ptr()
         self.st.kv_parent = None
         if n > 1 and self.kv_dtype is None:
             r = torch.arange(n_rows, dtype=torch.int32)
@@ -333,6 +352,29 @@ def _check_num_samples(n, seed, return_scores: bool, trace, forced, sample_on_ho
         raise ValueError("return_scores scores the seeded draws; forced ids replace them")
     if bf16_rows is not None and n > bf16_rows:
         raise ValueError(f"num_samples={n}: a bf16 decode group holds at most {bf16_rows} candidates of one utterance")
+    return n
+
+
+def _check_num_beams(n, seed, top_k, top_p, ras, num_samples, trace, forced, sample_on_host: bool, fp8: bool) -> int:
+    """Validated beam width of generate(): an int in [1, 16].  n > 1 searches by the AR log-likelihood alone, so it
+    excludes every sampler argument (seed, top_k != 1, top_p, ras), best-of-n, host sampling, the trace / forced test
+    hooks and the FP8 KV cache."""
+    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or not 1 <= n <= 16:
+        raise ValueError(f"num_beams must be an int in [1, 16] (got {n!r})")
+    n = int(n)
+    if n == 1:
+        return n
+    if seed is not None or ras is not None or (_is_seq(top_k) or int(top_k) != 1) or \
+            (_is_seq(top_p) or float(top_p) != 1.0):
+        raise ValueError("num_beams > 1 ranks by the AR log-likelihood: it takes no seed, top_k, top_p or ras")
+    if isinstance(num_samples, bool) or not isinstance(num_samples, (int, np.integer)) or num_samples != 1:
+        raise ValueError("num_beams > 1 cannot be combined with num_samples")
+    if sample_on_host:
+        raise ValueError("num_beams > 1 searches on the device; it cannot be combined with sample_on_host = True")
+    if trace is not None or forced is not None:
+        raise ValueError("num_beams > 1 cannot be combined with the trace / forced test hooks")
+    if fp8:
+        raise ValueError("num_beams > 1 is not supported on the FP8 KV cache")
     return n
 
 
@@ -543,7 +585,7 @@ class ValleEngine:
                  max_new_tokens=None, poll: int = 32,
                  return_device: bool = False, trace: Optional[dict] = None,
                  forced: Optional[Sequence[torch.Tensor]] = None, seed=None, top_p=1.0,
-                 ras=None, num_samples: int = 1, return_scores: bool = False):
+                 ras=None, num_samples: int = 1, return_scores: bool = False, num_beams: int = 1):
         """texts[b]: int64 [S_b] phoneme ids; prompts[b]: int64 [Tp_b, Q] codec ids (host or device).
         Returns codes[b]: int64 [Tgen_b, Q] -- per utterance exactly what VALLE.inference returns.
 
@@ -572,6 +614,15 @@ class ValleEngine:
         candidate, the sum over its first-codebook codes of log_softmax(raw logits)[code] (before temperature, top-k
         and top-p), accumulated in fp32 on the device.
 
+        Beam search: num_beams=n > 1 (an int in [1, 16]; no seed, top_k, top_p, ras, num_samples, host sampling, test
+        hooks or FP8 KV cache) keeps the n most likely first-codebook hypotheses of each utterance and returns one [T, Q]
+        code matrix per utterance, its first codebook the winning hypothesis, the NAR run once on it; include/
+        valle_b200.h "Beam search" states the ranking and the exact stop rule (no length normalisation).
+        return_scores=True returns (codes, scores [B] fp32), the winner's AR log-likelihood over its codes.  The n
+        beams of an utterance are n decode rows that read one copy of the prompt prefix, and the batch caveat of
+        best-of-n applies: in bf16 a decode group holds floor(64 / n) whole utterances; with VB_DECODE_NSPLIT fixed an
+        utterance's result does not depend on its batch.  num_beams=1 runs the default path.
+
         Test hooks: `trace` collects AR logits (trace["steps"] = set of iterations or "all") and, with
         trace["nar"] = True, the NAR logits / argmax of every stage; `forced[b]` = int64 [T_b, Q] codes the decode is
         teacher-forced with (every sampled id is replaced by the given one before it is appended, AR and NAR), so
@@ -581,12 +632,19 @@ class ValleEngine:
         if B < 1 or len(prompts) != B:
             raise ValueError(f"generate: {B} texts and {len(prompts)} prompts (one of each per utterance, >= 1)")
         bf16 = self.dtype == torch.bfloat16
-        n = _check_num_samples(num_samples, seed, return_scores, trace, forced, self.sample_on_host,
-                               self.max_tc_batch if bf16 else None)
+        beams = _check_num_beams(num_beams, seed, top_k, top_p, ras, num_samples, trace, forced, self.sample_on_host,
+                                 self.kv_cache_dtype() is not None) > 1
+        if beams:
+            n = int(num_beams)
+        else:
+            n = _check_num_samples(num_samples, seed, return_scores, trace, forced, self.sample_on_host,
+                                   self.max_tc_batch if bf16 else None)
         if n > 1:
-            seed, per, ras = _candidates(B, n, seed, dict(texts=texts, prompts=prompts, enroll_lens=enroll_lens,
-                                                          max_new_tokens=max_new_tokens, top_k=top_k,
-                                                          temperature=temperature, top_p=top_p), ras)
+            seeds, per, ras = _candidates(B, n, 0 if beams else seed,
+                                          dict(texts=texts, prompts=prompts, enroll_lens=enroll_lens,
+                                               max_new_tokens=max_new_tokens, top_k=top_k,
+                                               temperature=temperature, top_p=top_p), ras)
+            seed = None if beams else seeds
             texts, prompts, enroll_lens, max_new_tokens = (per[k] for k in ("texts", "prompts", "enroll_lens",
                                                                             "max_new_tokens"))
             top_k, temperature, top_p = per["top_k"], per["temperature"], per["top_p"]
@@ -609,8 +667,8 @@ class ValleEngine:
             _check_top_p([top_p])
         if not (rows > self.max_tc_batch and bf16 and trace is None and forced is None):
             outs, scores = self._generate(texts, prompts, enroll_lens, draws, top_k, temperature, top_p,
-                                          max_new_tokens, poll, return_device, trace, forced, n, return_scores)
-            return self._best_of(outs, scores, B, n, return_scores, return_device)
+                                          max_new_tokens, poll, return_device, trace, forced, n, return_scores, beams)
+            return self._best_of(outs, scores, B, n, return_scores, return_device, beams)
         # the tensor-core decode projections take up to 64 rows (one UMMA N tile): a larger batch is decoded as
         # consecutive groups of <= 64 rows instead of falling onto the CUDA-core GEMV path; a group holds whole
         # utterances, all n candidates of each
@@ -624,7 +682,7 @@ class ValleEngine:
             mnt = max_new_tokens[b0:b1] if _is_seq(max_new_tokens) else max_new_tokens
             o, sc = self._generate(texts[b0:b1], prompts[b0:b1], None if enroll_lens is None else enroll_lens[b0:b1],
                                    None if draws is None else draws[b0:b1], top_k, temperature, top_p, mnt, poll,
-                                   return_device, num_samples=n, scores=return_scores)
+                                   return_device, num_samples=n, scores=return_scores, beams=beams)
             outs += o
             scores.append(sc)
             stats.ar_steps += self.stats.ar_steps
@@ -634,27 +692,30 @@ class ValleEngine:
             packed.append(self.last_packed)
         self.stats = stats
         self.last_packed = torch.cat(packed) if return_device else None
-        return self._best_of(outs, torch.cat(scores) if return_scores else None, B, n, return_scores, return_device)
+        return self._best_of(outs, torch.cat(scores) if return_scores else None, B, n, return_scores, return_device,
+                             beams)
 
     @staticmethod
     def _best_of(outs: List[torch.Tensor], scores: Optional[torch.Tensor], B: int, n: int, return_scores: bool,
-                 return_device: bool):
+                 return_device: bool, beams: bool = False):
         """generate()'s result from the codes of its B * n rows and their scores: the rows grouped per utterance when
-        n > 1, and (codes, scores [B, n]) with return_scores"""
-        codes = outs if n == 1 else [outs[b * n:(b + 1) * n] for b in range(B)]
+        n > 1, and (codes, scores [B, n]) with return_scores.  beams: outs and scores hold one entry per utterance
+        already (scores [B])."""
+        codes = outs if n == 1 or beams else [outs[b * n:(b + 1) * n] for b in range(B)]
         if not return_scores:
             return codes
-        scores = scores.view(B, n)
+        scores = scores.view(B) if beams else scores.view(B, n)
         return codes, scores if return_device else scores.cpu()
 
     def _generate(self, texts, prompts, enroll_lens, draws: Optional[List[_Draw]], top_k, temperature, top_p,
                   max_new_tokens, poll: int, return_device: bool, trace: Optional[dict] = None,
                   forced: Optional[Sequence[torch.Tensor]] = None, num_samples: int = 1,
-                  scores: bool = False) -> Tuple[List[torch.Tensor], Optional[torch.Tensor]]:
+                  scores: bool = False, beams: bool = False) -> Tuple[List[torch.Tensor], Optional[torch.Tensor]]:
         """generate() of one group of utterances with validated sampler arguments: draws (the seeded device sampler), or
         None and top_k / temperature / top_p (greedy, or torch's sampler).  num_samples > 1: the rows are the
         candidates of B / num_samples utterances, num_samples consecutive rows each, which decode reading their first row's prompt prefix.  Returns the
-        codes and, with scores (seeded draws only), the rows' AR log-likelihoods on the device."""
+        codes and, with scores (seeded draws only), the rows' AR log-likelihoods on the device.  beams: the rows are
+        the beams of B / num_samples utterances (beam search); returns one code matrix and score per utterance."""
         m, dev, Q = self.model, self.device, self.Q
         B = len(texts)
         kv_dtype = self.kv_cache_dtype()
@@ -690,10 +751,10 @@ class ValleEngine:
         buf.load_rows(p, draws if native else None)
         buf.n_gen.zero_()
         buf.finished.zero_()
-        buf.set_best_of(B, num_samples, scores)
+        buf.set_best_of(B, num_samples, scores and not beams, beams)
         pe_a = self._pe(m.ar_audio_position, max(p.Tp) + max(cap_new) + 2)
         h_last = self._prefill(buf, p, pe_a)
-        head = self._head(pe_a, 2 if native else int(greedy))
+        head = self._head(pe_a, 3 if beams else 2 if native else int(greedy))
         self._head_ref = head
         L.check(self.lib.vb_ar_head_step(self.ar.handle, C.byref(head), h_last.data_ptr(), C.byref(buf.st),
                                          buf.ws.data_ptr(), buf.ws.numel(), L.stream_ptr()), "vb_ar_head_step")
@@ -716,8 +777,11 @@ class ValleEngine:
         # ---- AR decode loop (valle.py:1012-1057) ----
         max_steps = max(cap_new) + 1     # the stop rule has fired in every row by then
         steps = 0
-        running = dict(enumerate(utts))
-        Tg = [0] * B
+        # beam search: the first row of each group stands for its utterance (it receives the result)
+        rows = list(range(0, B, num_samples)) if beams else list(range(B))
+        utts = [utts[r] for r in rows]
+        running = dict(zip(rows, utts))
+        Tg_row = {}
         while running and steps < max_steps:
             n = min(poll, max_steps - steps)
             if (greedy or native) and self.use_cuda_graph:
@@ -734,14 +798,18 @@ class ValleEngine:
             if trace is not None and want(steps):  # poll == 1 here: the logits row of iteration `steps`
                 trace["ar_logits"][steps] = buf.logits[:, : self.n_vocab].clone()
             for b, n_b in self._stopped(buf, running).items():
-                Tg[b] = n_b
+                Tg_row[b] = n_b
                 del running[b]
+        Tg = [Tg_row.get(r, 0) for r in rows]
         self.stats.ar_steps = steps
-        logprob = buf.logprob[:B].clone() if scores else None
+        if beams:
+            logprob = buf.beam_score[rows].clone() if scores else None
+        else:
+            logprob = buf.logprob[:B].clone() if scores else None
         ev[2].record()
 
         # ---- NAR (valle.py:1059-1137) ----
-        src = torch.from_numpy(_seg_ranges(np.arange(B, dtype=np.int64) * tok_stride, Tg)[0]).to(dev)
+        src = torch.from_numpy(_seg_ranges(np.asarray(rows, dtype=np.int64) * tok_stride, Tg)[0]).to(dev)
         fc = None
         if forced is not None:
             fc = torch.cat([forced[b][: Tg[b]].to(torch.int64) for b in range(B)]).to(dev)
@@ -758,9 +826,9 @@ class ValleEngine:
         #: as is instead of re-packing the views)
         self.last_packed = codes
         if return_device:
-            return [codes[cu_g[b]:cu_g[b + 1]] for b in range(B)], logprob
+            return [codes[cu_g[b]:cu_g[b + 1]] for b in range(len(rows))], logprob
         host = codes.cpu()
-        return [host[cu_g[b]:cu_g[b + 1]] for b in range(B)], logprob
+        return [host[cu_g[b]:cu_g[b + 1]] for b in range(len(rows))], logprob
 
     def generate_stream(self, requests: Iterable, slots: Optional[int] = None, max_context: Optional[int] = None,
                         poll: int = 32, nar_batch: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor]]:
@@ -1064,7 +1132,7 @@ class ValleEngine:
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
         draw mode, shared prefixes, scores, k))"""
         key = (head.pe, head.predict_w, head.audio_emb, head.greedy, buf.kv_dtype, bool(buf.st.kv_parent),
-               bool(buf.st.logprob), k)
+               bool(buf.st.logprob), buf.st.beam_width, k)
         graphs = buf.graphs
         ent = graphs.get(key)
         if ent is None:

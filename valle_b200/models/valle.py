@@ -212,13 +212,14 @@ class VALLE(nn.Module):
     def inference(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor,
                   enroll_x_lens: Optional[torch.Tensor] = None, top_k: int = -100,
                   temperature: float = 1.0, max_new_tokens: Optional[int] = None, seed: Optional[int] = None,
-                  top_p: float = 1.0, ras=None) -> torch.Tensor:
+                  top_p: float = 1.0, ras=None, num_beams: int = 1) -> torch.Tensor:
         """x: (1, S) phoneme ids, x_lens: (1,), y: (1, T, 8) acoustic prompt.
         Returns the predicted audio code matrix (1, T', 8) -- same contract as the reference.
         seed: None samples with torch's generator as the reference does; an int in [0, 2**64) draws with the seeded
         device sampler inside the CUDA-graph decode step (ValleEngine.generate), reproducible from the seed alone.
         top_p: nucleus filtering after top-k, in (0, 1]; ras: repetition-aware sampling, a (window, threshold) pair
-        (needs seed); see ValleEngine.generate."""
+        (needs seed); see ValleEngine.generate.  num_beams=n > 1: beam search over the first codebook instead of
+        sampling (top_k left at its default, no seed / top_p / ras), the NAR run on the winning hypothesis."""
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
@@ -226,9 +227,11 @@ class VALLE(nn.Module):
         assert torch.all(x_lens > 0)
         S = int(x_lens.max())
         enroll = [int(enroll_x_lens.max())] if (self.prefix_mode in (2, 4) and enroll_x_lens is not None) else None
+        if num_beams != 1 and top_k == -100:   # the reference's sampling default: beam search draws nothing
+            top_k = 1
         out = self.engine().generate([x[0, :S]], [y[0]], enroll_lens=enroll, top_k=top_k,
                                      temperature=temperature, max_new_tokens=max_new_tokens,
-                                     return_device=True, seed=seed, top_p=top_p, ras=ras)
+                                     return_device=True, seed=seed, top_p=top_p, ras=ras, num_beams=num_beams)
         return out[0].unsqueeze(0).to(y.device)
 
     @torch.no_grad()
@@ -236,7 +239,8 @@ class VALLE(nn.Module):
                         enroll_lens: Optional[Sequence[int]] = None, top_k: int = 1,
                         temperature: float = 1.0, max_new_tokens=None,
                         dtype: Optional[torch.dtype] = None, return_device: bool = False,
-                        seed=None, top_p=1.0, ras=None, num_samples: int = 1, return_scores: bool = False):
+                        seed=None, top_p=1.0, ras=None, num_samples: int = 1, return_scores: bool = False,
+                        num_beams: int = 1):
         """Engine feature (the reference asserts batch 1, valle.py:989): B independent utterances
         decoded together; result[b] equals `inference()` on utterance b alone.  Codes come back on the host, or
         (return_device=True) stay on the GPU, e.g. for the data-parallel gather of valle_b200.dist.
@@ -244,11 +248,14 @@ class VALLE(nn.Module):
         `inference(..., seed=s + b)`; top_k, temperature and top_p may be per-utterance sequences, and ras one
         (window, threshold) pair or one per utterance (ValleEngine.generate).  max_new_tokens: one int or one per
         utterance.  Best-of-n (seeded calls): num_samples=n draws n candidates per utterance, result[b][j], and
-        return_scores=True returns (codes, [B, n] AR log-likelihoods) (ValleEngine.generate)."""
+        return_scores=True returns (codes, [B, n] AR log-likelihoods) (ValleEngine.generate).  Beam search:
+        num_beams=n > 1 returns one code matrix per utterance, the most likely first codebook the search finds, and
+        with return_scores its [B] AR log-likelihood (ValleEngine.generate)."""
         return self.engine(dtype).generate(texts, prompts, enroll_lens=enroll_lens, top_k=top_k,
                                            temperature=temperature, max_new_tokens=max_new_tokens,
                                            return_device=return_device, seed=seed, top_p=top_p, ras=ras,
-                                           num_samples=num_samples, return_scores=return_scores)
+                                           num_samples=num_samples, return_scores=return_scores,
+                                           num_beams=num_beams)
 
     def inference_stream(self, requests, slots: Optional[int] = None, max_context: Optional[int] = None,
                          poll: int = 32, nar_batch: Optional[int] = None, dtype: Optional[torch.dtype] = None):
