@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 14
+#define VB_ABI_VERSION 15
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
@@ -364,11 +364,12 @@ typedef struct vb_ar_state {
    * text_len, prompt_len and max_new, its rows' caches prefilled alike), row j of a group holding beam j.  Generated
    * position t of a hypothesis is a token tokens[r, t] and the cache rows S_b + Tp_b + t of row r's streams, r being the
    * group's row named by the hypothesis's ancestry entry for t; each such entry is written once, by the beam that held
-   * row r at step t.  vb_ar_admit and continuous batching use none of these fields.
-   *   Decode attention (beam_width > 1, vb_ar_decode_step): row b reads its generated cache rows
-   *   [S_b + Tp_b, current row) from the streams of row b - b % n + beam_anc[b, row - S_b - Tp_b], the rows below P_b
-   *   from kv_parent (when set), every other row from its own streams; bitwise the step whose rows sit in row b's own
-   *   streams.  bf16 and fp32 caches only: with kv_dtype == VB_E4M3 the step returns VB_ERR_UNSUPPORTED.
+   * row r at step t.  vb_ar_admit uses these fields only with per-row groups (beam_first, below).
+   *   Decode attention (beam_width > 1, or beam_first set; vb_ar_decode_step): row b reads its generated cache rows
+   *   [S_b + Tp_b, current row) from the streams of row g_b + beam_anc[b, row - S_b - Tp_b], g_b the first row of b's
+   *   group (b - b % n, or beam_first[b]), the rows below P_b from kv_parent (when set), every other row from its own
+   *   streams; bitwise the step whose rows sit in row b's own streams.  bf16 and fp32 caches only: with
+   *   kv_dtype == VB_E4M3 the step returns VB_ERR_UNSUPPORTED.
    *   Beam tail (vb_ar_head.greedy == 3, vb_ar_head_step and vb_ar_decode_step; beam_width in [1, 16]): see "Beam
    *   search" below vb_ar_head. */
   int32_t beam_width;          /* n, or 0 */
@@ -380,6 +381,16 @@ typedef struct vb_ar_state {
                                   score over its codes */
   int32_t *beam_fin_len;       /* [B / n] the finished hypothesis's length */
   uint8_t *beam_fin_anc;       /* [B / n, tok_stride] the finished hypothesis's ancestry */
+  /* per-row beam groups (ABI 15; vb_ar_head.greedy == 4 only): beam groups of any width decoding next to rows in no
+   * group, as continuous batching admits them.  NULL means off, so a zero-initialised tail decodes as before.  Set
+   * together with greedy == 4 (either without the other, or with beam_width > 1: VB_ERR_ARG), with beam_anc and the
+   * beam arrays above, which then have B rows: beam_fin_* of a group are indexed by its first row.  A group is n
+   * contiguous rows [g, g + n), n in [2, 16], anywhere in [0, B): beam_first[r] = g and beam_n[r] = n for each of
+   * them; a row in no group has beam_first = -1 (beam_n ignored).  vb_ar_head_step, vb_ar_beam_step, vb_ar_admit
+   * and vb_ar_decode_step read both arrays back and check them (VB_ERR_ARG) unless the stream is capturing a graph,
+   * where the caller guarantees them.  The FP8 cache refuses them (VB_ERR_UNSUPPORTED), as it refuses beam_width. */
+  const int32_t *beam_first;   /* [B] or NULL */
+  const int32_t *beam_n;       /* [B] */
 } vb_ar_state;
 
 typedef struct vb_ar_head {
@@ -393,7 +404,9 @@ typedef struct vb_ar_head {
   int32_t greedy;             /* 1: argmax + stop rule + append on device; 0: logits only (the caller draws and
                                  calls vb_ar_push_tokens); 2: seeded draw on the device from the state's sampler
                                  arrays (vb_sample_logits_ex, with the row's n_gen as step and its tokens row as
-                                 history), then the stop rule + append as for 1; 3: one beam-search step (below) */
+                                 history), then the stop rule + append as for 1; 3: one beam-search step (below);
+                                 4: the mixed tail: every row in no group as 2, every per-row beam group
+                                 (vb_ar_state.beam_first) one beam-search step as 3, in one launch more than 2 */
   vb_ln_fold fold;            /* final LayerNorm folded into predict_w (all-NULL: separate LayerNorm launch) */
 } vb_ar_head;
 
@@ -416,7 +429,11 @@ typedef struct vb_ar_head {
  *   On the stop, the result's tokens are gathered into tokens[first row, 0..len), its length into that row's n_gen
  *   and its score (the sum over its codes: the EOS term ranks but is not part of it, so n = 1 reports what greedy == 2
  *   with logprob reports) into beam_score[first row]; every row of the group gets finished = 1 (2 for a result of
- *   length 0). */
+ *   length 0).
+ * Per-row groups (vb_ar_head.greedy == 4, vb_ar_state.beam_first): each group g of n = beam_n[g] rows runs the same
+ * step, bit for bit, as it would alone in a state with beam_width = n and greedy == 3, its finished hypothesis at
+ * beam_fin_*[g]; the rows in no group run the seeded sampler tail of greedy == 2, bit for bit.  Its sampler arrays
+ * must be set for every row; a group's rows ignore them. */
 
 /* bytes of scratch for vb_ar_head_step / vb_ar_decode_step.  The buffer must not be shared between
  * concurrently running streams. */
@@ -434,12 +451,19 @@ size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab);
 
 /* Admit k new utterances into rows slots[0..k) (device int32 [k], distinct, in [0, st->B)) of a running state (ABI 10;
  * after their prefill through vb_decoder_forward with cache_slots).  h: fp32 [k, d], the last prefill row of each.
- * On entry the slots' text_len, prompt_len, max_new (and, for head->greedy == 2, the sampler arrays, top_p / ras_*
- * included) hold the new utterances' values.  The call runs vb_ar_head_step on a k-row state built from those rows, with n_gen = 0 and
- * finished = 0, so admitted row i gets exactly what vb_ar_head_step on a fresh k-row state gives its row i.
+ * On entry the slots' text_len, prompt_len, max_new (and, for head->greedy == 2 or 4, the sampler arrays, top_p /
+ * ras_* included, and for 4 beam_first / beam_n) hold the new utterances' values.  The call runs vb_ar_head_step on a
+ * k-row state built from those rows, with n_gen = 0 and finished = 0, so admitted row i gets exactly what
+ * vb_ar_head_step on a fresh k-row state gives its row i.
  * Writes, for the slots only: n_gen, finished, tokens[slot, 0], x_cur[slot, :] and logits[slot, 0:n_vocab].  Every other
  * row of every array, the slots' other entries and the KV cache are left unchanged.  No host reads: safe to capture in
- * a CUDA graph. */
+ * a CUDA graph (with per-row groups: when not capturing, the groups and slots are read back and checked).
+ * Beam groups (ABI 15, head->greedy == 4): the slots of a group g of n rows are passed together and in order,
+ * slots[i..i+n) = g..g+n-1.  Its rows get what vb_ar_head_step with greedy == 3 gives on a fresh state holding the
+ * group alone: beam_score 0 for row g and -inf for the others, beam_fin_score[g, 0] = -inf, n_gen = finished = 0,
+ * then step t = 0, which writes tokens[., 0], beam_anc[., 0], beam_score and x_cur (and beam_fin_score[g] /
+ * beam_fin_len[g] when an EOS candidate is taken).  Rows in no group are admitted as with greedy == 2.  greedy == 3:
+ * VB_ERR_ARG. */
 int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h, int k, const int32_t *slots,
                 vb_ar_state *st, void *workspace, size_t workspace_bytes, vb_stream_t stream);
 
@@ -459,8 +483,8 @@ int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st,
 int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int64_t *sampled, int d,
                       vb_stream_t stream);
 
-/* one beam-search step (head->greedy == 3, "Beam search" above) on the logits already in st->logits, as the decode
- * step's tail runs it.  lse: NULL or [B], receives each row's log-sum-exp (written unless the step is a cap step), so
+/* one beam-search step (head->greedy == 3, or 4 with per-row groups: their steps alone, "Beam search" above) on the
+ * logits already in st->logits, as the decode step's tail runs it.  lse: NULL or [B], receives each row's log-sum-exp (written unless the step is a cap step), so
  * that a caller can restate the ranking exactly. */
 int vb_ar_beam_step(const vb_ar_head *head, vb_ar_state *st, int d, float *lse, vb_stream_t stream);
 

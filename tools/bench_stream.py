@@ -1,17 +1,24 @@
 """Continuous batching against static batches on bench.py's model (d=1024/16h/12L, bf16, 47-phoneme texts, 225-frame
 prompts), N requests in 64 decode slots.
 
-Two workloads: (1) a length mix, max_new_tokens drawn from a seeded U[75, 752] (1-10 s of audio); (2) bench.py's
+Three workloads: (1) a length mix, max_new_tokens drawn from a seeded U[75, 752] (1-10 s of audio); (2) bench.py's
 uniform workload, every utterance cap-terminated at 753 frames, where the stream has nothing to gain and any loss is
-admission or poll overhead.  Three schedules: inference_batch in input order (groups of 64), inference_batch
-longest-first, inference_stream.  They alternate, three repetitions each; the stream's `poll` is the best of 8 / 16 /
-32 on workload 1.  The three schedules must return identical codes.
+admission or poll overhead; (3) the length mix with every eighth request a num_beams=4 beam search.  Workloads 1 and 2
+run three schedules: inference_batch in input order (groups of 64), inference_batch longest-first, inference_stream.
+Workload 3 runs two: (a) one stream of every request, the beam groups decoding next to the other requests, and (b)
+what a server did before the stream took beam requests: the stream over the other requests, then
+generate(num_beams=4) over the beam requests (groups of 16 utterances, 64 rows).  The schedules alternate, three
+repetitions each; the stream's `poll` is the best of 8 / 16 / 32 on workload 1.  Every schedule of a workload must
+return identical codes.  Last, the decode step at 64 running slots, timed with CUDA events over graph replays: the
+seeded head (vb_ar_head.greedy == 2) against the mixed head (4) with no beam group present, the cost a stream pays
+from its first beam request on.
 
     python tools/bench_stream.py [--n 256] [--reps 3] [--out results.json]
 """
 from __future__ import annotations
 
 import argparse
+import ctypes as C
 import json
 import os
 import statistics
@@ -25,7 +32,8 @@ sys.path.insert(0, ROOT)
 import torch  # noqa: E402
 
 import bench  # noqa: E402
-from valle_b200.engine import StreamRequest  # noqa: E402
+from valle_b200 import _lib as L  # noqa: E402
+from valle_b200.engine import StreamRequest, _ArBuffers, _draws  # noqa: E402
 
 SLOTS = 64
 
@@ -74,6 +82,95 @@ def run(eng, sched, texts, prompts, mnt, poll):
                  "occupancy": frames / (steps * SLOTS) if steps else None}
 
 
+def run_beams(eng, sched, texts, prompts, mnt, beam, poll):
+    """workload 3: (a) "mixed", one stream of every request; (b) "separate", the stream over the requests not in
+    `beam`, then generate(num_beams=4) over those in it"""
+    n = len(texts)
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    out = [None] * n
+    reqs = [StreamRequest(t, p, max_new_tokens=k, num_beams=4 if i in beam else 1)
+            for i, (t, p, k) in enumerate(zip(texts, prompts, mnt))]
+    ids = list(range(n)) if sched == "mixed" else [i for i in range(n) if i not in beam]
+    for j, c in eng.generate_stream([reqs[i] for i in ids], slots=SLOTS, poll=poll):
+        out[ids[j]] = c
+    if sched == "separate":
+        bs = sorted(beam)
+        cs = eng.generate([texts[i] for i in bs], [prompts[i] for i in bs], max_new_tokens=[mnt[i] for i in bs],
+                          num_beams=4, return_device=True)
+        for i, c in zip(bs, cs):
+            out[i] = c
+    torch.cuda.synchronize()
+    ms = (time.perf_counter() - t0) * 1000.0
+    frames = sum(int(c.shape[0]) for c in out)
+    return out, {"sched": sched, "wall_ms": ms, "audio_tokens_per_s": frames * bench.N_Q / (ms / 1000.0),
+                 "frames": frames}
+
+
+def beam_workload(eng, texts, prompts, mnt, reps, poll):
+    beam = {i for i in range(len(texts)) if i % 8 == 7}
+    res = {"workload": "mix U[75, 752], every eighth request num_beams=4", "poll": poll, "beam_requests": len(beam),
+           "runs": []}
+    ref = {}
+    for _ in range(reps + 1):               # the first round warms up every shape (graphs, buffers)
+        for sched in ("mixed", "separate"):
+            out, r = run_beams(eng, sched, texts, prompts, mnt, beam, poll)
+            if ref:
+                bad = [i for i, (a, b) in enumerate(zip(out, ref["codes"])) if not torch.equal(a.cpu(), b)]
+                assert not bad, f"beams: {sched} differs from the mixed stream at requests {bad[:8]}"
+            else:
+                ref["codes"] = [c.cpu() for c in out]
+            res["runs"].append(r)
+    res["runs"] = res["runs"][2:]
+    res["summary"] = {sched: {"audio_tokens_per_s": statistics.median(r["audio_tokens_per_s"] for r in rs),
+                              "tokens_per_s_min_max": [min(r["audio_tokens_per_s"] for r in rs),
+                                                       max(r["audio_tokens_per_s"] for r in rs)],
+                              "wall_ms": statistics.median(r["wall_ms"] for r in rs)}
+                      for sched in ("mixed", "separate")
+                      for rs in [[r for r in res["runs"] if r["sched"] == sched]]}
+    res["codes_identical"] = True
+    return res
+
+
+def step_times(eng, texts, prompts, reps, steps=128):
+    """ms per decode step at SLOTS running rows (each capped at bench.FRAMES), graphs of 8 steps: the seeded head
+    (greedy == 2) and the mixed head (greedy == 4, every row in no group), alternating"""
+    m = eng.model
+    dev = eng.device
+    cap = (max(int(t.numel()) + int(p.shape[0]) for t, p in zip(texts, prompts)) + bench.FRAMES + 2 + 63) // 64 * 64
+    ts = (bench.FRAMES + 2 + 7) // 8 * 8
+    pe_a = eng._pe(m.ar_audio_position, cap + 2)
+    runs = {}
+    for greedy in (2, 4):
+        buf = _ArBuffers(eng, SLOTS, cap, ts)
+        p = eng._prefill_inputs(texts[:SLOTS], prompts[:SLOTS], [bench.FRAMES] * SLOTS)
+        buf.load_rows(p, _draws(SLOTS, 0, 1, 1.0))
+        buf.n_gen.zero_()
+        buf.finished.zero_()
+        buf.set_best_of(SLOTS, 1, False)
+        if greedy == 4:
+            buf.set_groups()
+        h = eng._prefill(buf, p, pe_a)
+        head = eng._head(pe_a, greedy)
+        L.check(eng.lib.vb_ar_head_step(eng.ar.handle, C.byref(head), h.data_ptr(), C.byref(buf.st),
+                                        buf.ws.data_ptr(), buf.ws.numel(), L.stream_ptr()), "vb_ar_head_step")
+        eng._device_steps(buf, head, 16)    # capture + warm-up
+        runs[greedy] = (buf, head)
+    out = {2: [], 4: []}
+    for _ in range(reps):
+        for greedy, (buf, head) in runs.items():
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            eng._device_steps(buf, head, steps)
+            e1.record()
+            e1.synchronize()
+            out[greedy].append(e0.elapsed_time(e1) / steps)
+    assert all(int(b.finished.sum()) == 0 for b, _ in runs.values()), "a row stopped inside the timed steps"
+    torch.cuda.synchronize(dev)
+    return {"slots": SLOTS, "steps_per_rep": steps, "ms_per_step_greedy2": out[2], "ms_per_step_greedy4": out[4],
+            "median_greedy2": statistics.median(out[2]), "median_greedy4": statistics.median(out[4])}
+
+
 def workload(eng, name, texts, prompts, mnt, reps, polls):
     res = {"workload": name, "runs": []}
     ref = None
@@ -120,6 +217,9 @@ def main():
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--seed", type=int, default=0)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--only", choices=["all", "beams"], default="all",
+                    help="beams: workload 3 and the decode-step times only (the stream's poll: --poll)")
+    ap.add_argument("--poll", type=int, default=16)
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_stream.py measures on the GPU; no CUDA device found")
@@ -132,14 +232,25 @@ def main():
     mix = [int(v) for v in torch.randint(75, 753, (a.n,), generator=g)]
     out = {"card": card(), "n": a.n, "slots": SLOTS, "seed": a.seed,
            "mix_lower_bound_steps": sum(k - 1 for k in mix) / SLOTS}
+    if a.only == "beams":
+        out["beams"] = beam_workload(eng, texts, prompts, mix, a.reps, a.poll)
+        out["decode_step"] = step_times(eng, texts, prompts, a.reps)
+        out["card_after"] = card()
+        return emit(out, a.out)
     out["mix"] = workload(eng, "mix U[75, 752]", texts, prompts, mix, a.reps, [8, 16, 32])
     uni = [bench.FRAMES] * a.n
     out["uniform"] = workload(eng, "uniform, cap-terminated", texts, prompts, uni, a.reps, [out["mix"]["poll"]])
+    out["beams"] = beam_workload(eng, texts, prompts, mix, a.reps, out["mix"]["poll"])
+    out["decode_step"] = step_times(eng, texts, prompts, a.reps)
+    emit(out, a.out)
+
+
+def emit(out, path):
     line = json.dumps(out)
     print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
+    if path:
+        os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+        with open(path, "w") as f:
             f.write(line + "\n")
 
 

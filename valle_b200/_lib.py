@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 14
+ABI_VERSION = 15
 VB_F32, VB_BF16, VB_E4M3 = 0, 1, 2
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -49,7 +49,8 @@ class ArState(C.Structure):
                 ("kv_dtype", C.c_int32), ("_kv_pad", C.c_int32), ("k_exp", vp), ("v_exp", vp),
                 ("top_p", vp), ("ras_window", vp), ("ras_max", vp), ("kv_parent", vp), ("logprob", vp),
                 ("beam_width", C.c_int32), ("_beam_pad", C.c_int32), ("beam_anc", vp), ("beam_score", vp),
-                ("beam_fin_score", vp), ("beam_fin_len", vp), ("beam_fin_anc", vp)]
+                ("beam_fin_score", vp), ("beam_fin_len", vp), ("beam_fin_anc", vp), ("beam_first", vp),
+                ("beam_n", vp)]
 
 
 class LnFold(C.Structure):

@@ -6,6 +6,7 @@
 #include <new>
 
 #include <algorithm>
+#include <vector>
 
 #include "common.cuh"
 #include "kernels.cuh"
@@ -552,25 +553,76 @@ QkvScatter layer_kv(const vb_decoder_desc &D, const vb_ar_state *st, int l, floa
                     KvRows{st->text_len, st->prompt_len, st->n_gen, st->finished}};
 }
 
-// the beam ancestry the decode attention follows (beam_width > 1), or none
+// the beam ancestry the decode attention follows (beam_width > 1, or per-row groups), or none
 BeamAnc beam_anc(const vb_ar_state *st) {
+  if (st->beam_first) return BeamAnc{st->beam_anc, st->tok_stride, 0, st->beam_first};
   return st->beam_width > 1 ? BeamAnc{st->beam_anc, st->tok_stride, st->beam_width} : BeamAnc{};
 }
+// The per-row beam groups (vb_ar_state.beam_first / beam_n) as the header states them, read back on `s` unless `s`
+// is capturing a graph (a captured call reads no host values: there the caller guarantees them).  slots / k:
+// vb_ar_admit's slots, which must pass every admitted group's rows together and in order.
+int check_groups(const char *fn, const vb_ar_state *st, const int32_t *slots, int k, cudaStream_t s) {
+  cudaStreamCaptureStatus cap;
+  VB_CUDA(cudaStreamIsCapturing(s, &cap));
+  if (cap != cudaStreamCaptureStatusNone) return VB_OK;
+  const int B = st->B;
+  std::vector<int32_t> f(B), w(B), sl(k);
+  VB_CUDA(cudaMemcpyAsync(f.data(), st->beam_first, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  VB_CUDA(cudaMemcpyAsync(w.data(), st->beam_n, B * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  if (k > 0) VB_CUDA(cudaMemcpyAsync(sl.data(), slots, k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+  VB_CUDA(cudaStreamSynchronize(s));
+  for (int b = 0; b < B; ++b) {
+    const int g = f[b], n = w[b];
+    if (g == -1) continue;
+    VB_CHECK_ARG(n >= 2 && n <= 16, "%s: beam_n[%d] = %d not in [2, 16]", fn, b, n);
+    VB_CHECK_ARG(g >= 0 && g <= b && b < g + n && g + n <= B && f[g] == g && w[g] == n,
+                 "%s: row %d: beam_first %d / beam_n %d is not a group of rows [first, first + n) within B = %d", fn,
+                 b, g, n, B);
+    if (g == b)
+      for (int j = 1; j < n; ++j)
+        VB_CHECK_ARG(f[b + j] == b, "%s: row %d of the group at row %d has beam_first %d", fn, b + j, b, f[b + j]);
+  }
+  for (int i = 0; i < k; ++i) {
+    VB_CHECK_ARG(sl[i] >= 0 && sl[i] < B, "%s: slots[%d] = %d not in [0, B = %d)", fn, i, sl[i], B);
+    const int g = f[sl[i]], j = sl[i] - g, i0 = i - j;
+    if (g < 0) continue;
+    bool whole = i0 >= 0 && i0 + w[g] <= k;
+    for (int q = 0; whole && q < w[g]; ++q) whole = sl[i0 + q] == g + q;
+    VB_CHECK_ARG(whole, "%s: slots[%d] = %d: the group at row %d is not admitted whole and in order", fn, i, sl[i], g);
+  }
+  return VB_OK;
+}
 // the beam-search fields a step with this head reads (include/valle_b200.h "Beam search")
-int check_beam(const char *fn, const vb_ar_head *head, const vb_ar_state *st) {
+int check_beam(const char *fn, const vb_ar_head *head, const vb_ar_state *st, cudaStream_t s,
+               const int32_t *slots = nullptr, int k = 0) {
+  const bool per_row = st->beam_first != nullptr;
+  if (per_row || head->greedy == 4) {
+    VB_CHECK_ARG(st->beam_width <= 1, "%s: per-row beam groups (beam_first) with beam_width %d > 1", fn,
+                 st->beam_width);
+    VB_CHECK_ARG(head->greedy == 4, "%s: per-row beam groups run with vb_ar_head.greedy == 4 (got %d)", fn,
+                 head->greedy);
+    VB_CHECK_ARG(per_row && st->beam_n && st->beam_anc, "%s: vb_ar_head.greedy == 4 needs beam_first, beam_n and "
+                 "beam_anc", fn);
+  }
   if (head->greedy == 3 || st->beam_width > 1) {
     VB_CHECK_ARG(st->beam_width >= 1 && st->beam_width <= 16 && st->B % st->beam_width == 0,
                  "%s: beam_width %d not in [1, 16] or not dividing B = %d", fn, st->beam_width, st->B);
     VB_CHECK_ARG(st->beam_anc != nullptr, "%s: beam search needs beam_anc", fn);
   }
-  if (head->greedy == 3)
+  if (head->greedy >= 3)
     VB_CHECK_ARG(st->beam_score && st->beam_fin_score && st->beam_fin_len && st->beam_fin_anc,
-                 "%s: vb_ar_head.greedy == 3: beam arrays not set", fn);
+                 "%s: vb_ar_head.greedy == %d: beam arrays not set", fn, head->greedy);
+  if (per_row) VB_TRY(check_groups(fn, st, slots, k, s));
   return VB_OK;
 }
 // the step's tail on the head's logits (in: their pending partials): the argmax / seeded draw, the reduce alone
-// (greedy == 0), or the reduce and the beam step (greedy == 3)
+// (greedy == 0), the reduce and the beam step (greedy == 3), or the seeded draw of the rows in no group and the beam
+// step of every group (greedy == 4)
 int ar_tail(int ldl, const SplitK &in, const vb_ar_head *head, vb_ar_state *st, int d, bool pdl, cudaStream_t s) {
+  if (head->greedy == 4) {
+    VB_TRY(launch_ar_sample(st->logits, ldl, in, head, st, d, nullptr, 0, pdl, s));
+    return launch_beam_tail(head, st, d, pdl, s);
+  }
   if (head->greedy != 3)
     return launch_ar_sample(st->logits, ldl, in, head, st, d, nullptr, head->greedy ? 0 : 1, pdl, s);
   if (in.part) VB_TRY(launch_ar_sample(st->logits, ldl, in, head, st, d, nullptr, 1, pdl, s));
@@ -609,14 +661,11 @@ VB_API size_t vb_ar_step_workspace(const vb_decoder_desc *desc, int B, int cache
   return carved_bytes(carve_step_ws, *desc, B, cache_cap);
 }
 
-VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
-                           void *workspace, size_t workspace_bytes, vb_stream_t stream) {
-  VB_CHECK_ARG(dec && head && h && st, "vb_ar_head_step: null argument");
-  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 3, "vb_ar_head_step: greedy %d not in {0, 1, 2, 3}", head->greedy);
-  VB_TRY(check_beam("vb_ar_head_step", head, st));
+namespace {
+// vb_ar_head_step once its arguments are checked (vb_ar_decode_step's CUDA-core chain ends with it)
+int head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st, void *workspace,
+              size_t workspace_bytes, cudaStream_t s) {
   const vb_decoder_desc &D = dec->desc;
-  VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_head_step: a pre-LN decoder needs its final norm");
-  cudaStream_t s = (cudaStream_t)stream;
   const int d = D.d_model;
   const int ldl = (head->n_vocab + 3) & ~3;
   if (use_tc_decode(D, st->B)) {
@@ -631,6 +680,17 @@ VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float
                      D.final_norm_w ? &ln : nullptr, 0, nullptr, s));
   if (head->greedy) VB_TRY(ar_tail(ldl, SplitK{}, head, st, d, false, s));
   return VB_OK;
+}
+}  // namespace
+
+VB_API int vb_ar_head_step(vb_decoder_t dec, const vb_ar_head *head, const float *h, vb_ar_state *st,
+                           void *workspace, size_t workspace_bytes, vb_stream_t stream) {
+  VB_CHECK_ARG(dec && head && h && st, "vb_ar_head_step: null argument");
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 4, "vb_ar_head_step: greedy %d not in {0, 1, 2, 3, 4}",
+               head->greedy);
+  VB_TRY(check_beam("vb_ar_head_step", head, st, (cudaStream_t)stream));
+  VB_CHECK_ARG(!dec->desc.norm_first || dec->desc.final_norm_w, "vb_ar_head_step: a pre-LN decoder needs its final norm");
+  return head_step(dec, head, h, st, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 namespace {
@@ -662,6 +722,13 @@ AdmitWs carve_admit_ws(Carve &c, const vb_decoder_desc &D, int k, int n_vocab) {
   cs.top_p = c.take<float>(k * 4);
   cs.ras_window = c.take<int32_t>(k * 4);
   cs.ras_max = c.take<int32_t>(k * 4);
+  cs.beam_first = c.take<int32_t>(k * 4);   // the per-row beam groups (head->greedy == 4 only)
+  cs.beam_n = c.take<int32_t>(k * 4);
+  cs.beam_anc = c.take<uint8_t>(k);
+  cs.beam_score = c.take<float>(k * 4);
+  cs.beam_fin_score = c.take<float>(k * 8);
+  cs.beam_fin_len = c.take<int32_t>(k * 4);
+  cs.beam_fin_anc = c.take<uint8_t>(k);
   w.head_ws_bytes = vb_ar_step_workspace(&D, k, kAdmitCap);
   w.head_ws = c.take(w.head_ws_bytes);
   return w;
@@ -676,9 +743,11 @@ VB_API int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h,
                        vb_ar_state *st, void *workspace, size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && head && h && slots && st, "vb_ar_admit: null argument");
   VB_CHECK_ARG(k >= 1 && k <= st->B, "vb_ar_admit: k=%d not in [1, B=%d]", k, st->B);
-  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 2, "vb_ar_admit: greedy %d not in {0, 1, 2}", head->greedy);
-  VB_CHECK_ARG(head->greedy != 2 || (st->sample_seed && st->top_k && st->temperature),
-               "vb_ar_admit: vb_ar_head.greedy == 2: sampler arrays not set");
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 4 && head->greedy != 3, "vb_ar_admit: greedy %d not in {0, 1, 2, 4}",
+               head->greedy);
+  VB_CHECK_ARG(head->greedy < 2 || (st->sample_seed && st->top_k && st->temperature),
+               "vb_ar_admit: vb_ar_head.greedy == %d: sampler arrays not set", head->greedy);
+  VB_TRY(check_beam("vb_ar_admit", head, st, (cudaStream_t)stream, slots, k));
   const vb_decoder_desc &D = dec->desc;
   VB_CHECK_ARG(workspace && workspace_bytes >= vb_ar_admit_workspace(&D, k, head->n_vocab),
                "vb_ar_admit: workspace too small (%zu < %zu)", workspace_bytes,
@@ -686,9 +755,12 @@ VB_API int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h,
   cudaStream_t s = (cudaStream_t)stream;
   Carve c(workspace);
   AdmitWs w = carve_admit_ws(c, D, k, head->n_vocab);
+  if (head->greedy != 4)
+    w.cs.beam_first = w.cs.beam_n = nullptr;
   const int ldl = (head->n_vocab + 3) & ~3;
   VB_TRY(launch_ar_admit_copy(st, &w.cs, slots, D.d_model, ldl, head->n_vocab, false, s));
-  VB_TRY(vb_ar_head_step(dec, head, h, &w.cs, w.head_ws, w.head_ws_bytes, stream));
+  VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_admit: a pre-LN decoder needs its final norm");
+  VB_TRY(head_step(dec, head, h, &w.cs, w.head_ws, w.head_ws_bytes, s));
   return launch_ar_admit_copy(st, &w.cs, slots, D.d_model, ldl, head->n_vocab, true, s);
 }
 
@@ -707,17 +779,18 @@ VB_API int vb_ar_push_tokens(const vb_ar_head *head, vb_ar_state *st, const int6
 
 VB_API int vb_ar_beam_step(const vb_ar_head *head, vb_ar_state *st, int d, float *lse, vb_stream_t stream) {
   VB_CHECK_ARG(head && st, "vb_ar_beam_step: null argument");
-  VB_CHECK_ARG(head->greedy == 3, "vb_ar_beam_step: vb_ar_head.greedy %d != 3", head->greedy);
-  VB_TRY(check_beam("vb_ar_beam_step", head, st));
+  VB_CHECK_ARG(head->greedy == 3 || head->greedy == 4, "vb_ar_beam_step: vb_ar_head.greedy %d not in {3, 4}",
+               head->greedy);
+  VB_TRY(check_beam("vb_ar_beam_step", head, st, (cudaStream_t)stream));
   return launch_beam_tail(head, st, d, false, (cudaStream_t)stream, lse);
 }
 
 VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_state *st, void *workspace,
                              size_t workspace_bytes, vb_stream_t stream) {
   VB_CHECK_ARG(dec && head && st, "vb_ar_decode_step: null argument");
-  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 3, "vb_ar_decode_step: greedy %d not in {0, 1, 2, 3}",
+  VB_CHECK_ARG(head->greedy >= 0 && head->greedy <= 4, "vb_ar_decode_step: greedy %d not in {0, 1, 2, 3, 4}",
                head->greedy);
-  VB_TRY(check_beam("vb_ar_decode_step", head, st));
+  VB_TRY(check_beam("vb_ar_decode_step", head, st, (cudaStream_t)stream));
   const vb_decoder_desc &D = dec->desc;
   // the pre-LN chain leaves the last FFN2's partial sums to the final norm's reduce: without one they would be lost
   VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_decode_step: a pre-LN decoder needs its final norm");
@@ -735,8 +808,8 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     set_error("vb_ar_decode_step: kv_parent (shared prompt prefixes) is not supported on the FP8 KV cache");
     return VB_ERR_UNSUPPORTED;
   }
-  if (f8 && st->beam_width > 1) {
-    set_error("vb_ar_decode_step: beam search (beam_width > 1) is not supported on the FP8 KV cache");
+  if (f8 && (st->beam_width > 1 || st->beam_first)) {
+    set_error("vb_ar_decode_step: beam search (beam_width > 1 or beam_first) is not supported on the FP8 KV cache");
     return VB_ERR_UNSUPPORTED;
   }
   cudaStream_t s = (cudaStream_t)stream;
@@ -844,5 +917,5 @@ VB_API int vb_ar_decode_step(vb_decoder_t dec, const vb_ar_head *head, vb_ar_sta
     VB_TRY(launch_gemv(w.hb, dff, B, P.lin2_w, dt, P.lin2_b, d, dff, x, d, nullptr, 2, nullptr, s));
     if (post) VB_TRY(launch_post_norm(x, B, d, P.norm2_w, P.norm2_b, nullptr, 1e-5f, nullptr, VB_F32, s));
   }
-  return vb_ar_head_step(dec, head, x, st, workspace, workspace_bytes, stream);
+  return head_step(dec, head, x, st, workspace, workspace_bytes, s);
 }

@@ -166,11 +166,14 @@ __device__ __forceinline__ int kv_shared_rows(const int32_t *parent, const KvRow
   par = parent[b];
   return par == b ? 0 : (rows.text_len[b] + rows.prompt_len[b]) & ~15;
 }
-// Beam search (vb_ar_state.beam_width > 1): the ancestry table the decode attention follows.  Row b's generated cache
-// row S_b + Tp_b + t, below its current row, lives in the streams of row b - b % width + anc[b * ld + t].
+// Beam search (vb_ar_state.beam_width > 1, or the per-row groups beam_first): the ancestry table the decode attention
+// follows.  Row b's generated cache row S_b + Tp_b + t, below its current row, lives in the streams of row
+// g_b + anc[b * ld + t], g_b the first row of b's group: b - b % width, or first[b] (-1: b is in no group and reads
+// its own streams).
 struct BeamAnc {
   const uint8_t *anc = nullptr;  // [B, ld]
   int ld = 0, width = 0;
+  const int32_t *first = nullptr;  // [B] or NULL (groups of `width` rows)
 };
 // The rows of one (utterance, head) stream as a decode kernel reads them: element offset of row `pos` from the
 // stream's row 0.  kShared = false: the stream's own rows, nothing else is
@@ -205,11 +208,13 @@ struct KvStreamRows {
       pre = kv_shared_rows(parent, rows, b, par);
       pd = par - b;
     }
-    const int jb = b % ba.width;
+    const int g0 = ba.first != nullptr ? ba.first[b] : b - b % ba.width;
+    const int jb = b - g0;
+    const int gen_end = g0 >= 0 ? cur : gen0;   // a row in no group: no generated row comes from elsewhere
     const uint8_t *a = ba.anc + (int64_t)b * ba.ld;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       const int p = c0_ + i;
-      dl_s[i] = (int16_t)(p < pre ? pd : (p >= gen0 && p < cur) ? (int)a[p - gen0] - jb : 0);
+      dl_s[i] = (int16_t)(p < pre ? pd : (p >= gen0 && p < gen_end) ? (int)a[p - gen0] - jb : 0);
     }
     dl = dl_s;
     c0 = c0_;

@@ -278,7 +278,9 @@ __device__ __forceinline__ float row_logsumexp(const float (&lv)[5], float mx, f
   return mx + logf(z);
 }
 
-template <bool kSample, bool kScore = false>
+// kMixed (vb_ar_head.greedy == 4): the rows of beam groups (beam_first[b] >= 0) only reduce their logits, the beam tail
+// that follows takes them
+template <bool kSample, bool kScore = false, bool kMixed = false>
 __global__ void __launch_bounds__(256)
 ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__restrict__ partials, int splits,
                  int ldp, int n_vocab, int eos_id,
@@ -288,13 +290,14 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
                  int32_t *__restrict__ n_gen, int32_t *__restrict__ finished,
                  int32_t *__restrict__ tokens, int tok_stride, float *__restrict__ x_cur, int d,
                  const int64_t *__restrict__ forced, int reduce_only, LnFoldStats fold, const float *__restrict__ fold_d,
-                 SamplerArgs sa, float *__restrict__ logprob) {
+                 SamplerArgs sa, float *__restrict__ logprob, const int32_t *__restrict__ beam_first) {
   __shared__ ArgMax wbest[8];
   __shared__ int s_tok, s_pos;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   pdl_launch_dependents();
   pdl_wait();
   vb_trace(TR_SAMPLE * 2);
+  if constexpr (kMixed) reduce_only |= beam_first[b] >= 0;
   if (finished[b] != 0 && !reduce_only) {  // uniform per CTA
     // a stopped utterance still rides through the batched step: give it a fixed, bounded input row (its residual
     // stream is updated in place by the layer chain and would otherwise drift step over step); the scatter and
@@ -359,7 +362,7 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
       for (int j = 0; j < 5; ++j) lv[j] = tid + j * 256 < n_vocab ? row[tid + j * 256] : -CUDART_INF_F;
     }
   }
-  if constexpr (!kSample) {
+  if constexpr (!kSample || kMixed) {
     if (reduce_only) return;
   }
   int draw = -1;
@@ -419,21 +422,24 @@ ar_sample_kernel(float *__restrict__ logits, int64_t ld_logits, const float *__r
 
 int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const vb_ar_head *head, vb_ar_state *st,
                      int d, const int64_t *forced, int reduce_only, bool pdl, cudaStream_t s) {
-  const bool sample = head->greedy == 2 && forced == nullptr && !reduce_only;
+  const bool sample = (head->greedy == 2 || head->greedy == 4) && forced == nullptr && !reduce_only;
   const bool score = sample && st->logprob != nullptr;
+  const bool mixed = sample && head->greedy == 4;
   SamplerArgs sa{};
   if (sample) {
-    VB_CHECK_ARG(st->sample_seed && st->top_k && st->temperature, "vb_ar_head.greedy == 2: sampler arrays not set");
+    VB_CHECK_ARG(st->sample_seed && st->top_k && st->temperature,
+                 "vb_ar_head.greedy == %d: sampler arrays not set", head->greedy);
     VB_CHECK_ARG(head->n_vocab <= 5 * 256, "device sampler: n_vocab %d > 1280", head->n_vocab);
     sa = SamplerArgs{st->sample_seed, st->top_k, st->temperature, st->top_p, st->ras_window, st->ras_max};
   }
-  const auto k = score ? ar_sample_kernel<true, true> : sample ? ar_sample_kernel<true> : ar_sample_kernel<false>;
+  const auto k = mixed ? (score ? ar_sample_kernel<true, true, true> : ar_sample_kernel<true, false, true>)
+                 : score ? ar_sample_kernel<true, true> : sample ? ar_sample_kernel<true> : ar_sample_kernel<false>;
   VB_CUDA(launch_kernel(k, dim3(st->B), dim3(256), 0, s, pdl,
                         logits, ld_logits, in.part, in.splits, in.ldp, head->n_vocab, head->eos_id, head->audio_emb,
                         head->alpha, head->pe, head->pe_rows, (const int32_t *)st->text_len,
                         (const int32_t *)st->prompt_len, (const int32_t *)st->max_new, st->n_gen, st->finished,
                         st->tokens, st->tok_stride, st->x_cur, d, forced, reduce_only, in.fold, in.bias, sa,
-                        score ? st->logprob : nullptr));
+                        score ? st->logprob : nullptr, mixed ? st->beam_first : nullptr));
   count_launch();
   return VB_OK;
 }
@@ -458,7 +464,8 @@ ar_beam_kernel(const float *__restrict__ logits, int64_t ld_logits, int n_vocab,
                int32_t *__restrict__ n_gen, int32_t *__restrict__ finished, int32_t *__restrict__ tokens,
                int tok_stride, float *__restrict__ x_cur, int d, uint8_t *__restrict__ anc,
                float *__restrict__ score, float *__restrict__ fin_score, int32_t *__restrict__ fin_len,
-               uint8_t *__restrict__ fin_anc, float *__restrict__ lse_out) {
+               uint8_t *__restrict__ fin_anc, float *__restrict__ lse_out, const int32_t *__restrict__ first,
+               const int32_t *__restrict__ width) {
   __shared__ ArgMax wbest[8];
   __shared__ float wz[8];
   __shared__ float lse[kBeamMax];
@@ -467,10 +474,20 @@ ar_beam_kernel(const float *__restrict__ logits, int64_t ld_logits, int n_vocab,
   __shared__ int npar[kBeamMax], ntok[kBeamMax];
   __shared__ float nsc[kBeamMax];
   __shared__ int s_stop, s_fpar, s_len, s_from_fin;
-  const int g = blockIdx.x, r0 = g * n, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int K = 2 * n;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   pdl_launch_dependents();
   pdl_wait();
+  // per-row groups: one CTA per row, the first row of a group runs it (and indexes its finished hypothesis); a width
+  // out of range, or a group past the last row, is refused on the host and never read out of bounds here
+  const int g = blockIdx.x;
+  int r0 = g * n;
+  if (first != nullptr) {
+    if (first[g] != g) return;
+    r0 = g;
+    n = width[g];
+    if (n < 2 || n > kBeamMax || g + n > (int)gridDim.x) return;
+  }
+  const int K = 2 * n;
   if (finished[r0] != 0) {   // a stopped group rides along with fixed input rows, as ar_sample_kernel's rows do
     for (int j = 0; j < n; ++j) {
       float *xo = x_cur + (int64_t)(r0 + j) * d;
@@ -661,14 +678,16 @@ ar_beam_kernel(const float *__restrict__ logits, int64_t ld_logits, int n_vocab,
 }
 
 int launch_beam_tail(const vb_ar_head *head, vb_ar_state *st, int d, bool pdl, cudaStream_t s, float *lse) {
-  const int n = st->beam_width;
+  const bool per_row = st->beam_first != nullptr;
+  const int n = per_row ? kBeamMax : st->beam_width;   // per-row groups: the widest group
   VB_CHECK_ARG(head->n_vocab <= 40 * 32 && 2 * n <= head->n_vocab, "beam tail: n_vocab %d not in [2n, 1280]",
                head->n_vocab);
   const int64_t ldl = (head->n_vocab + 3) & ~3;
-  VB_CUDA(launch_kernel(ar_beam_kernel, dim3(st->B / n), dim3(256), 0, s, pdl, (const float *)st->logits, ldl,
-                        head->n_vocab, head->eos_id, n, head->audio_emb, head->alpha, head->pe, head->pe_rows,
-                        st->prompt_len, st->max_new, st->n_gen, st->finished, st->tokens, st->tok_stride, st->x_cur, d,
-                        st->beam_anc, st->beam_score, st->beam_fin_score, st->beam_fin_len, st->beam_fin_anc, lse));
+  VB_CUDA(launch_kernel(ar_beam_kernel, dim3(per_row ? st->B : st->B / n), dim3(256), 0, s, pdl,
+                        (const float *)st->logits, ldl, head->n_vocab, head->eos_id, n, head->audio_emb, head->alpha,
+                        head->pe, head->pe_rows, st->prompt_len, st->max_new, st->n_gen, st->finished, st->tokens,
+                        st->tok_stride, st->x_cur, d, st->beam_anc, st->beam_score, st->beam_fin_score,
+                        st->beam_fin_len, st->beam_fin_anc, lse, st->beam_first, st->beam_n));
   count_launch();
   return VB_OK;
 }
@@ -695,6 +714,16 @@ ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__
         const_cast<int32_t *>(cs.ras_window)[i] = st.ras_window ? st.ras_window[s] : 0;
         const_cast<int32_t *>(cs.ras_max)[i] = st.ras_max ? st.ras_max[s] : 0;
       }
+      if (cs.beam_first) {   // greedy == 4: a group's rows start as a fresh beam state's (include/valle_b200.h)
+        const int f = st.beam_first[s];
+        const_cast<int32_t *>(cs.beam_first)[i] = f < 0 ? -1 : i - (s - f);
+        const_cast<int32_t *>(cs.beam_n)[i] = f < 0 ? 0 : st.beam_n[s];
+        cs.beam_anc[i] = 0;
+        cs.beam_score[i] = s == f ? 0.f : -CUDART_INF_F;
+        cs.beam_fin_score[2 * i] = -CUDART_INF_F;
+        cs.beam_fin_score[2 * i + 1] = st.beam_fin_score[2 * s + 1];
+        cs.beam_fin_len[i] = st.beam_fin_len[s];
+      }
     }
     return;
   }
@@ -702,6 +731,15 @@ ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__
     st.n_gen[s] = cs.n_gen[i];
     st.finished[s] = cs.finished[i];
     st.tokens[(int64_t)s * st.tok_stride] = cs.tokens[i];
+    if (cs.beam_first && st.beam_first[s] >= 0) {
+      st.beam_anc[(int64_t)s * st.tok_stride] = cs.beam_anc[i];
+      st.beam_score[s] = cs.beam_score[i];
+      if (st.beam_first[s] == s) {
+        st.beam_fin_score[2 * s] = cs.beam_fin_score[2 * i];
+        st.beam_fin_score[2 * s + 1] = cs.beam_fin_score[2 * i + 1];
+        st.beam_fin_len[s] = cs.beam_fin_len[i];
+      }
+    }
   }
   for (int c = tid; c < d; c += 256) st.x_cur[(int64_t)s * d + c] = cs.x_cur[(int64_t)i * d + c];
   for (int c = tid; c < n_vocab; c += 256) st.logits[(int64_t)s * ldl + c] = cs.logits[(int64_t)i * ldl + c];

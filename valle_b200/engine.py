@@ -78,7 +78,8 @@ class EngineStats:
 
 class StreamRequest(NamedTuple):
     """One utterance of ValleEngine.generate_stream: text int64 [S] phoneme ids, prompt int64 [Tp, Q] codec ids, and
-    what generate() takes per utterance.  top_k != 1 and ras need a seed (the seeded device sampler)."""
+    what generate() takes per utterance.  top_k != 1 and ras need a seed (the seeded device sampler); num_beams > 1
+    decodes it by beam search, as generate(num_beams=) does, and takes no seed, top_k, top_p or ras."""
     text: torch.Tensor
     prompt: torch.Tensor
     enroll_len: Optional[int] = None
@@ -88,6 +89,22 @@ class StreamRequest(NamedTuple):
     max_new_tokens: Optional[int] = None
     top_p: float = 1.0
     ras: Optional[Tuple[int, float]] = None
+    num_beams: int = 1
+
+
+def _take_slots(free: List[int], widths: Sequence[int]) -> List[List[int]]:
+    """First-in first-out admission into decode slots.  widths: the slots each queued request needs, in queue order (1,
+    or n for a beam group of n rows).  Each request takes the lowest run of that many consecutive free slots, up to the
+    first request that finds no such run: it waits, and every request behind it waits too.  free: the free slots,
+    sorted; the taken ones are removed from it.  Returns the slots of the requests that were admitted."""
+    out = []
+    for n in widths:
+        i = next((i for i in range(len(free) - n + 1) if free[i + n - 1] == free[i] + n - 1), None)
+        if i is None:
+            break
+        out.append(free[i:i + n])
+        del free[i:i + n]
+    return out
 
 
 class _ArBuffers:
@@ -133,6 +150,9 @@ class _ArBuffers:
         self.beam_fin_score = torch.zeros((B, 2), dtype=torch.float32, device=dev)
         self.beam_fin_len = torch.zeros(B, **i32)
         self.beam_fin_anc = torch.zeros((B, tok_stride), dtype=torch.uint8, device=dev)
+        #: per-row beam groups of continuous batching (set_groups): each row's group's first row (-1: none), its width
+        self.beam_first = torch.full((B,), -1, **i32)
+        self.beam_n = torch.zeros(B, **i32)
         st = L.ArState()
         st.B, st.tok_stride = B, tok_stride
         st.text_len, st.prompt_len, st.max_new = self.text_len.data_ptr(), self.prompt_len.data_ptr(), self.max_new.data_ptr()
@@ -161,14 +181,13 @@ class _ArBuffers:
         st = self.st
         st.beam_width, st.beam_anc, st.beam_score, st.beam_fin_score, st.beam_fin_len, st.beam_fin_anc = \
             0, None, None, None, None, None
+        st.beam_first = st.beam_n = None
         if beams:
             r = torch.arange(n_rows, device=self.beam_score.device)
             self.beam_score[:n_rows] = torch.where(r % n == 0, 0.0, float("-inf"))
             self.beam_fin_score[:, 0] = float("-inf")
             st.beam_width = n
-            st.beam_anc, st.beam_score = self.beam_anc.data_ptr(), self.beam_score.data_ptr()
-            st.beam_fin_score, st.beam_fin_len = self.beam_fin_score.data_ptr(), self.beam_fin_len.data_ptr()
-            st.beam_fin_anc = self.beam_fin_anc.data_ptr()
+            self._point_beams()
         self.st.kv_parent = None
         if n > 1 and self.kv_dtype is None:
             r = torch.arange(n_rows, dtype=torch.int32)
@@ -179,9 +198,27 @@ class _ArBuffers:
             self.logprob.zero_()
             self.st.logprob = self.logprob.data_ptr()
 
-    def load_rows(self, p: _Prefill, draws: Optional[Sequence[_Draw]] = None):
+    def _point_beams(self):
+        st = self.st
+        st.beam_anc, st.beam_score = self.beam_anc.data_ptr(), self.beam_score.data_ptr()
+        st.beam_fin_score, st.beam_fin_len = self.beam_fin_score.data_ptr(), self.beam_fin_len.data_ptr()
+        st.beam_fin_anc = self.beam_fin_anc.data_ptr()
+
+    def set_groups(self):
+        """Point the state at per-row beam groups (vb_ar_state.beam_first, the stream's mixed head) and at kv_parent,
+        with every row in no group and its own parent; vb_ar_admit starts each group it admits"""
+        self.beam_first.fill_(-1)
+        self.kv_parent.copy_(torch.arange(self.B, dtype=torch.int32))
+        st = self.st
+        st.beam_first, st.beam_n, st.kv_parent = self.beam_first.data_ptr(), self.beam_n.data_ptr(), \
+            self.kv_parent.data_ptr()
+        self._point_beams()
+
+    def load_rows(self, p: _Prefill, draws: Optional[Sequence[_Draw]] = None,
+                  groups: Optional[Sequence[Tuple[int, int, int]]] = None):
         """Write the lengths and token caps of prefill block p's utterances into their rows (0..B-1, or p.slots_d)
-        and, given their draws, the sampler columns, all six from one host -> device copy"""
+        and, given their draws, the sampler columns, all six from one host -> device copy; groups: also each row's
+        (kv_parent, beam_first, beam_n) (set_groups), in the same copy"""
         rows = None if p.slots_d is None else p.slots_d.long()
 
         def put(col, v):
@@ -195,8 +232,11 @@ class _ArBuffers:
         if draws is None:
             return
         # _Draw's fields in order; the int64 seeds first, so that every column starts aligned to its element size
-        cols = (self.sample_seed, self.top_k, self.temperature, self.top_p, self.ras_window, self.ras_max)
-        vals = zip(*(d._replace(seed=d.seed_i64) for d in draws))
+        cols = [self.sample_seed, self.top_k, self.temperature, self.top_p, self.ras_window, self.ras_max]
+        vals = list(zip(*(d._replace(seed=d.seed_i64) for d in draws)))
+        if groups is not None:
+            cols += [self.kv_parent, self.beam_first, self.beam_n]
+            vals += list(zip(*groups))
         block = torch.cat([torch.tensor(v, dtype=c.dtype).view(torch.uint8) for c, v in zip(cols, vals)])
         block = block.to(self.text_len.device, non_blocking=True).split([len(draws) * c.element_size() for c in cols])
         for c, v in zip(cols, block):
@@ -844,7 +884,10 @@ class ValleEngine:
         `poll` decode steps; the NAR runs over every `nar_batch` (default `slots`) finished utterances, and over the
         rest once nothing is left to decode.  Sampling is greedy, or seeded per request (`seed`, with top_k /
         temperature / top_p / ras): the draws depend on the seed, the step and the request's own codes only, never on
-        the slot or the schedule."""
+        the slot or the schedule.  A request with num_beams=n > 1 is decoded by beam search (generate(num_beams=n)'s
+        rules; not on the FP8 cache, n <= slots) in n consecutive slots that read one copy of its prompt prefix and are
+        freed together; requests are admitted first in, first out, so one that finds no run of n free slots waits, and
+        the requests behind it with it.  Its codes are those of generate(num_beams=n) on it alone."""
         with torch.cuda.device(self.device):
             self._refresh()
         kv_dtype = self.kv_cache_dtype()
@@ -898,12 +941,15 @@ class ValleEngine:
             buf.x_cur.zero_()
             buf.set_best_of(n_slots, 1, False)   # no shared prefixes or scores: slots are refilled one by one
             pe_a = self._pe(m.ar_audio_position, cap + 2)
-            heads = {g: self._head(pe_a, g) for g in (1, 2)}
+            heads = {g: self._head(pe_a, g) for g in (1, 2, 4)}
             ws = torch.empty(self.lib.vb_ar_admit_workspace(C.byref(self.ar.desc), n_slots, self.n_vocab),
                              dtype=torch.uint8, device=dev)
-        mode = 1                               # 2 (the seeded sampler) from the first seeded request on
+        # 2 (the seeded sampler) from the first seeded request on, 4 (2 next to beam groups) from the first beam request
+        mode = 1
         free = list(range(n_slots))
-        active: Dict[int, _Utt] = {}           # slot -> the utterance decoding in it
+        queue: List[Tuple[int, StreamRequest, _Draw]] = []   # pulled requests waiting for slots, in order
+        active: Dict[int, _Utt] = {}           # slot -> the utterance decoding in it (a beam group's first slot)
+        width: Dict[int, int] = {}             # active slot -> the slots its utterance holds from there on
         pending: List[Tuple[_Utt, torch.Tensor]] = []   # finished utterances and their codes, waiting for the NAR
         n_pulled, exhausted, device_ids = 0, False, False
 
@@ -920,6 +966,13 @@ class ValleEngine:
                 idx = n_pulled
                 n_pulled += 1
                 _check_utt(f"request {idx}", r.text, r.prompt, Q)
+                try:
+                    beams = _check_num_beams(r.num_beams, r.seed, r.top_k, r.top_p, r.ras, 1, None, None, False,
+                                             kv_dtype is not None)
+                except ValueError as e:
+                    raise ValueError(f"request {idx}: {e}") from None
+                if beams > n_slots:
+                    raise ValueError(f"request {idx}: num_beams={beams} needs more than the {n_slots} slots")
                 seed, top_k = r.seed, r.top_k
                 if seed is None:
                     if top_k != 1 or r.ras is not None:
@@ -930,31 +983,41 @@ class ValleEngine:
                     raise ValueError(f"request {idx}: prefix_mode {pm} needs enroll_len")
                 if self._context(r) > max_context:
                     raise ValueError(f"request {idx} needs {self._context(r)} KV-cache rows > max_context={max_context}")
-                if not draw.greedy:
-                    mode = 2
-                out.append((idx, r, draw))
+                if beams > 1:
+                    mode = 4
+                elif not draw.greedy:
+                    mode = max(mode, 2)
+                out.append((idx, r._replace(num_beams=beams), draw))
             return out
 
-        def admit(new):
+        def admit(new, taken):
+            """the requests `new`, each into its slots of `taken`: a beam group's n rows are its request n times, the
+            prefill writing each row's own cache streams"""
             nonlocal device_ids
-            k = len(new)
-            sl = free[:k]
-            del free[:k]
-            texts = [r.text for _, r, _ in new]
-            prompts = [r.prompt for _, r, _ in new]
-            cap_new = [self._cap_new([int(r.text.numel())], r.max_new_tokens)[0] for _, r, _ in new]
+            rows = [q for q, sl in zip(new, taken) for _ in sl]
+            sl = [s for ss in taken for s in ss]
+            texts = [r.text for _, r, _ in rows]
+            prompts = [r.prompt for _, r, _ in rows]
+            cap_new = [self._cap_new([int(r.text.numel())], r.max_new_tokens)[0] for _, r, _ in rows]
             p = self._prefill_inputs(texts, prompts, cap_new, slots=sl)
             ev = timed("prefill_ms")
-            buf.load_rows(p, [draw for *_, draw in new])
+            groups = None
+            if mode == 4:   # (kv_parent, beam_first, beam_n) of each row
+                groups = [(ss[0], ss[0] if len(ss) > 1 else -1, len(ss)) for ss in taken for _ in ss]
+            buf.load_rows(p, [draw for *_, draw in rows], groups)
             h = self._prefill(buf, p, pe_a)
-            L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), k, p.slots_d.data_ptr(),
-                                         C.byref(buf.st), ws.data_ptr(), ws.numel(), L.stream_ptr()), "vb_ar_admit")
+            L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), len(sl),
+                                         p.slots_d.data_ptr(), C.byref(buf.st), ws.data_ptr(), ws.numel(),
+                                         L.stream_ptr()), "vb_ar_admit")
             e = torch.cuda.Event(enable_timing=True)
             e.record()
             ev.append(e)
-            active.update(zip(sl, p.utts([idx for idx, *_ in new], [r.enroll_len for _, r, _ in new])))
+            utts = dict(zip(sl, p.utts([idx for idx, *_ in rows], [r.enroll_len for _, r, _ in rows])))
+            for ss in taken:
+                active[ss[0]] = utts[ss[0]]
+                width[ss[0]] = len(ss)
             device_ids |= any(t.is_cuda for t in texts + prompts)
-            stats.admissions += k
+            stats.admissions += len(new)
 
         def nar(batch):
             ev = timed("nar_ms")
@@ -967,10 +1030,14 @@ class ValleEngine:
 
         def advance():
             """admission, `poll` decode steps and the stop flags; returns the utterances whose codes are ready"""
-            if free and not exhausted:
-                new = pull(len(free))
-                if new:
-                    admit(new)
+            if free and (queue or not exhausted):
+                queue.extend(pull(len(free) - len(queue)))
+                if mode == 4 and buf.st.beam_first is None:
+                    buf.set_groups()
+                taken = _take_slots(free, [r.num_beams for _, r, _ in queue])
+                if taken:
+                    admit(queue[:len(taken)], taken)
+                    del queue[:len(taken)]
             if active:
                 ev = timed("ar_ms")
                 head = heads[mode]
@@ -986,11 +1053,14 @@ class ValleEngine:
                 for s, n in self._stopped(buf, active).items():
                     # copied out now: the slot may be refilled before the NAR batch runs
                     pending.append((active.pop(s), buf.tokens[s, :n].to(torch.int64)))
-                    stats.slot_steps += n
-                    free.append(s)
+                    w = width.pop(s)
+                    if w > 1:   # its rows leave the group: any request may take any of them
+                        buf.beam_first[s:s + w] = -1
+                    stats.slot_steps += n * w
+                    free.extend(range(s, s + w))
                 free.sort()
             ready = []
-            drain = exhausted and not active
+            drain = exhausted and not active and not queue
             while len(pending) >= nar_batch or (drain and pending):
                 batch = pending[:nar_batch]
                 del pending[:nar_batch]
@@ -1003,7 +1073,7 @@ class ValleEngine:
             with torch.cuda.device(dev):
                 ready = advance()
             yield from ready
-            if exhausted and not active and not pending:
+            if exhausted and not active and not pending and not queue:
                 break
         torch.cuda.synchronize(dev)
         for name, evs in phases.items():
@@ -1132,7 +1202,7 @@ class ValleEngine:
         """k decode steps that draw on the device as ONE CUDA graph (captured on first use per (buffer, head tables,
         draw mode, shared prefixes, scores, k))"""
         key = (head.pe, head.predict_w, head.audio_emb, head.greedy, buf.kv_dtype, bool(buf.st.kv_parent),
-               bool(buf.st.logprob), buf.st.beam_width, k)
+               bool(buf.st.logprob), buf.st.beam_width, bool(buf.st.beam_first), k)
         graphs = buf.graphs
         ent = graphs.get(key)
         if ent is None:
