@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define VB_ABI_VERSION 15
+#define VB_ABI_VERSION 16
 
 enum vb_status { VB_OK = 0, VB_ERR_ARG = 1, VB_ERR_CUDA = 2, VB_ERR_UNSUPPORTED = 3 };
 /* storage type of the big matrices / activations.  Accumulation is always fp32.  VB_E4M3: the opt-in FP8 KV cache of
@@ -344,8 +344,10 @@ typedef struct vb_ar_state {
   const int32_t *ras_window;   /* [B] in [0, 256] */
   const int32_t *ras_max;      /* [B] >= 0: fall back when the draw's count in the window exceeds it */
   /* best-of-n decoding (ABI 13): n candidates of one utterance decode side by side and read one copy of their shared
-   * prompt prefix.  NULL means off, so a zero-initialised tail decodes as before.  vb_ar_admit does not use either
-   * field (it admits rows through a state of its own), and continuous batching does not set them. */
+   * prompt prefix.  NULL means off, so a zero-initialised tail decodes as before.  vb_ar_admit scores the first draw
+   * of the rows it admits into logprob (ABI 16) and leaves kv_parent to the caller; continuous batching points the
+   * state at both for best-of requests and scores (vb_ar_fork_prefix gives a sibling the rows the shared read leaves
+   * to its own streams). */
   const int32_t *kv_parent;    /* [B] or NULL (vb_ar_decode_step).  Row b reads its cache rows below
                                   P_b = 16 * floor((text_len[b] + prompt_len[b]) / 16) from row kv_parent[b]'s streams,
                                   and every other row from its own.  Not checked (the step reads no host values): the
@@ -354,7 +356,9 @@ typedef struct vb_ar_state {
                                   wrote them, and a finished row leaves its cache untouched).  The result is bitwise
                                   the step in which row b reads the same rows from its own streams.  bf16 and fp32
                                   caches only: with kv_dtype == VB_E4M3 the step returns VB_ERR_UNSUPPORTED. */
-  float *logprob;              /* [B] or NULL (vb_ar_head.greedy == 2 only: vb_ar_head_step, vb_ar_decode_step).  Each
+  float *logprob;              /* [B] or NULL (vb_ar_head.greedy == 2, or 4 for the rows in no beam group, whose beam
+                                  rows only reduce their logits and add nothing: vb_ar_head_step, vb_ar_decode_step,
+                                  vb_ar_admit, which zeroes the admitted rows' entries before their first draw).  Each
                                   token the seeded sampler appends to row b adds log_softmax(l)[token] to logprob[b],
                                   l = the step's raw fp32 logits over all n_vocab ids (before temperature, top-k and
                                   top-p), in fp32: logsumexp = max + logf(sum expf(l_i - max)).  A step that stops the
@@ -455,8 +459,10 @@ size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab);
  * ras_* included, and for 4 beam_first / beam_n) hold the new utterances' values.  The call runs vb_ar_head_step on a
  * k-row state built from those rows, with n_gen = 0 and finished = 0, so admitted row i gets exactly what
  * vb_ar_head_step on a fresh k-row state gives its row i.
- * Writes, for the slots only: n_gen, finished, tokens[slot, 0], x_cur[slot, :] and logits[slot, 0:n_vocab].  Every other
- * row of every array, the slots' other entries and the KV cache are left unchanged.  No host reads: safe to capture in
+ * Writes, for the slots only: n_gen, finished, tokens[slot, 0], x_cur[slot, :], logits[slot, 0:n_vocab] and, when
+ * st->logprob is set (ABI 16), logprob[slot]: the first draw's log_softmax term as vb_ar_head_step adds it to a zeroed
+ * entry (0 for a row that stops at once, belongs to a beam group, or runs with greedy < 2).  Every other row of every
+ * array, the slots' other entries and the KV cache are left unchanged.  No host reads: safe to capture in
  * a CUDA graph (with per-row groups: when not capturing, the groups and slots are read back and checked).
  * Beam groups (ABI 15, head->greedy == 4): the slots of a group g of n rows are passed together and in order,
  * slots[i..i+n) = g..g+n-1.  Its rows get what vb_ar_head_step with greedy == 3 gives on a fresh state holding the
@@ -466,6 +472,15 @@ size_t vb_ar_admit_workspace(const vb_decoder_desc *desc, int k, int n_vocab);
  * VB_ERR_ARG. */
 int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h, int k, const int32_t *slots,
                 vb_ar_state *st, void *workspace, size_t workspace_bytes, vb_stream_t stream);
+
+/* Shared prompt prefix of an admitted row (ABI 16).  For each of the k rows slots[i] (device int32 [k], in [0, st->B))
+ * whose kv_parent is another row: copy its cache rows [P, S + Tp) of every layer, K and V, from kv_parent's streams
+ * (P = 16 * floor((S + Tp) / 16) as vb_ar_state.kv_parent computes it, S + Tp from the row's text_len and
+ * prompt_len).  Those are the prompt rows the shared read does not cover; with them, a row that was never prefilled
+ * decodes bitwise as if its own prefill had written its cache.  A row that is its own parent is left unchanged, and so
+ * is every other row.  kv_parent, text_len and prompt_len must be set.  bf16 / fp32 caches; VB_E4M3:
+ * VB_ERR_UNSUPPORTED.  No host reads: capturable. */
+int vb_ar_fork_prefix(vb_decoder_t dec, const int32_t *slots, int k, vb_ar_state *st, vb_stream_t stream);
 
 /* one decode step for all B rows: 12 x (LN -> QKV -> KV append -> single-query attention over
  * the cache -> out-proj -> LN -> FFN), then vb_ar_head_step.  Post-LN stacks run

@@ -12,7 +12,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libvalle_b200.so")
 
-ABI_VERSION = 15
+ABI_VERSION = 16
 VB_F32, VB_BF16, VB_E4M3 = 0, 1, 2
 VB_EPI_NONE, VB_EPI_RELU, VB_EPI_RESIDUAL = 0, 1, 2
 VB_MASK_FULL, VB_MASK_VALLE_AR, VB_MASK_PADDED_AR, VB_MASK_PADDED, VB_MASK_DENSE = 0, 1, 2, 3, 4
@@ -164,6 +164,7 @@ PROTOTYPES = {
     "vb_ar_head_step": (C.c_int, [vp, C.POINTER(ArHead), vp, C.POINTER(ArState), vp, C.c_size_t, vp]),
     "vb_ar_admit_workspace": (C.c_size_t, [C.POINTER(DecoderDesc), C.c_int, C.c_int]),
     "vb_ar_admit": (C.c_int, [vp, C.POINTER(ArHead), vp, C.c_int, vp, C.POINTER(ArState), vp, C.c_size_t, vp]),
+    "vb_ar_fork_prefix": (C.c_int, [vp, vp, C.c_int, C.POINTER(ArState), vp]),
     "vb_ar_decode_step": (C.c_int, [vp, C.POINTER(ArHead), C.POINTER(ArState), vp, C.c_size_t, vp]),
     "vb_ar_push_tokens": (C.c_int, [C.POINTER(ArHead), C.POINTER(ArState), vp, C.c_int, vp]),
     "vb_ar_beam_step": (C.c_int, [C.POINTER(ArHead), C.POINTER(ArState), C.c_int, vp, vp]),

@@ -729,6 +729,7 @@ AdmitWs carve_admit_ws(Carve &c, const vb_decoder_desc &D, int k, int n_vocab) {
   cs.beam_fin_score = c.take<float>(k * 8);
   cs.beam_fin_len = c.take<int32_t>(k * 4);
   cs.beam_fin_anc = c.take<uint8_t>(k);
+  cs.logprob = c.take<float>(k * 4);        // the first draw's score (st->logprob set only)
   w.head_ws_bytes = vb_ar_step_workspace(&D, k, kAdmitCap);
   w.head_ws = c.take(w.head_ws_bytes);
   return w;
@@ -757,11 +758,25 @@ VB_API int vb_ar_admit(vb_decoder_t dec, const vb_ar_head *head, const float *h,
   AdmitWs w = carve_admit_ws(c, D, k, head->n_vocab);
   if (head->greedy != 4)
     w.cs.beam_first = w.cs.beam_n = nullptr;
+  if (!st->logprob) w.cs.logprob = nullptr;
   const int ldl = (head->n_vocab + 3) & ~3;
   VB_TRY(launch_ar_admit_copy(st, &w.cs, slots, D.d_model, ldl, head->n_vocab, false, s));
   VB_CHECK_ARG(!D.norm_first || D.final_norm_w, "vb_ar_admit: a pre-LN decoder needs its final norm");
   VB_TRY(head_step(dec, head, h, &w.cs, w.head_ws, w.head_ws_bytes, s));
   return launch_ar_admit_copy(st, &w.cs, slots, D.d_model, ldl, head->n_vocab, true, s);
+}
+
+VB_API int vb_ar_fork_prefix(vb_decoder_t dec, const int32_t *slots, int k, vb_ar_state *st, vb_stream_t stream) {
+  VB_CHECK_ARG(dec && slots && st, "vb_ar_fork_prefix: null argument");
+  if (kv_fp8(st)) {
+    set_error("vb_ar_fork_prefix: kv_parent (shared prompt prefixes) is not supported on the FP8 KV cache");
+    return VB_ERR_UNSUPPORTED;
+  }
+  VB_CHECK_ARG(k >= 1 && k <= st->B, "vb_ar_fork_prefix: k=%d not in [1, B=%d]", k, st->B);
+  VB_CHECK_ARG(st->kv_parent && st->text_len && st->prompt_len && st->kcache && st->vcache,
+               "vb_ar_fork_prefix: needs kv_parent, text_len, prompt_len and the cache");
+  const vb_decoder_desc &D = dec->desc;
+  return launch_ar_fork_prefix(st, D.n_layer, D.n_head, (int)elem_size(D.wdtype), slots, k, (cudaStream_t)stream);
 }
 
 VB_API int vb_cast_from_f32(const float *in, void *out, int dtype, int64_t n, vb_stream_t stream) {

@@ -420,8 +420,12 @@ int launch_ar_sample(float *logits, int64_t ld_logits, const SplitK &in, const v
 int launch_beam_tail(const vb_ar_head *head, vb_ar_state *st, int d, bool pdl, cudaStream_t s, float *lse = nullptr);
 // vb_ar_admit: row i of the k-row state cs <-> row slots[i] of the running state st.  Gather (scatter = false): the
 // lengths and sampler parameters into cs, n_gen / finished / tokens of cs zeroed.  Scatter: n_gen, finished,
-// tokens[., 0], x_cur and logits[., 0:n_vocab] back into the slots
+// tokens[., 0], x_cur and logits[., 0:n_vocab] back into the slots; with cs->logprob, logprob too (zeroed by the gather)
 int launch_ar_admit_copy(vb_ar_state *st, const vb_ar_state *cs, const int32_t *slots, int d, int ldl, int n_vocab,
                          bool scatter, cudaStream_t s);
+// vb_ar_fork_prefix on a bf16 / fp32 cache of `elem`-byte elements: the k rows slots[i] whose kv_parent is another row
+// copy their cache rows [P, S + Tp) of every layer and head, K and V, from the parent's streams
+int launch_ar_fork_prefix(const vb_ar_state *st, int n_layer, int n_head, int elem, const int32_t *slots, int k,
+                          cudaStream_t s);
 
 }  // namespace vb

@@ -706,6 +706,7 @@ ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__
       cs.n_gen[i] = 0;
       cs.finished[i] = 0;
       cs.tokens[i] = 0;
+      if (cs.logprob) cs.logprob[i] = 0.f;
       if (st.sample_seed) {
         const_cast<uint64_t *>(cs.sample_seed)[i] = st.sample_seed[s];
         const_cast<int32_t *>(cs.top_k)[i] = st.top_k[s];
@@ -731,6 +732,7 @@ ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__
     st.n_gen[s] = cs.n_gen[i];
     st.finished[s] = cs.finished[i];
     st.tokens[(int64_t)s * st.tok_stride] = cs.tokens[i];
+    if (cs.logprob) st.logprob[s] = cs.logprob[i];
     if (cs.beam_first && st.beam_first[s] >= 0) {
       st.beam_anc[(int64_t)s * st.tok_stride] = cs.beam_anc[i];
       st.beam_score[s] = cs.beam_score[i];
@@ -748,6 +750,39 @@ ar_admit_copy_kernel(vb_ar_state st, vb_ar_state cs, const int32_t *__restrict__
 int launch_ar_admit_copy(vb_ar_state *st, const vb_ar_state *cs, const int32_t *slots, int d, int ldl, int n_vocab,
                          bool scatter, cudaStream_t s) {
   ar_admit_copy_kernel<<<cs->B, 256, 0, s>>>(*st, *cs, slots, d, ldl, n_vocab, scatter ? 1 : 0);
+  VB_LAUNCH_CHECK();
+  return VB_OK;
+}
+
+// vb_ar_fork_prefix: one CTA per (row i, layer, head).  Row b = slots[i] gets the rows [P_b, S_b + Tp_b) of its K and V
+// streams of that layer and head from its parent's, the rows the shared prompt prefix (kv_shared_rows) leaves to its
+// own streams: at most 15 rows of 64 elements each, copied as 16-byte vectors.  A row that is its own parent is left.
+__global__ void __launch_bounds__(128)
+ar_fork_prefix_kernel(KvCache cache, int64_t layer_stride, const int32_t *__restrict__ slots,
+                      const int32_t *__restrict__ kv_parent, KvRows rows) {
+  const int b = slots[blockIdx.x], l = blockIdx.y, h = blockIdx.z;
+  int par;
+  const int lo = kv_shared_rows(kv_parent, rows, b, par);
+  if (par == b) return;
+  const int hi = min(rows.text_len[b] + rows.prompt_len[b], cache.cap);
+  if (hi <= lo) return;
+  const int vec_row = 64 * cache.elem / 16;      // 16-byte vectors per cached row
+  const int n = (hi - lo) * vec_row;             // of one stream
+  const int64_t layer = (int64_t)l * layer_stride;
+  const int64_t dst = (layer + cache.row(b, h, lo)) * cache.elem / 16, src = (layer + cache.row(par, h, lo)) * cache.elem / 16;
+  for (int t = threadIdx.x; t < 2 * n; t += blockDim.x) {
+    uint4 *base = reinterpret_cast<uint4 *>(t < n ? cache.k : cache.v);
+    const int j = t < n ? t : t - n;
+    base[dst + j] = base[src + j];
+  }
+}
+
+int launch_ar_fork_prefix(const vb_ar_state *st, int n_layer, int n_head, int elem, const int32_t *slots, int k,
+                          cudaStream_t s) {
+  const KvCache cache{st->kcache, st->vcache, nullptr, nullptr, st->cache_seq_stride, st->cache_cap, elem};
+  const KvRows rows{st->text_len, st->prompt_len, st->n_gen, st->finished};
+  ar_fork_prefix_kernel<<<dim3(k, n_layer, n_head), 128, 0, s>>>(cache, st->cache_layer_stride, slots, st->kv_parent,
+                                                                 rows);
   VB_LAUNCH_CHECK();
   return VB_OK;
 }

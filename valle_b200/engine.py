@@ -66,8 +66,8 @@ def _check_utt(who: str, text: torch.Tensor, codes: torch.Tensor, Q: int, name: 
 @dataclass
 class EngineStats:
     """CUDA-event timings (ms) of the phases of the last generate() / generate_stream() call and the number of decode
-    steps; generate_stream() also counts the utterances it admitted into decode slots and the decode steps they ran
-    (slot occupancy = slot_steps / (ar_steps * slots))"""
+    steps; generate_stream() also counts the requests it admitted into decode slots and the decode steps their
+    candidates ran, a beam group's rows counted each (slot occupancy = slot_steps / (ar_steps * slots))"""
     ar_steps: int = 0
     ar_ms: float = 0.0
     prefill_ms: float = 0.0
@@ -92,10 +92,66 @@ class StreamRequest(NamedTuple):
     num_beams: int = 1
 
 
+class BestOfRequest(NamedTuple):
+    """A best-of-n request of ValleEngine.generate_stream: `request` (a StreamRequest, or a tuple in its field order, with
+    a seed s and num_beams == 1) decoded as num_samples candidates, candidate j drawing from seed s + j with the
+    request's top_k / temperature / top_p / ras / max_new_tokens, as generate([text], [prompt], seed=s,
+    num_samples=n) draws them.  It yields the n candidates' codes as a list; num_samples == 1 is the plain request."""
+    request: StreamRequest
+    num_samples: int
+
+
+def _as_request(r):
+    """an item of generate_stream's requests: a BestOfRequest (its request coerced), or a StreamRequest / a tuple in
+    its field order.  BestOfRequest is a tuple too, so it is recognised first."""
+    if isinstance(r, BestOfRequest):
+        return BestOfRequest(StreamRequest(*r.request), r.num_samples)
+    return StreamRequest(*r)
+
+
+class _Candidates:
+    """The candidates of one request in the stream as they decode and come back from the NAR: n rows of a best-of
+    request, or the one utterance of a plain or beam request.  parent: the slot a best-of request was prefilled into,
+    whose cache holds the prompt prefix its other candidates read (kv_parent); it stays held until every candidate has
+    stopped.  None: each candidate's slot is freed when it stops."""
+
+    def __init__(self, index: int, n: int, parent: Optional[int] = None, best_of: bool = False, beam: bool = False):
+        self.index, self.parent, self.best_of, self.beam = index, parent, best_of, beam
+        self.running = set()            # slots of the candidates still decoding
+        self.codes: List[Optional[torch.Tensor]] = [None] * n
+        self.scores: List[Optional[torch.Tensor]] = [None] * n
+        self.left = n                   # candidates not back from the NAR yet
+
+    def stop(self, slot: int) -> List[int]:
+        """the slots freed when the candidate in `slot` stops: its own, except the parent while a candidate still reads
+        it, and the parent with the last candidate"""
+        self.running.discard(slot)
+        freed = [] if slot == self.parent else [slot]
+        if self.parent is not None and not self.running:
+            freed.append(self.parent)
+        return freed
+
+    def done(self, j: int, codes: torch.Tensor, score: Optional[torch.Tensor]) -> bool:
+        """candidate j's codes (and score) from the NAR; True once every candidate is back"""
+        self.codes[j], self.scores[j] = codes, score
+        self.left -= 1
+        return self.left == 0
+
+    def result(self, scores: bool) -> tuple:
+        """(index, codes) or (index, codes, scores): a best-of request's n codes and scores [n], a plain request's codes
+        and scores [1], a beam request's codes and its winner's score (0-d)"""
+        codes = self.codes if self.best_of else self.codes[0]
+        if not scores:
+            return self.index, codes
+        sc = torch.stack(self.scores) if self.best_of else self.scores[0] if self.beam else self.scores[0].view(1)
+        return self.index, codes, sc
+
+
 def _take_slots(free: List[int], widths: Sequence[int]) -> List[List[int]]:
     """First-in first-out admission into decode slots.  widths: the slots each queued request needs, in queue order (1,
-    or n for a beam group of n rows).  Each request takes the lowest run of that many consecutive free slots, up to the
-    first request that finds no such run: it waits, and every request behind it waits too.  free: the free slots,
+    n for a beam group of n rows, or n for the n candidates of a best-of request).  Each request takes the lowest run
+    of that many consecutive free slots, up to the first request that finds no such run: it waits, and every request
+    behind it waits too.  free: the free slots,
     sorted; the taken ones are removed from it.  Returns the slots of the requests that were admitted."""
     out = []
     for n in widths:
@@ -105,6 +161,30 @@ def _take_slots(free: List[int], widths: Sequence[int]) -> List[List[int]]:
         out.append(free[i:i + n])
         del free[i:i + n]
     return out
+
+
+def _stream_draws(idx: int, item, Q: int, n_slots: int, fp8: bool) -> Tuple[StreamRequest, List[_Draw]]:
+    """Request `idx` of generate_stream (a StreamRequest or a BestOfRequest, coerced), validated as generate() would
+    validate it alone, plus n <= n_slots: the request, its num_beams an int, and the draws of its candidates (one for
+    a plain or beam request, n for a best-of request: seeds s + j).  ValueError names the request."""
+    r, n = (item.request, item.num_samples) if isinstance(item, BestOfRequest) else (item, 1)
+    _check_utt(f"request {idx}", r.text, r.prompt, Q)
+    try:
+        beams = _check_num_beams(r.num_beams, r.seed, r.top_k, r.top_p, r.ras, n, None, None, False, fp8)
+        n = _check_num_samples(n, r.seed, False, None, None, False, None)
+    except ValueError as e:
+        raise ValueError(f"request {idx}: {e}") from None
+    if beams > n_slots:
+        raise ValueError(f"request {idx}: num_beams={beams} needs more than the {n_slots} slots")
+    if n > n_slots:
+        raise ValueError(f"request {idx}: num_samples={n} needs more than the {n_slots} slots")
+    seed, top_k = r.seed, r.top_k
+    if seed is None:
+        if top_k != 1 or r.ras is not None:
+            raise ValueError(f"request {idx}: top_k={top_k} / ras need a seed (the seeded device sampler)")
+        seed = 0
+    draws = _draws(n, seed, top_k, r.temperature, r.top_p, None if r.ras is None else [r.ras] * n)
+    return r._replace(num_beams=beams), draws
 
 
 class _ArBuffers:
@@ -204,31 +284,38 @@ class _ArBuffers:
         st.beam_fin_score, st.beam_fin_len = self.beam_fin_score.data_ptr(), self.beam_fin_len.data_ptr()
         st.beam_fin_anc = self.beam_fin_anc.data_ptr()
 
-    def set_groups(self):
-        """Point the state at per-row beam groups (vb_ar_state.beam_first, the stream's mixed head) and at kv_parent,
-        with every row in no group and its own parent; vb_ar_admit starts each group it admits"""
-        self.beam_first.fill_(-1)
+    def set_parents(self):
+        """Point the state at kv_parent, every row its own parent (the stream sets a best-of request's rows to their
+        parent when it admits them)"""
         self.kv_parent.copy_(torch.arange(self.B, dtype=torch.int32))
+        self.st.kv_parent = self.kv_parent.data_ptr()
+
+    def set_groups(self, parents: bool = True):
+        """Point the state at per-row beam groups (vb_ar_state.beam_first, the stream's mixed head), every row in no
+        group, and at kv_parent, every row its own parent (parents=False: keep the kv_parent table the state points at
+        already); vb_ar_admit starts each group it admits"""
+        self.beam_first.fill_(-1)
+        if parents:
+            self.set_parents()
         st = self.st
-        st.beam_first, st.beam_n, st.kv_parent = self.beam_first.data_ptr(), self.beam_n.data_ptr(), \
-            self.kv_parent.data_ptr()
+        st.beam_first, st.beam_n = self.beam_first.data_ptr(), self.beam_n.data_ptr()
         self._point_beams()
 
     def load_rows(self, p: _Prefill, draws: Optional[Sequence[_Draw]] = None,
-                  groups: Optional[Sequence[Tuple[int, int, int]]] = None):
-        """Write the lengths and token caps of prefill block p's utterances into their rows (0..B-1, or p.slots_d)
-        and, given their draws, the sampler columns, all six from one host -> device copy; groups: also each row's
-        (kv_parent, beam_first, beam_n) (set_groups), in the same copy"""
-        rows = None if p.slots_d is None else p.slots_d.long()
+                  groups: Optional[Sequence[Tuple[int, int, int]]] = None, parents: Optional[Sequence[int]] = None):
+        """Write the lengths and token caps of prefill block p's utterances into their rows (0..B-1, or p.slots_d, and
+        the rows forked from them, p.admit_d) and, given their draws, the sampler columns, all six from one host ->
+        device copy; groups: also each row's (kv_parent, beam_first, beam_n) (set_groups), parents: its kv_parent
+        alone (set_parents), in the same copy"""
+        rows = None if p.slots_d is None else (p.slots_d if p.admit_d is None else p.admit_d).long()
 
         def put(col, v):
             if rows is None:
                 col[:len(p.S)].copy_(v)
             else:
                 col.index_copy_(0, rows, v)
-        put(self.text_len, p.S_d)
-        put(self.prompt_len, p.Tp_d)
-        put(self.max_new, p.capn_d)
+        for col, v in ((self.text_len, p.S_d), (self.prompt_len, p.Tp_d), (self.max_new, p.capn_d)):
+            put(col, v if p.gather_d is None else v.index_select(0, p.gather_d))
         if draws is None:
             return
         # _Draw's fields in order; the int64 seeds first, so that every column starts aligned to its element size
@@ -237,6 +324,9 @@ class _ArBuffers:
         if groups is not None:
             cols += [self.kv_parent, self.beam_first, self.beam_n]
             vals += list(zip(*groups))
+        elif parents is not None:
+            cols.append(self.kv_parent)
+            vals.append(tuple(parents))
         block = torch.cat([torch.tensor(v, dtype=c.dtype).view(torch.uint8) for c, v in zip(cols, vals)])
         block = block.to(self.text_len.device, non_blocking=True).split([len(draws) * c.element_size() for c in cols])
         for c, v in zip(cols, block):
@@ -274,6 +364,10 @@ class _Prefill(NamedTuple):
     apos_d: torch.Tensor
     last_d: torch.Tensor
     slots_d: Optional[torch.Tensor]
+    # rows admitted next to the prefilled ones that take an utterance's prefill (vb_ar_fork_prefix): every admitted
+    # row's slot, slots_d's then the forked rows', and the utterance each takes its lengths and last prefill row from
+    admit_d: Optional[torch.Tensor] = None
+    gather_d: Optional[torch.Tensor] = None
 
     def utts(self, index: Sequence[int], enroll_lens: Sequence[Optional[int]]) -> List[_Utt]:
         return [_Utt(i, t, pr, tp, None if e is None else int(e)) for i, t, pr, tp, e in
@@ -871,8 +965,9 @@ class ValleEngine:
         return [host[cu_g[b]:cu_g[b + 1]] for b in range(len(rows))], logprob
 
     def generate_stream(self, requests: Iterable, slots: Optional[int] = None, max_context: Optional[int] = None,
-                        poll: int = 32, nar_batch: Optional[int] = None) -> Iterator[Tuple[int, torch.Tensor]]:
-        """Continuous batching: decode `requests` (StreamRequest records, or tuples in its field order) in `slots`
+                        poll: int = 32, nar_batch: Optional[int] = None, return_scores: bool = False) -> Iterator[tuple]:
+        """Continuous batching: decode `requests` (StreamRequest or BestOfRequest records, or tuples in
+        StreamRequest's field order) in `slots`
         decode rows, refilling a row with the next request as soon as its utterance stops, and yield (index, codes) in
         completion order.  codes: int64 [Tgen, Q] on the device, what generate() returns for that utterance; index:
         the request's position in `requests`.
@@ -887,32 +982,49 @@ class ValleEngine:
         the slot or the schedule.  A request with num_beams=n > 1 is decoded by beam search (generate(num_beams=n)'s
         rules; not on the FP8 cache, n <= slots) in n consecutive slots that read one copy of its prompt prefix and are
         freed together; requests are admitted first in, first out, so one that finds no run of n free slots waits, and
-        the requests behind it with it.  Its codes are those of generate(num_beams=n) on it alone."""
+        the requests behind it with it.  Its codes are those of generate(num_beams=n) on it alone.
+
+        A BestOfRequest(request, n) (a seed s, n <= slots, no beams) decodes n seeded candidates in n consecutive
+        slots, candidate j drawing from seed s + j, and yields the list of their n codes, bit for bit
+        generate([text], [prompt], seed=s, num_samples=n)[0] (with the KV split count caveat of any batch).  On the
+        bf16 and fp32 caches the request is prefilled once, into its first slot, whose prompt prefix the other
+        candidates read; that slot is held until every candidate has stopped, every other one is freed as its
+        candidate stops.  On the FP8 cache each candidate is a row of its own.  The candidates go to the NAR as they
+        stop (nar_batch counts candidates); the request is yielded once all n are through.
+
+        return_scores=True yields (index, codes, scores): scores a device fp32 tensor, what
+        generate(..., return_scores=True, return_device=True)[1][0] gives for the request alone: [1] for a request,
+        [n] for a best-of request, the winner's score (0-d) for a beam request.  A greedy request without a seed is
+        scored as generate(seed=0) scores it; every request then runs the seeded sampler's head."""
         with torch.cuda.device(self.device):
             self._refresh()
         kv_dtype = self.kv_cache_dtype()
         if self.sample_on_host:
             raise ValueError("generate_stream draws on the device: sample_on_host = True is not supported")
         if isinstance(requests, (list, tuple)):
-            reqs = [StreamRequest(*r) for r in requests]
+            reqs = [_as_request(r) for r in requests]
             if not reqs:
                 return iter(())
             if max_context is None:
-                max_context = max(self._context(r) for r in reqs)
-            slots = min(len(reqs), self.max_tc_batch) if slots is None else slots
+                max_context = max(self._context(r.request if isinstance(r, BestOfRequest) else r) for r in reqs)
+
+            def rows(r):   # the candidates of a best-of request (validated when the request is pulled)
+                n = r.num_samples if isinstance(r, BestOfRequest) else 1
+                return int(n) if isinstance(n, (int, np.integer)) and not isinstance(n, bool) and n > 1 else 1
+            slots = min(sum(rows(r) for r in reqs), self.max_tc_batch) if slots is None else slots
             it = iter(reqs)
         else:
             if max_context is None:
                 raise ValueError("generate_stream: an iterator of requests needs max_context")
             slots = self.max_tc_batch if slots is None else slots
-            it = (StreamRequest(*r) for r in requests)
+            it = (_as_request(r) for r in requests)
         slots, poll = int(slots), int(poll)
         nar_batch = slots if nar_batch is None else int(nar_batch)
         if slots < 1 or poll < 1 or nar_batch < 1:
             raise ValueError("generate_stream: slots, poll and nar_batch must be >= 1")
         if self.dtype == torch.bfloat16 and slots > self.max_tc_batch:
             raise ValueError(f"generate_stream: bf16 decodes at most {self.max_tc_batch} slots (got {slots})")
-        return self._stream(it, slots, int(max_context), poll, nar_batch, kv_dtype)
+        return self._stream(it, slots, int(max_context), poll, nar_batch, kv_dtype, bool(return_scores))
 
     def _context(self, r: StreamRequest) -> int:
         """KV-cache rows a request needs: text + prompt + the most tokens it may generate + 2"""
@@ -920,11 +1032,14 @@ class ValleEngine:
         return S + int(r.prompt.shape[0]) + self._cap_new([S], r.max_new_tokens)[0] + 2
 
     @torch.no_grad()
-    def _stream(self, it, n_slots: int, max_context: int, poll: int, nar_batch: int, kv_dtype):
+    def _stream(self, it, n_slots: int, max_context: int, poll: int, nar_batch: int, kv_dtype, scores: bool = False):
         m, dev, Q = self.model, self.device, self.Q
         cap = (max_context + 63) // 64 * 64
         tok_stride = (max_context + 2 + 7) // 8 * 8
         pm = self.prefix_mode
+        # a best-of request's candidates read one prefill of its prompt (kv_parent); the FP8 cache refuses kv_parent,
+        # and its shared read is no faster there (DESIGN section 7): each candidate is prefilled into its own slot
+        fork = kv_dtype is None
         stats = EngineStats()
         phases: Dict[str, list] = {"prefill_ms": [], "ar_ms": [], "nar_ms": []}
 
@@ -939,23 +1054,33 @@ class ValleEngine:
             buf.n_gen.zero_()
             buf.finished.fill_(1)              # a slot that is never filled never runs, nor reads its sampler columns
             buf.x_cur.zero_()
-            buf.set_best_of(n_slots, 1, False)   # no shared prefixes or scores: slots are refilled one by one
+            # no shared prefixes yet; logprob zeroed with scores
+            buf.set_best_of(n_slots, 1, scores)
             pe_a = self._pe(m.ar_audio_position, cap + 2)
             heads = {g: self._head(pe_a, g) for g in (1, 2, 4)}
             ws = torch.empty(self.lib.vb_ar_admit_workspace(C.byref(self.ar.desc), n_slots, self.n_vocab),
                              dtype=torch.uint8, device=dev)
-        # 2 (the seeded sampler) from the first seeded request on, 4 (2 next to beam groups) from the first beam request
-        mode = 1
+        # 2 (the seeded sampler) from the first seeded request on, or from the start with scores (scores keep the seeded
+        # sampler, as in generate()); 4 (2 next to beam groups) from the first beam request
+        mode = 2 if scores else 1
+        shared = False                         # a best-of request reads its parent's prompt prefix (kv_parent)
         free = list(range(n_slots))
-        queue: List[Tuple[int, StreamRequest, _Draw]] = []   # pulled requests waiting for slots, in order
+        # pulled requests waiting for slots, in order: (index, request, the draws of its candidates)
+        queue: List[Tuple[int, StreamRequest, List[_Draw]]] = []
         active: Dict[int, _Utt] = {}           # slot -> the utterance decoding in it (a beam group's first slot)
         width: Dict[int, int] = {}             # active slot -> the slots its utterance holds from there on
-        pending: List[Tuple[_Utt, torch.Tensor]] = []   # finished utterances and their codes, waiting for the NAR
+        cand: Dict[int, Tuple[_Candidates, int]] = {}   # active slot -> its request's candidates, and which one
+        # stopped candidates waiting for the NAR: utterance, codes, request, candidate, score
+        pending: List[Tuple[_Utt, torch.Tensor, _Candidates, int, Optional[torch.Tensor]]] = []
         n_pulled, exhausted, device_ids = 0, False, False
 
+        def slots_of(q):
+            _, r, draws = q
+            return r.num_beams if r.num_beams > 1 else len(draws)
+
         def pull(k):
-            """up to k validated requests: (index, request, draw)"""
-            nonlocal n_pulled, exhausted, mode
+            """up to k validated requests: (index, request, the draws of its candidates)"""
+            nonlocal n_pulled, exhausted, mode, shared
             out = []
             while len(out) < k and not exhausted:
                 try:
@@ -965,76 +1090,102 @@ class ValleEngine:
                     break
                 idx = n_pulled
                 n_pulled += 1
-                _check_utt(f"request {idx}", r.text, r.prompt, Q)
-                try:
-                    beams = _check_num_beams(r.num_beams, r.seed, r.top_k, r.top_p, r.ras, 1, None, None, False,
-                                             kv_dtype is not None)
-                except ValueError as e:
-                    raise ValueError(f"request {idx}: {e}") from None
-                if beams > n_slots:
-                    raise ValueError(f"request {idx}: num_beams={beams} needs more than the {n_slots} slots")
-                seed, top_k = r.seed, r.top_k
-                if seed is None:
-                    if top_k != 1 or r.ras is not None:
-                        raise ValueError(f"request {idx}: top_k={top_k} / ras need a seed (the seeded device sampler)")
-                    seed = 0
-                draw = _draws(1, seed, top_k, r.temperature, r.top_p, None if r.ras is None else [r.ras])[0]
+                r, draws = _stream_draws(idx, r, Q, n_slots, kv_dtype is not None)
+                beams = r.num_beams
                 if pm in (2, 4) and r.enroll_len is None:
                     raise ValueError(f"request {idx}: prefix_mode {pm} needs enroll_len")
                 if self._context(r) > max_context:
                     raise ValueError(f"request {idx} needs {self._context(r)} KV-cache rows > max_context={max_context}")
                 if beams > 1:
                     mode = 4
-                elif not draw.greedy:
+                elif not all(d.greedy for d in draws):
                     mode = max(mode, 2)
-                out.append((idx, r._replace(num_beams=beams), draw))
+                shared |= len(draws) > 1 and fork
+                out.append((idx, r, draws))
             return out
 
         def admit(new, taken):
             """the requests `new`, each into its slots of `taken`: a beam group's n rows are its request n times, the
-            prefill writing each row's own cache streams"""
+            prefill writing each row's own cache streams; a best-of request's candidates are its request n times too,
+            except where they share its prompt prefix: then its first slot (the parent) is prefilled alone, and the
+            other candidates read the prefix below P from it and get the rows from P on copied (vb_ar_fork_prefix)"""
             nonlocal device_ids
-            rows = [q for q, sl in zip(new, taken) for _ in sl]
-            sl = [s for ss in taken for s in ss]
-            texts = [r.text for _, r, _ in rows]
-            prompts = [r.prompt for _, r, _ in rows]
-            cap_new = [self._cap_new([int(r.text.numel())], r.max_new_tokens)[0] for _, r, _ in rows]
-            p = self._prefill_inputs(texts, prompts, cap_new, slots=sl)
+            pre, forked = [], []   # (request, slot, candidate, its slots' first, the prefill row it takes)
+            for q, ss in zip(new, taken):
+                _, r, draws = q
+                parent = len(pre)
+                for j, sl in enumerate(ss):
+                    row = (q, sl, j, ss[0], parent)
+                    if j > 0 and len(draws) > 1 and fork:
+                        forked.append(row)
+                    else:
+                        pre.append(row[:4] + (len(pre),))
+            rows = pre + forked
+            texts = [q[1].text for q, *_ in pre]
+            prompts = [q[1].prompt for q, *_ in pre]
+            cap_new = [self._cap_new([int(q[1].text.numel())], q[1].max_new_tokens)[0] for q, *_ in pre]
+            p = self._prefill_inputs(texts, prompts, cap_new, slots=[sl for _, sl, *_ in pre],
+                                     forks=([sl for _, sl, *_ in forked], [i for *_, i in forked]) if forked else None)
             ev = timed("prefill_ms")
-            groups = None
+            # each row's kv_parent: a beam group's and a shared best-of request's first slot, else the row itself
+            kvp = [first if q[1].num_beams > 1 or (len(q[2]) > 1 and fork) else sl for q, sl, _, first, _ in rows]
+            groups = parents = None
             if mode == 4:   # (kv_parent, beam_first, beam_n) of each row
-                groups = [(ss[0], ss[0] if len(ss) > 1 else -1, len(ss)) for ss in taken for _ in ss]
-            buf.load_rows(p, [draw for *_, draw in rows], groups)
+                groups = [(kp, first if q[1].num_beams > 1 else -1, slots_of(q))
+                          for kp, (q, _, _, first, _) in zip(kvp, rows)]
+            elif buf.st.kv_parent is not None:
+                parents = kvp
+            buf.load_rows(p, [q[2][j if len(q[2]) > 1 else 0] for q, _, j, *_ in rows], groups, parents)
             h = self._prefill(buf, p, pe_a)
-            L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), len(sl),
-                                         p.slots_d.data_ptr(), C.byref(buf.st), ws.data_ptr(), ws.numel(),
+            slots_d = p.slots_d
+            if forked:
+                slots_d = p.admit_d
+                h = ops.gather_rows(h, p.gather_d)
+                L.check(self.lib.vb_ar_fork_prefix(self.ar.handle, p.admit_d[len(pre):].data_ptr(), len(forked),
+                                                   C.byref(buf.st), L.stream_ptr()), "vb_ar_fork_prefix")
+            L.check(self.lib.vb_ar_admit(self.ar.handle, C.byref(heads[mode]), h.data_ptr(), len(rows),
+                                         slots_d.data_ptr(), C.byref(buf.st), ws.data_ptr(), ws.numel(),
                                          L.stream_ptr()), "vb_ar_admit")
             e = torch.cuda.Event(enable_timing=True)
             e.record()
             ev.append(e)
-            utts = dict(zip(sl, p.utts([idx for idx, *_ in rows], [r.enroll_len for _, r, _ in rows])))
-            for ss in taken:
-                active[ss[0]] = utts[ss[0]]
-                width[ss[0]] = len(ss)
+            utts = p.utts([q[0] for q, *_ in pre], [q[1].enroll_len for q, *_ in pre])
+            reqs = {}
+            for q, ss in zip(new, taken):
+                idx, r, draws = q
+                beam = r.num_beams > 1
+                reqs[idx] = _Candidates(idx, 1 if beam else len(draws), ss[0] if len(draws) > 1 and fork else None,
+                                        len(draws) > 1, beam)
+            for q, sl, j, first, i in rows:
+                if q[1].num_beams > 1 and sl != first:
+                    continue   # a beam group decodes as its first slot
+                active[sl], width[sl], cand[sl] = utts[i], slots_of(q) if q[1].num_beams > 1 else 1, (reqs[q[0]], j)
+                reqs[q[0]].running.add(sl)
             device_ids |= any(t.is_cuda for t in texts + prompts)
             stats.admissions += len(new)
 
         def nar(batch):
             ev = timed("nar_ms")
-            codes, cu_g = self._nar([u for u, _ in batch], [int(c.shape[0]) for _, c in batch],
-                                    torch.cat([c for _, c in batch]))
+            codes, cu_g = self._nar([u for u, *_ in batch], [int(c.shape[0]) for _, c, *_ in batch],
+                                    torch.cat([c for _, c, *_ in batch]))
             e = torch.cuda.Event(enable_timing=True)
             e.record()
             ev.append(e)
-            return [(u.index, codes[cu_g[i]:cu_g[i + 1]]) for i, (u, _) in enumerate(batch)]
+            out = []
+            for i, (_, _, req, j, sc) in enumerate(batch):
+                if req.done(j, codes[cu_g[i]:cu_g[i + 1]], sc):
+                    out.append(req.result(scores))
+            return out
 
         def advance():
-            """admission, `poll` decode steps and the stop flags; returns the utterances whose codes are ready"""
+            """admission, `poll` decode steps and the stop flags; returns the requests whose codes are ready"""
             if free and (queue or not exhausted):
                 queue.extend(pull(len(free) - len(queue)))
                 if mode == 4 and buf.st.beam_first is None:
-                    buf.set_groups()
-                taken = _take_slots(free, [r.num_beams for _, r, _ in queue])
+                    buf.set_groups(parents=buf.st.kv_parent is None)
+                if shared and buf.st.kv_parent is None:
+                    buf.set_parents()
+                taken = _take_slots(free, [slots_of(q) for q in queue])
                 if taken:
                     admit(queue[:len(taken)], taken)
                     del queue[:len(taken)]
@@ -1051,13 +1202,17 @@ class ValleEngine:
                 ev.append(e)
                 stats.ar_steps += poll
                 for s, n in self._stopped(buf, active).items():
-                    # copied out now: the slot may be refilled before the NAR batch runs
-                    pending.append((active.pop(s), buf.tokens[s, :n].to(torch.int64)))
                     w = width.pop(s)
+                    req, j = cand.pop(s)
+                    # copied out now: the slot may be refilled before the NAR batch runs
+                    sc = (buf.beam_score if w > 1 else buf.logprob)[s].clone() if scores else None
+                    pending.append((active.pop(s), buf.tokens[s, :n].to(torch.int64), req, j, sc))
+                    freed = req.stop(s)
                     if w > 1:   # its rows leave the group: any request may take any of them
                         buf.beam_first[s:s + w] = -1
+                        freed = list(range(s, s + w))
                     stats.slot_steps += n * w
-                    free.extend(range(s, s + w))
+                    free.extend(freed)
                 free.sort()
             ready = []
             drain = exhausted and not active and not queue
@@ -1111,9 +1266,11 @@ class ValleEngine:
             out[s] = n_gen[s]
         return out
 
-    def _prefill_inputs(self, texts, prompts, cap_new, slots: Optional[Sequence[int]] = None) -> _Prefill:
+    def _prefill_inputs(self, texts, prompts, cap_new, slots: Optional[Sequence[int]] = None,
+                        forks: Optional[Tuple[Sequence[int], Sequence[int]]] = None) -> _Prefill:
         """the host -> device copies of one packed AR prefill (ids, and one int32 block of lengths and row maps);
-        slots: the decode slots the utterances go to (generate_stream)"""
+        slots: the decode slots the utterances go to (generate_stream); forks: (slots, utterances) of rows admitted
+        without a prefill of their own, each taking utterance i's (a best-of request's other candidates)"""
         dev, Q = self.device, self.Q
         B = len(texts)
         S = [int(t.numel()) for t in texts]
@@ -1129,11 +1286,18 @@ class ValleEngine:
         cu_np = _offsets(seq_len)
         text_rows, text_pos = _seg_ranges(cu_np[:-1], S)
         aud_rows, aud_pos = _seg_ranges(cu_np[:-1] + np.asarray(S, dtype=np.int64), Tp)
+        fs, fi = ([], []) if forks is None else forks
         meta = torch.from_numpy(np.concatenate([cu_np, S, Tp, cap_new, text_rows, text_pos, aud_rows, aud_pos,
-                                                cu_np[1:] - 1, [] if slots is None else slots]).astype(np.int32)
+                                                cu_np[1:] - 1, [] if slots is None else slots, fs,
+                                                [] if forks is None else list(range(B)) + list(fi)]).astype(np.int32)
                                 ).to(dev, non_blocking=True)
-        v = meta.split([B + 1, B, B, B, sum(S), sum(S), sum(Tp), sum(Tp), B, 0 if slots is None else B])
-        return _Prefill(S, Tp, Tp_nar, text_all, prm_all, ar_tok, *v[:-1], None if slots is None else v[-1])
+        sizes = [B + 1, B, B, B, sum(S), sum(S), sum(Tp), sum(Tp), B, 0 if slots is None else B]
+        v = meta.split(sizes + [len(fs), len(fs) + B if forks else 0])
+        admit_d = gather_d = None
+        if forks is not None:   # slots_d and the forked rows' slots, as one array
+            admit_d, gather_d = meta.narrow(0, sum(sizes) - B, B + len(fs)), v[-1]
+        return _Prefill(S, Tp, Tp_nar, text_all, prm_all, ar_tok, *v[:9], None if slots is None else v[9], admit_d,
+                        gather_d)
 
     def _prefill(self, buf: _ArBuffers, p: _Prefill, pe_a: torch.Tensor) -> torch.Tensor:
         """embedding (+ pre-net) + positions of every [text | prompt] row and the AR prefill (valle.py:995-997,

@@ -258,15 +258,19 @@ class VALLE(nn.Module):
                                            num_beams=num_beams)
 
     def inference_stream(self, requests, slots: Optional[int] = None, max_context: Optional[int] = None,
-                         poll: int = 32, nar_batch: Optional[int] = None, dtype: Optional[torch.dtype] = None):
+                         poll: int = 32, nar_batch: Optional[int] = None, dtype: Optional[torch.dtype] = None,
+                         return_scores: bool = False):
         """Engine feature: continuous batching (ValleEngine.generate_stream).  requests: StreamRequest records
-        (text, prompt, enroll_len, seed, top_k, temperature, max_new_tokens, top_p, ras, num_beams), a sequence or a
-        lazy iterator; yields (index, codes [Tgen, 8] on the GPU) as each utterance completes, codes equal to
-        `inference()` of that request alone (`inference_batch([...], num_beams=n)[0]` for num_beams=n > 1: beam search
-        in n decode slots, next to the other requests).  Decodes in `engine_dtype` (or `dtype`) with the model's
-        `kv_cache_dtype`."""
+        (text, prompt, enroll_len, seed, top_k, temperature, max_new_tokens, top_p, ras, num_beams) or
+        BestOfRequest(request, n) records, a sequence or a lazy iterator; yields (index, codes [Tgen, 8] on the GPU) as
+        each utterance completes, codes equal to `inference()` of that request alone (`inference_batch([...],
+        num_beams=n)[0]` for num_beams=n > 1: beam search in n decode slots, next to the other requests; for a
+        BestOfRequest the list of its n candidates' codes, `inference_batch([...], seed=s, num_samples=n)[0]`).
+        return_scores=True yields (index, codes, scores), the AR log-likelihoods `inference_batch(...,
+        return_scores=True)` reports for the request, on the GPU.  Decodes in `engine_dtype` (or `dtype`) with the
+        model's `kv_cache_dtype`."""
         return self.engine(dtype).generate_stream(requests, slots=slots, max_context=max_context, poll=poll,
-                                                  nar_batch=nar_batch)
+                                                  nar_batch=nar_batch, return_scores=return_scores)
 
     @torch.no_grad()
     def continual(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
