@@ -269,6 +269,16 @@ attn_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_qkv, int n_head, cons
     __syncwarp();
     mbar_wait(&full_bar[stage], phase);
     uint8_t *sk = ring + stage * kStageBytes;
+    // The tail tile's box runs past the sequence: into the next one's rows, or TMA's zero fill past M.  P is 0 there,
+    // but 0 * inf and 0 * NaN are NaN in P V, so the working warpgroups zero those V rows (whole 128-byte rows: the
+    // swizzle stays within a row) and make the zeros visible to the wgmma before either warpgroup's P V reads them.
+    // Only the last tile can be the tail tile (n_tiles <= ceil(L / 64)).
+    if (j0 + BKV > L) {
+      uint4 *sv = reinterpret_cast<uint4 *>(sk + kBoxBytes);
+      for (int i = (L - j0) * 8 + threadIdx.x; i < BKV * 8; i += 128 * n_wg) sv[i] = make_uint4(0u, 0u, 0u, 0u);
+      fence_proxy_async_smem();
+      named_bar_sync(1, 128 * n_wg);
+    }
     float s[32], corr_a, corr_b;
     issue_qk(s, sk);
     wgmma_wait<0>();
