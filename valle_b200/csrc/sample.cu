@@ -22,7 +22,12 @@ struct ArgMax {
   int i;
 };
 __device__ __forceinline__ ArgMax better(ArgMax a, ArgMax b) {
-  // larger value wins; on ties the smaller index (torch.argmax returns the first maximum)
+  // larger value wins; on ties the smaller index (torch.argmax returns the first maximum).  torch.argmax also takes
+  // NaN as the maximum, the first NaN first: a NaN beats any number, and the smaller index wins between NaNs.  Without
+  // that rule a row of NaN would keep the initial {-inf, 0x7fffffff} and the NAR tail would read next_emb far out of
+  // bounds.  For rows without NaN the result is the same as the plain comparison.
+  const bool an = a.v != a.v, bn = b.v != b.v;
+  if (an || bn) return (bn && (!an || b.i < a.i)) ? b : a;
   return (b.v > a.v || (b.v == a.v && b.i < a.i)) ? b : a;
 }
 __device__ __forceinline__ ArgMax warp_argmax(ArgMax a) {
