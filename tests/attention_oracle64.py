@@ -189,6 +189,134 @@ def ratio(got: torch.Tensor, ref: Ref, bnd: torch.Tensor) -> float:
     return float(r.max()) if r.numel() else 0.0
 
 
+# -------------------------------------------------------------------------------------------------------- backward
+def _probs(q, k, vis):
+    s = (q @ k.transpose(-1, -2)) * 0.125
+    s = s.masked_fill(~vis, -math.inf)
+    m = s.amax(-1, keepdim=True)
+    m = torch.where(torch.isfinite(m), m, torch.zeros_like(m))
+    p = torch.exp(s - m)
+    l = p.sum(-1, keepdim=True)
+    return s, m, p / torch.where(l > 0, l, torch.ones_like(l)), m + torch.log(torch.where(l > 0, l, torch.ones_like(l)))
+
+
+def attention_bwd64(q, k, v, o, dO, vis, w=None, head_chunk: int = 4):
+    """(dq, dk, dv) [H, L, 64] float64 of O = (P o w) V, P = softmax(q k^T / 8 + mask), for the output gradient dO:
+    dV = (P o w)^T dO, dP = w o (dO V^T), D = rowsum(dO o o), dS = P o (dP - D), dQ = dS K / 8, dK = dS^T Q / 8.
+    D is formed from the `o` given; w: the dropout scale [H, L, L] (None: no dropout)."""
+    H = q.shape[0]
+    out = ([], [], [])
+    for h0 in range(0, H, head_chunk):
+        sl = slice(h0, h0 + head_chunk)
+        qh, kh, vh, oh, gh = (t[sl].double() for t in (q, k, v, o, dO))
+        _, _, P, _ = _probs(qh, kh, vis)
+        Pw = P if w is None else P * w[sl]
+        dP = gh @ vh.transpose(-1, -2)
+        if w is not None:
+            dP = dP * w[sl]
+        dS = P * (dP - (gh * oh).sum(-1, keepdim=True))
+        out[0].append(dS @ kh * 0.125)
+        out[1].append(dS.transpose(-1, -2) @ qh * 0.125)
+        out[2].append(Pw.transpose(-1, -2) @ gh)
+    return tuple(torch.cat(t) for t in out)
+
+
+def bwd_bound(q, k, v, o_st, dO, vis, w=None, head_chunk: int = 4):
+    """(exact, bound) for dq, dk, dv of `attn_bwd_dq_kernel` / `attn_bwd_dkv_kernel` (csrc/backward.cu), each
+    [H, L, 64] float64, from the inputs the kernels read: q, k, v [H, L, 64], the stored output o_st and dO (all
+    already rounded as stored) and the dropout scale w [H, L, L] (None: none).  `exact` is the true
+    gradient: attention_bwd64 with D formed from the float64 output O = (P o w) V, not from o_st.
+
+    The kernels, in fp32 over 64 x 64 tiles, sums as fmaf chains in order (u = 2^-24; the score and product sums
+    get 2u, as `score_error`):
+      p:   p^ = expf(s^ / 8 - lse^) = P (1 + eta).  The score error E (`score_error`), lse = m + logf(l) from the
+           online sweep: l is off by gamma_{L+64}, logf adds 2^-23, the sum m + log l one u |lse|; s / 8 - lse one u
+           (|s / 8| + |lse|) and expf 2^-22: eta <= E + gamma_{L+64}(2u) + 2^-21 (|s / 8| + |lse| + 2).
+      dP:  dP^ = dP + e, |e| <= gamma_64(2u) |dO| |V|^T; the dropout scale one more u |w dP|.
+      D:   D^ = rowsum(dO o o_st) in 16-term chains and two shuffle adds: |D^ - D| <= gamma_64(2u) rowsum |dO| |o_st|
+           + rowsum |dO| |o_st - O|, the second the stored output's own rounding, which D inherits.
+      dS:  fl(p^ fl(dP^ - D^)): the errors above are absolute, so the cancellation in dP - D costs nothing extra:
+           |dS^ - dS| <= P (|e| + u |w dP| + |D^ - D|) + (eta + 2u) P |w dP - D| =: e_S.
+      sums: dQ = sum over key tiles of dS K (one fmaf chain of kv_max <= L terms), dK over query tiles (L terms):
+           |dQ^ - dQ| <= (e_S |K| + gamma_{L+64}(u) |dS| |K|) / 8, dK the same with dS^T and |Q|;
+           dV = sum_q fl(p^ w) dO: |dV^ - dV| <= ((eta + u) P w)^T |dO| + gamma_{L+64}(u) (P w)^T |dO|.
+      out: the scale by 1/8 is exact; a bf16 store adds half_ulp(out), which the caller adds
+           (stack_oracle64.attn_bwd_ratio), as it has the output.
+    Bound: the first-order sum times 1 + 2^-5, + 2^-120.  A key no query sees and a query that sees no key get a
+    bound of 2^-120 (+ the half ulp of 0): their gradient rows must be exactly 0."""
+    H, L, _ = q.shape
+    u, g64 = U_F32, gamma(HD, 2 * U_F32)
+    gL = gamma(L + 64, 2 * U_F32)
+    ex, bd = ([], [], []), ([], [], [])
+    for h0 in range(0, H, head_chunk):
+        sl = slice(h0, h0 + head_chunk)
+        qh, kh, vh, oh, gh = (t[sl].double() for t in (q, k, v, o_st, dO))
+        s, m, P, lse = _probs(qh, kh, vis)
+        E = score_error(qh, kh, s, m, vis)[..., None]
+        ww = torch.ones_like(P) if w is None else w[sl].double()
+        Pw = P * ww
+        O = Pw @ vh
+        dP = gh @ vh.transpose(-1, -2)
+        D = (gh * O).sum(-1, keepdim=True)
+        wdP = ww * dP
+        dS = P * (wdP - D)
+        sfin = torch.where(vis, s.abs(), torch.zeros_like(s))
+        eta = E + gL + 2.0 ** -21 * (sfin + lse.abs() + 2)
+        e_dp = g64 * (gh.abs() @ vh.abs().transpose(-1, -2)) * ww + u * wdP.abs()
+        e_D = g64 * (gh.abs() * oh.abs()).sum(-1, keepdim=True) + (gh.abs() * (oh - O).abs()).sum(-1, keepdim=True)
+        e_S = P * (e_dp + e_D) + (eta + 2 * u) * P * (wdP - D).abs()
+        ex[0].append(dS @ kh * 0.125)
+        ex[1].append(dS.transpose(-1, -2) @ qh * 0.125)
+        ex[2].append(Pw.transpose(-1, -2) @ gh)
+        aS = dS.abs()
+        bd[0].append((e_S @ kh.abs() + gL * aS @ kh.abs()) * 0.125)
+        bd[1].append((e_S.transpose(-1, -2) @ qh.abs() + gL * aS.transpose(-1, -2) @ qh.abs()) * 0.125)
+        bd[2].append((((eta + u) * Pw).transpose(-1, -2) + gL * Pw.transpose(-1, -2)) @ gh.abs())
+    exact = tuple(torch.cat(t) for t in ex)
+    return exact, tuple(torch.cat(b) * (1 + 2.0 ** -5) + 2.0 ** -120 for b in bd)
+
+
+def emulate_bwd(q, k, v, o, dO, vis, w=None, out_dtype=torch.float32, skip_last_q_tile=False,
+                skip_last_k_tile=False, d_dims=HD, drop_dp=True):
+    """the arithmetic of attn_bwd_dq_kernel / attn_bwd_dkv_kernel in fp32 on the stored inputs (q, k, v, o, dO
+    [H, L, 64] of the storage dtype): lse by the online sweep over 64-key tiles, D = rowsum(dO o o) in fp32, p =
+    exp(s / 8 - lse), dS = p (w dP - D), dQ summed over key tiles in order, dK / dV over query tiles in order, then
+    the store.  The keyword arguments plant mistakes: dK / dV skipping the last partial query tile, dQ skipping the
+    last key tile, D over the first d_dims head dims, the dropout scale on P but not on dP (drop_dp=False)."""
+    H, L, _ = q.shape
+    qf, kf, vf, of, gf = (t.float() for t in (q, k, v, o, dO))
+    s = (qf @ kf.transpose(-1, -2)) * 0.125
+    s = s.masked_fill(~vis, -math.inf)
+    m = torch.full((H, L), -math.inf)
+    l = torch.zeros(H, L)
+    for j0 in range(0, L, BKV):
+        t = s[..., j0:j0 + BKV]
+        mn = torch.maximum(m, t.amax(-1))
+        mu = torch.where(mn == -math.inf, torch.zeros_like(mn), mn)
+        l = l * torch.exp(m - mu) + torch.exp(t - mu[..., None]).sum(-1)
+        m = mn
+    lse = torch.where(l > 0, m + torch.log(l), torch.full_like(l, math.inf))
+    D = (gf[..., :d_dims] * of[..., :d_dims]).sum(-1, keepdim=True)
+    p = torch.exp(s - lse[..., None])
+    dP = gf @ vf.transpose(-1, -2)
+    wf = torch.ones(H, L, L) if w is None else w.float()
+    dS = p * ((dP * wf if drop_dp else dP) - D)
+    pw = p * wf
+    dq = torch.zeros(H, L, HD)
+    n_kt = -(-L // BKV)
+    for j0 in range(0, L, BKV):
+        if skip_last_k_tile and j0 // BKV == n_kt - 1 and n_kt > 1:
+            break
+        dq = dq + dS[..., j0:j0 + BKV] @ kf[:, j0:j0 + BKV]
+    dk, dv = torch.zeros(H, L, HD), torch.zeros(H, L, HD)
+    for q0 in range(0, L, BKV):
+        if skip_last_q_tile and q0 + BKV > L:
+            break
+        dk = dk + dS[:, q0:q0 + BKV].transpose(-1, -2) @ qf[:, q0:q0 + BKV]
+        dv = dv + pw[:, q0:q0 + BKV].transpose(-1, -2) @ gf[:, q0:q0 + BKV]
+    return tuple((t * (0.125 if i < 2 else 1.0)).to(out_dtype) for i, t in enumerate((dq, dk, dv)))
+
+
 # ------------------------------------------------------------------------------------------------------- emulation
 def emulate(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, vis: torch.Tensor, kind: str) -> torch.Tensor:
     """the arithmetic of one kernel path in float32 / bf16 on the rounded inputs (q, k, v [H, L, 64] float32): 64-key

@@ -10,6 +10,7 @@ import torch.nn.functional as F
 
 from conftest import assert_checksums, build_model, load_golden
 from oracle import valle_oracle as O
+from stack_oracle64 import keep_mask as _keep_mask
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -29,20 +30,6 @@ def _no_dropout(m):
         if isinstance(mod, torch.nn.Dropout):
             mod.p = 0.0
     return m
-
-
-def _keep_mask(seed, stream, n, p, idx=None):
-    """the stateless mask of csrc/kernels.cuh::drop_keep restated in numpy: True = kept"""
-    import numpy as np
-    with np.errstate(over="ignore"):
-        i = np.arange(n, dtype=np.uint64) if idx is None else idx.astype(np.uint64)
-        z = np.uint64(seed) + np.uint64(stream) * np.uint64(0x9E3779B97F4A7C15) + i * np.uint64(0xD1342543DE82EF95)
-        z ^= z >> np.uint64(30)
-        z *= np.uint64(0xBF58476D1CE4E5B9)
-        z ^= z >> np.uint64(27)
-        z *= np.uint64(0x94D049BB133111EB)
-        z ^= z >> np.uint64(31)
-        return torch.from_numpy(((z >> np.uint64(32)) >= np.uint64(int(p * 4294967296.0))).astype(np.bool_))
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 2e-5), (torch.bfloat16, 2e-2)])
