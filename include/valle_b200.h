@@ -172,8 +172,8 @@ size_t vb_decoder_forward_workspace(const vb_decoder_desc *desc, int64_t M);
  * Layout (vb_decoder_forward and vb_ar_decode_step, VB_ERR_ARG otherwise): cache_layer_stride and cache_seq_stride
  * multiples of 1024, cache_cap a multiple of 16, k_exp / v_exp both set and 16-byte aligned -- the decode attention
  * reads the exponent rows 16 bytes at a time.
- * bf16 decoders only, on the tensor-core decode chains (B <= 64, not VB_DECODE_SIMT, not VB_ATTN_DECODE_1PASS) and the
- * wgmma prefill attention (not VB_ATTN_SIMT); everything else returns VB_ERR_UNSUPPORTED.
+ * bf16 decoders only, on the tensor-core decode chains (B <= 64, not VB_DECODE_SIMT) and the wgmma prefill attention
+ * (not VB_ATTN_SIMT); everything else returns VB_ERR_UNSUPPORTED.
  * ---------------------------------------------------------------------------------------- */
 
 /* a5/a6  TransformerEncoder.forward WITHOUT the final norm over packed ragged sequences

@@ -8,7 +8,7 @@ kv_len - 1, and its query attends to rows [0, kv_len).  A finished row appends n
 zero (the kernels skip it); its other outputs are not meaningful.
 
 Chains (where the operands are rounded to bf16; every sum is float64 here, fp32 in the kernels):
-  fp32           no rounding: the CUDA-core GEMV chain and attn_decode_kernel<float>, either layer order
+  fp32           no rounding: the CUDA-core GEMV chain and attn_decode_kernel, either layer order
   bf16_unfolded  pre-LN, VB_DECODE_FOLD=0: the projection operands bf16(LN(x)), bf16(attn_out), bf16(relu(.)); K and
                  V rounded to bf16 (the current token's too, as attention reads it); q unrounded; bf16(W); biases and
                  the residual stream fp32

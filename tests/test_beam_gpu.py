@@ -63,14 +63,16 @@ def _state(t, B):
 
 
 # ------------------------------------------------------------------------------------------- 1. decode attention
-# name: (chain, B, n, switches).  The chains are those of tests/test_decode_step_bitwise_gpu.py; "1pass" runs the
-# single-pass attention kernel.  B < 17 rows take the split-KV path at the default split count.
+# name: (chain, B, n, switches).  The chains are those of tests/test_decode_step_bitwise_gpu.py.  B < 17 rows take
+# the split-KV path at the default split count.
 STEP_CASES = {
     "folded_b2_n2": ("folded", 2, 2, ()),
     "folded_b16_n16_ns1": ("folded", 16, 16, (("VB_DECODE_NSPLIT", 1),)),
+    "folded_b48_n4": ("folded", 48, 4, ()),
     "folded_b48_n16": ("folded", 48, 16, ()),
     "folded_b64_n4_ns3": ("folded", 64, 4, (("VB_DECODE_NSPLIT", 3),)),
     "folded_b64_n8": ("folded", 64, 8, ()),
+    "nofold_b2_n2_ns7": ("unfolded", 2, 2, (("VB_DECODE_NSPLIT", 7),)),
     "nofold_b4_n4": ("unfolded", 4, 4, ()),
     "nofold_b48_n2_ns1": ("unfolded", 48, 2, (("VB_DECODE_NSPLIT", 1),)),
     "nofold_b64_n8_ns7": ("unfolded", 64, 8, (("VB_DECODE_NSPLIT", 7),)),
@@ -80,8 +82,6 @@ STEP_CASES = {
     "fp32_b16_n16": ("fp32", 16, 16, ()),
     "fp32_b48_n8_ns1": ("fp32", 48, 8, (("VB_DECODE_NSPLIT", 1),)),
     "fp32_b64_n4_ns7": ("fp32", 64, 4, (("VB_DECODE_NSPLIT", 7),)),
-    "1pass_b48_n4": ("folded", 48, 4, (("VB_ATTN_DECODE_1PASS", 1),)),
-    "1pass_b2_n2_ns7": ("unfolded", 2, 2, (("VB_ATTN_DECODE_1PASS", 1), ("VB_DECODE_NSPLIT", 7))),
 }
 
 

@@ -25,8 +25,7 @@ STEPS = 2
 
 
 # ------------------------------------------------------------------------------------------- 1. decode step
-# name: (chain, B, n, greedy, FP8 cache, switches).  The chains are those of tests/test_decode_step_bitwise_gpu.py;
-# "1pass" is the folded chain with the single-pass attention kernel.
+# name: (chain, B, n, greedy, FP8 cache, switches).  The chains are those of tests/test_decode_step_bitwise_gpu.py.
 STEP_CASES = {
     "folded_b2_n2_g1": ("folded", 2, 2, 1, False, ()),
     "folded_b17_n4_g2": ("folded", 17, 4, 2, False, ()),
@@ -36,12 +35,11 @@ STEP_CASES = {
     "folded_b64_n2_g2_ns7": ("folded", 64, 2, 2, False, (("VB_DECODE_NSPLIT", 7),)),
     "nofold_b17_n8_g0": ("unfolded", 17, 8, 0, False, ()),
     "nofold_b64_n4_g2_ns3": ("unfolded", 64, 4, 2, False, (("VB_DECODE_NSPLIT", 3),)),
+    "nofold_b64_n2_g0_ns7": ("unfolded", 64, 2, 0, False, (("VB_DECODE_NSPLIT", 7),)),
     "postln_b17_n4_g1": ("postln", 17, 4, 1, False, ()),
     "postln_b64_n2_g2_ns7": ("postln", 64, 2, 2, False, (("VB_DECODE_NSPLIT", 7),)),
     "fp32_b17_n4_g2": ("fp32", 17, 4, 2, False, ()),
     "fp32_b64_n8_g1_ns3": ("fp32", 64, 8, 1, False, (("VB_DECODE_NSPLIT", 3),)),
-    "1pass_b17_n4_g2": ("folded", 17, 4, 2, False, (("VB_ATTN_DECODE_1PASS", 1),)),
-    "1pass_b64_n2_g0_ns7": ("unfolded", 64, 2, 0, False, (("VB_ATTN_DECODE_1PASS", 1), ("VB_DECODE_NSPLIT", 7))),
     "simt_b17_n4_g1": ("folded", 17, 4, 1, False, (("VB_DECODE_SIMT", 1),)),
     "simt_postln_b2_n2_g2": ("postln", 2, 2, 2, False, (("VB_DECODE_SIMT", 1),)),
 }

@@ -46,12 +46,10 @@ CASES = {
     "folded_b64_g0": ("folded", 64, 0, (5, 40), ()),
     "folded_b17_out16": ("folded", 17, 1, (), (("VB_SPLITS_OUT", 16),)),
     "folded_b64_nopdl": ("folded", 64, 1, (0,), (("VB_NO_PDL", 1),)),
-    "folded_b17_1pass": ("folded", 17, 2, (), (("VB_ATTN_DECODE_1PASS", 1),)),
     "unfolded_b1_g0": ("unfolded", 1, 0, (), ()),
     "unfolded_b17_g1": ("unfolded", 17, 1, (16,), ()),
     "unfolded_b64_g2": ("unfolded", 64, 2, (7, 63), ()),
     "unfolded_b17_ffn2_1": ("unfolded", 17, 1, (), (("VB_SPLITS_FFN2", 1),)),
-    "unfolded_b64_1pass": ("unfolded", 64, 0, (), (("VB_ATTN_DECODE_1PASS", 1),)),
     "postln_b1_g1": ("postln", 1, 1, (), ()),
     "postln_b17_g0": ("postln", 17, 0, (2,), ()),
     "postln_b64_g2": ("postln", 64, 2, (9, 33), ()),

@@ -149,7 +149,7 @@ def _c(name, shape, chain, B, cap, **kw):
 OFF = (0.0, 4.0, 16.0, 64.0)
 NS = "VB_DECODE_NSPLIT"
 Q, OUT, F1, F2 = "VB_SPLITS_QKV", "VB_SPLITS_OUT", "VB_SPLITS_FFN1", "VB_SPLITS_FFN2"
-ONE_PASS, NO_PDL = ("VB_ATTN_DECODE_1PASS", 1), ("VB_NO_PDL", 1)
+NO_PDL = ("VB_NO_PDL", 1)
 CASES = [
     # ---- folded chain (the default) ----
     _c("big_folded_b1_clamp", "big", "bf16_folded", 1, 4160, lens=[4169], content="peak_last"),
@@ -159,8 +159,8 @@ CASES = [
        tune=[(NS, 7), (Q, 7), (OUT, 3), (F1, 4), (F2, 9)]),
     _c("big_folded_b64_out3", "big", "bf16_folded", 64, 96, offsets=OFF,
        tune=[(NS, 1), (Q, 16), (OUT, 3), (F1, 16), (F2, 16)]),
-    _c("big_folded_b17_1pass", "big", "bf16_folded", 17, 300, content="peak_current",
-       tune=[(NS, 32), (Q, 5), (OUT, 16), (F1, 1), (F2, 1), ONE_PASS]),
+    _c("big_folded_b17_ns32", "big", "bf16_folded", 17, 300, content="peak_current",
+       tune=[(NS, 32), (Q, 5), (OUT, 16), (F1, 1), (F2, 1)]),
     _c("big_folded_b33_nopdl", "big", "bf16_folded", 33, 130, offsets=OFF,
        tune=[(NS, 3), (Q, 2), (OUT, 8), (F1, 16), (F2, 9), NO_PDL]),
     _c("tiny_folded_b1", "tiny", "bf16_folded", 1, 4160, lens=[4160], content="peak_first"),
@@ -170,7 +170,7 @@ CASES = [
        tune=[(NS, 2), (Q, 4), (OUT, 3), (F1, 4), (F2, 9)]),
     _c("tiny_folded_b33_peak_current", "tiny", "bf16_folded", 33, 400, content="peak_current", offsets=OFF,
        tune=[(NS, 3), (OUT, 8), (F2, 16), NO_PDL]),
-    _c("tiny_folded_b63", "tiny", "bf16_folded", 63, 200, offsets=OFF, tune=[(NS, 7), (OUT, 16), (F1, 16), ONE_PASS]),
+    _c("tiny_folded_b63", "tiny", "bf16_folded", 63, 200, offsets=OFF, tune=[(NS, 7), (OUT, 16), (F1, 16)]),
     _c("tiny_folded_b64_out3", "tiny", "bf16_folded", 64, 200, offsets=OFF[::-1], finished=[62],
        tune=[(NS, 1), (OUT, 3), (F2, 9)]),
     _c("tiny_folded_b64_default", "tiny", "bf16_folded", 64, 300, content="peak_boundary", tune=[(NS, 3)]),
@@ -178,8 +178,8 @@ CASES = [
     _c("big_unfolded_b2_qkv16", "big", "bf16_unfolded", 2, 4160, lens=[4159, 33], content="peak_last", tune=[(Q, 16)]),
     _c("big_unfolded_b63_qkv1", "big", "bf16_unfolded", 63, 80, offsets=OFF, finished=[1],
        tune=[(NS, 2), (Q, 1), (OUT, 1), (F1, 1), (F2, 1)]),
-    _c("big_unfolded_b9_1pass_qkv7", "big", "bf16_unfolded", 9, 700, content="peak_first",
-       tune=[(NS, 7), (Q, 7), (OUT, 3), (F1, 4), (F2, 9), ONE_PASS]),
+    _c("big_unfolded_b9_qkv7", "big", "bf16_unfolded", 9, 700, content="peak_first",
+       tune=[(NS, 7), (Q, 7), (OUT, 3), (F1, 4), (F2, 9)]),
     _c("tiny_unfolded_b1_qkv1", "tiny", "bf16_unfolded", 1, 3000, lens=[1501], tune=[(NS, 32), (Q, 1)]),
     _c("tiny_unfolded_b17", "tiny", "bf16_unfolded", 17, 500, offsets=OFF, content="peak_current",
        tune=[(NS, 7), (Q, 2), (OUT, 8), (F1, 4), (F2, 16), NO_PDL]),
@@ -189,10 +189,10 @@ CASES = [
     _c("big_postln_b17", "big", "bf16_postln", 17, 300, content="peak_first"),
     _c("big_postln_b2_qkv1", "big", "bf16_postln", 2, 1500, lens=[1, 1499], tune=[(NS, 7), (Q, 1), (OUT, 3)]),
     _c("tiny_postln_b9_qkv7", "tiny", "bf16_postln", 9, 400, finished=[3],
-       tune=[(NS, 32), (Q, 7), (OUT, 1), (F1, 16), (F2, 9), ONE_PASS]),
+       tune=[(NS, 32), (Q, 7), (OUT, 1), (F1, 16), (F2, 9)]),
     _c("tiny_postln_b64", "tiny", "bf16_postln", 64, 150, content="flat", tune=[(NS, 3), (Q, 1), NO_PDL]),
     _c("tiny_postln_b1", "tiny", "bf16_postln", 1, 4160, lens=[4160], content="peak_current"),
-    # ---- fp32 chain (CUDA-core GEMVs, attn_decode_kernel<float>) ----
+    # ---- fp32 chain (CUDA-core GEMVs, attn_decode_kernel) ----
     _c("big_fp32_b9", "big", "fp32", 9, 300, offsets=OFF, finished=[2], tune=[(NS, 3)]),
     _c("big_fp32_b1", "big", "fp32", 1, 4160, lens=[4160]),
     _c("tiny_fp32_b33", "tiny", "fp32", 33, 500, content="peak_boundary", tune=[(NS, 7)]),

@@ -19,7 +19,7 @@ import pytest
 import torch
 
 from test_beam_gpu import CAP, DEV, H, NINF, TS, _bits, _head, _lib, _state
-from test_decode_step_bitwise_gpu import D, EOS, LDL, NL, _model, _switches
+from test_decode_step_bitwise_gpu import D, EOS, LDL, NL, _model
 from test_stream_gpu import _model as _engine_model
 from test_stream_gpu import _rand_utts, _requests, tuned
 
@@ -41,8 +41,6 @@ def one_kv_split():
 # "run", "fin" (a finished hypothesis that beats every continuation: stops after the first step), "cap" (stops at its
 # length cap after two steps)
 LAYOUT = ["s", "g", "s", (4, "run"), "g", (2, "fin"), "s", (16, "run"), (2, "cap"), "g", (3, "run")]
-CHAINS = {"folded": ("folded", ()), "unfolded": ("unfolded", ()), "postln": ("postln", ()), "fp32": ("fp32", ()),
-          "1pass": ("folded", (("VB_ATTN_DECODE_1PASS", 1),))}
 STEPS = 5
 
 
@@ -126,47 +124,45 @@ def _bind(t, B, greedy):
     return s
 
 
-def _decode(m, chain, t, B, greedy, tune, beam_width=0):
+def _decode(m, chain, t, B, greedy, beam_width=0):
     L, lib = _lib()
     s = _bind(t, B, greedy)
     s.beam_width = beam_width
     h = _head(m, chain, greedy)
-    with _switches(lib, tune):
-        nbytes = lib.vb_ar_step_workspace(C.byref(m["nd"].desc), B, CAP)
-        ws = torch.zeros(nbytes, dtype=torch.uint8, device=DEV)
-        for _ in range(STEPS):
-            L.check(lib.vb_ar_decode_step(m["nd"].handle, C.byref(h), C.byref(s), ws.data_ptr(), nbytes,
-                                          L.stream_ptr()), "vb_ar_decode_step")
-        torch.cuda.synchronize()
+    nbytes = lib.vb_ar_step_workspace(C.byref(m["nd"].desc), B, CAP)
+    ws = torch.zeros(nbytes, dtype=torch.uint8, device=DEV)
+    for _ in range(STEPS):
+        L.check(lib.vb_ar_decode_step(m["nd"].handle, C.byref(h), C.byref(s), ws.data_ptr(), nbytes, L.stream_ptr()),
+                "vb_ar_decode_step")
+    torch.cuda.synchronize()
     return t
 
 
-@pytest.mark.parametrize("case", sorted(CHAINS))
-def test_mixed_step_equals_separate_steps(case):
-    chain, tune = CHAINS[case]
+@pytest.mark.parametrize("chain", ["folded", "fp32", "postln", "unfolded"])
+def test_mixed_step_equals_separate_steps(chain):
     singles, groups, B = _layout()
-    g = torch.Generator().manual_seed(sum(map(ord, case)))
+    g = torch.Generator().manual_seed(sum(map(ord, chain)))
     dtype = torch.float32 if chain == "fp32" else torch.bfloat16
     m = _model(chain in ("folded", "unfolded", "fp32"), dtype)
     t0 = _mixed_state(g, B, singles, groups, dtype)
-    mixed = _decode(m, chain, {k: v.clone() for k, v in t0.items()}, B, 4, tune)
+    mixed = _decode(m, chain, {k: v.clone() for k, v in t0.items()}, B, 4)
     rows = [r for r, _ in singles]
-    alone = _decode(m, chain, _rows(t0, rows), len(rows), 2, tune)
+    alone = _decode(m, chain, _rows(t0, rows), len(rows), 2)
     for k in ("tokens", "n_gen", "finished", "x"):
-        assert torch.equal(_bits(mixed[k][rows]), _bits(alone[k])), (case, "single rows", k)
+        assert torch.equal(_bits(mixed[k][rows]), _bits(alone[k])), (chain, "single rows", k)
     assert bool(mixed["finished"][rows].eq(0).any())
     for r0, n, kind in groups:
         rr = list(range(r0, r0 + n))
-        sep = _decode(m, chain, _rows(t0, rr, n), n, 3, tune, beam_width=n)
+        sep = _decode(m, chain, _rows(t0, rr, n), n, 3, beam_width=n)
         for k in ("tokens", "n_gen", "finished", "x", "anc", "score"):
-            assert torch.equal(_bits(mixed[k][rr]), _bits(sep[k])), (case, r0, n, kind, k)
-        assert torch.equal(_bits(mixed["fin"][r0]), _bits(sep["fin"][0])), (case, r0, kind, "fin")
+            assert torch.equal(_bits(mixed[k][rr]), _bits(sep[k])), (chain, r0, n, kind, k)
+        assert torch.equal(_bits(mixed["fin"][r0]), _bits(sep["fin"][0])), (chain, r0, kind, "fin")
         if float(sep["fin"][0, 0]) > NINF:
             ln = int(sep["fin_len"][0])
             assert int(mixed["fin_len"][r0]) == ln
-            assert torch.equal(mixed["fin_anc"][r0, :ln], sep["fin_anc"][0, :ln]), (case, r0, kind)
+            assert torch.equal(mixed["fin_anc"][r0, :ln], sep["fin_anc"][0, :ln]), (chain, r0, kind)
         stopped = bool(sep["finished"][0])
-        assert stopped == (kind in ("fin", "cap")), (case, r0, kind)
+        assert stopped == (kind in ("fin", "cap")), (chain, r0, kind)
 
 
 # ------------------------------------------------------------------------------------------- 2. admission

@@ -226,24 +226,12 @@ int launch_attention_varlen(const void *qkv, int dtype, int64_t M, int n_head, i
 // ------------------------------------------------------------------------------------------
 static constexpr int kDecMaxChunk = 4096;
 
-template <typename T> struct KvRow8 {  // 8 consecutive elements of a cache row as floats
-  static __device__ __forceinline__ void load(const T *p, float (&f)[8]);
-};
-template <> __device__ __forceinline__ void KvRow8<float>::load(const float *p, float (&f)[8]) {
+// 8 consecutive elements of an fp32 cache row
+__device__ __forceinline__ void kv_row8_f32(const float *p, float (&f)[8]) {
   const uint4 a = ldg_stream16(p), b = ldg_stream16(p + 4);
   f[0] = __uint_as_float(a.x); f[1] = __uint_as_float(a.y); f[2] = __uint_as_float(a.z); f[3] = __uint_as_float(a.w);
   f[4] = __uint_as_float(b.x); f[5] = __uint_as_float(b.y); f[6] = __uint_as_float(b.z); f[7] = __uint_as_float(b.w);
 }
-template <> __device__ __forceinline__ void KvRow8<bf16>::load(const bf16 *p, float (&f)[8]) {
-  Vec16<bf16> v;
-  v.raw = ldg_stream16(p);
-  v.unpack(f);
-}
-
-// Optional fused prologue (qp.part != nullptr): q/k/v of the CURRENT token arrive as split-K partials of the QKV
-// projection (gemm_decode.cu); the CTA sums them in fixed order, adds the bias, appends k/v to the cache (split 0)
-// and serves the new key/value from shared memory.  qp.fold.stats != NULL: the partials are x (gamma o W)^T of the
-// raw rows (gemm_decode_x_kernel).
 
 // A finished utterance (stop rule fired, vb_ar_state.finished != 0) takes no further part in the step: its KV
 // cache stays as it is (nothing appended, nothing streamed) and its attention output row is zero.  Uniform
@@ -268,19 +256,17 @@ __device__ __forceinline__ bool decode_row_finished(const int32_t *finished, int
   return true;
 }
 
-// Single pass, no block-level synchronisation inside the loop: each 8-lane group owns every 16th key of
-// the chunk, streams the K row and the V row of its keys together (4 keys = 8 x 16-byte loads in
-// flight per lane), and keeps its OWN online-softmax state (m, l, 8 output elements per lane).  The 16
-// groups are merged once at the end (flash-decoding style).
-template <typename T, bool kShared = false, bool kBeam = false>
+// fp32 cache (the fp32 parity chain): q of the current token and its k / v row are already in place, written by the
+// QKV projection.  Single pass, no block-level synchronisation inside the loop: each 8-lane group owns every 16th key
+// of the chunk, streams the K row and the V row of its keys together (4 keys = 16 x 16-byte loads in flight per lane),
+// and keeps its OWN online-softmax state (m, l, 8 output elements per lane).  The 16 groups are merged once at the end
+// (flash-decoding style).
+template <bool kShared = false, bool kBeam = false>
 __global__ void __launch_bounds__(128)
-attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache kv, KvRows rows,
-                   float *__restrict__ out, bf16 *__restrict__ out16,
+attn_decode_kernel(const float *__restrict__ q, int n_head, KvCache kv, KvRows rows, float *__restrict__ out,
                    float *__restrict__ part_o, float *__restrict__ part_ml, int nsplit,
                    const int32_t *__restrict__ kv_parent, BeamAnc beam) {
   __shared__ __align__(16) float qs[HD];
-  __shared__ __align__(16) float knew[HD];
-  __shared__ __align__(16) float vnew[HD];
   __shared__ float g_o[16][HD + 1];
   __shared__ float g_m[16], g_l[16];
   pdl_launch_dependents();
@@ -288,49 +274,20 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int d = n_head * HD;
   pdl_wait();
-  if (decode_row_finished(rows.finished, b, h, sp, d, threadIdx.x, nsplit, n_head, out, out16, part_o, part_ml)) return;
+  if (decode_row_finished(rows.finished, b, h, sp, d, threadIdx.x, nsplit, n_head, out, nullptr, part_o, part_ml)) return;
   const int pos = rows.cur(b, rows.n_gen[b], kv.cap);  // cache row of the current token
   const int kv_len = pos + 1;
   const int chunk = ((kv_len + nsplit - 1) / nsplit + 15) & ~15;
   const int c0 = sp * chunk, c1 = min(kv_len, c0 + chunk);
   const int n = max(0, c1 - c0);
-  T *kb = (T *)kv.k + kv.row(b, h, 0);
-  T *vb_ = (T *)kv.v + kv.row(b, h, 0);
+  const float *kb = (const float *)kv.k + kv.row(b, h, 0);
+  const float *vb_ = (const float *)kv.v + kv.row(b, h, 0);
   KvStreamRows<kShared, kBeam> sr(kv_parent, rows, kv, b);
   if constexpr (kBeam) {   // read after the __syncthreads below
     extern __shared__ __align__(16) int16_t beam_dl[];
     sr.stage_beam(beam_dl, kv_parent, rows, beam, b, c0, n, pos);
   }
-  const bool has_new = qp.part != nullptr;
-  if (tid < HD) {
-    if (has_new) {
-      float a[3];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const int col = j * d + h * HD + tid;
-        const float *p = qp.part + (int64_t)b * qp.ldp + col;
-        float acc = __ldcg(p);
-#pragma unroll 6
-        for (int s = 1; s < qp.splits; ++s) acc += __ldcg(p + (int64_t)s * 64 * qp.ldp);
-        if (qp.fold.stats) {
-          float mean, rstd;
-          ln_fold_moments(qp.fold, b, h, mean, rstd);
-          acc = rstd * (acc - mean * qp.fold.c[col]);
-        }
-        a[j] = acc + qp.bias[col];
-      }
-      qs[tid] = a[0] * 0.125f;
-      const T k16 = from_f32<T>(a[1]), v16 = from_f32<T>(a[2]);
-      knew[tid] = to_f32(k16);  // exactly what later steps will read back from the cache
-      vnew[tid] = to_f32(v16);
-      if (sp == 0) {
-        kb[(int64_t)pos * HD + tid] = k16;
-        vb_[(int64_t)pos * HD + tid] = v16;
-      }
-    } else {
-      qs[tid] = q[(int64_t)b * d + h * HD + tid] * 0.125f;
-    }
-  }
+  if (tid < HD) qs[tid] = q[(int64_t)b * d + h * HD + tid] * 0.125f;
   __syncthreads();
 
   const int grp = warp * 4 + (lane >> 3);  // 0..15
@@ -342,26 +299,24 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[i] = 0.f;
 
-  for (int base = 0; base < n; base += 64) {
-    float kf[4][8], vf[4][8];
+  // The K and V rows of a tile are requested at the end of the tile before it, so that all 16 loads are in flight
+  // together: requested at the top of the tile, the V loads would be scheduled behind the K dot products, one more
+  // round trip to memory per tile.
+  float kf[4][8], vf[4][8];
+  auto load_tile = [&](int base) {
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
-      const int key = base + u * 16 + grp;
-      const int kk = min(key, n - 1);
-      KvRow8<T>::load(kb + sr.row(c0 + kk) + j8, kf[u]);
-      KvRow8<T>::load(vb_ + sr.row(c0 + kk) + j8, vf[u]);
+      const int kk = min(base + u * 16 + grp, n - 1);
+      kv_row8_f32(kb + sr.row(c0 + kk) + j8, kf[u]);
+      kv_row8_f32(vb_ + sr.row(c0 + kk) + j8, vf[u]);
     }
+  };
+  if (n > 0) load_tile(0);
+  for (int base = 0; base < n; base += 64) {
     float s[4];
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       const int key = base + u * 16 + grp;
-      if (has_new && c0 + min(key, n - 1) == pos) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          kf[u][i] = knew[j8 + i];
-          vf[u][i] = vnew[j8 + i];
-        }
-      }
       float dot = 0.f;
 #pragma unroll
       for (int i = 0; i < 8; ++i) dot = fmaf(qf[i], kf[u][i], dot);
@@ -387,6 +342,7 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
       }
       m = mn;
     }
+    if (base + 64 < n) load_tile(base + 64);
   }
   // ---- merge the 16 groups ------------------------------------------------------------------------
 #pragma unroll
@@ -410,7 +366,6 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
     }
     if (nsplit == 1) {
       out[(int64_t)b * d + h * HD + tid] = ot / lt;
-      if (out16) out16[(int64_t)b * d + h * HD + tid] = __float2bfloat16_rn(ot / lt);
     } else {
       const int64_t pi = ((int64_t)b * n_head + h) * nsplit + sp;
       part_o[pi * HD + tid] = ot;
@@ -429,6 +384,10 @@ attn_decode_kernel(const float *__restrict__ q, SplitK qp, int n_head, KvCache k
 // 8 CTAs per SM (<= 64 registers, which holds U = 4 K / V rows per thread without spilling): the 1,024 CTAs of B=64 x
 // 16 heads are then resident at once on the H100's 132 SMs.  At 7 per SM (U = 8, 72 registers) 100 of them waited for
 // the first wave to drain and then streamed their whole K and V alone.
+// Fused QKV prologue (qp.part != nullptr): q/k/v of the CURRENT token arrive as split-K partials of the QKV
+// projection (gemm_decode.cu); the CTA sums them in fixed order, adds the bias, appends k/v to the cache (split 0)
+// and serves the new key/value from shared memory.  qp.fold.stats != NULL: the partials are x (gamma o W)^T of the
+// raw rows (gemm_decode_x_kernel).
 // CT = uint8_t: the FP8 cache (e4m3 rows, exponent bytes kexp / vexp; the fused QKV prologue is required).  A lane
 // then loads 8 bytes (its 8 elements) per row, so U = 8 rows keep the same bytes and registers in flight as U = 4 bf16
 // rows.  The exponents of the chunk come into shared memory by cp.async; 2^e is applied once per row: to the score
@@ -799,14 +758,10 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
   float *part_ml = part_o + (size_t)B * n_head * ns * HD;
   dim3 grid(n_head, B, ns);
   // beam search: the chunk's row table, int16 per row, behind the score buffer of the two-phase kernel (sized as the
-  // kernel sizes it) or alone (single-pass kernel); kBeam instantiations take kShared = true
+  // kernel sizes it) or alone (fp32 kernel); kBeam instantiations take kShared = true
   const bool bm = beam.anc != nullptr;
   const int dl_len = ((cache_cap + ns - 1) / ns + 32 + 15) & ~15;
   if (dtype == VB_E4M3) {
-    if (tune("VB_ATTN_DECODE_1PASS", 0) != 0) {
-      set_error("attn_decode: VB_ATTN_DECODE_1PASS has no FP8-cache variant");
-      return VB_ERR_UNSUPPORTED;
-    }
     VB_CHECK_ARG(qkv.part != nullptr && kv.kv.kexp != nullptr && kv.kv.vexp != nullptr && cache_cap % 16 == 0,
                  "attn_decode: the FP8 cache needs the fused QKV prologue, exponent arrays and cache_cap %% 16 == 0");
     // score buffer as for bf16 (rounded to 16 floats), then the chunk's K and V exponent bytes
@@ -816,12 +771,12 @@ int launch_attn_decode(const QkvScatter &kv, const SplitK &qkv, int B, int n_hea
     VB_TRY(set_attn_carveout<k>());
     VB_CUDA(launch_kernel(k, grid, dim3(128), smem, s, pdl, (const float *)kv.q, qkv, n_head, kv.kv, kv.rows, out,
                           (bf16 *)out16, part_o, part_ml, ns, nullptr, BeamAnc{}));   // no shared rows (vb_ar_decode_step)
-  } else if (dtype == VB_F32 || tune("VB_ATTN_DECODE_1PASS", 0) != 0) {  // fp32 parity path / single-pass variant
-    const auto k = bm ? (dtype == VB_F32 ? attn_decode_kernel<float, true, true> : attn_decode_kernel<bf16, true, true>)
-                      : dtype == VB_F32 ? (kv_parent ? attn_decode_kernel<float, true> : attn_decode_kernel<float>)
-                                        : (kv_parent ? attn_decode_kernel<bf16, true> : attn_decode_kernel<bf16>);
-    VB_CUDA(launch_kernel(k, grid, dim3(128), bm ? dl_len * sizeof(int16_t) : 0, s, pdl, (const float *)kv.q, qkv,
-                          n_head, kv.kv, kv.rows, out, (bf16 *)out16, part_o, part_ml, ns, kv_parent, beam));
+  } else if (dtype == VB_F32) {
+    VB_CHECK_ARG(qkv.part == nullptr && out16 == nullptr,
+                 "attn_decode: the fp32 cache takes q and the k / v rows in place, and writes fp32 rows only");
+    const auto k = bm ? attn_decode_kernel<true, true> : kv_parent ? attn_decode_kernel<true> : attn_decode_kernel<>;
+    VB_CUDA(launch_kernel(k, grid, dim3(128), bm ? dl_len * sizeof(int16_t) : 0, s, pdl, (const float *)kv.q, n_head,
+                          kv.kv, kv.rows, out, part_o, part_ml, ns, kv_parent, beam));
   } else if (bm) {
     constexpr auto k_bm = attn_decode_2phase_pf_kernel<4, bf16, true, true>;
     VB_TRY(set_attn_carveout<k_bm>());

@@ -163,34 +163,25 @@ __device__ __forceinline__ uint2 ldg_stream8(const void *p) {
 }
 
 // ---- grid-wide barrier of a cooperative launch (every CTA resident).  `ctr` is a monotonic arrival counter zeroed
-// before the launch; `target` (thread 0) advances by gridDim.x per barrier.  mode 0: every CTA polls the counter with
-// ld.acquire (simplest, but ~150 pollers hammer one L2 line and delay the late arrivals' atomics); mode 1: polling
-// with nanosleep back-off; mode 2: the LAST arriver publishes a generation word that the others poll, so the counter
-// line only sees one atomic per CTA.
-__device__ __forceinline__ void grid_barrier_sync(unsigned *ctr, unsigned &target, int mode) {
+// before the launch, together with the generation word 32 words behind it; `target` (thread 0) advances by gridDim.x
+// per barrier.  The LAST arriver publishes the target as the generation word, which the others poll: the counter line
+// sees one atomic per CTA, where ~150 CTAs polling the counter itself would hammer that L2 line and delay the late
+// arrivals' atomics.
+__device__ __forceinline__ void grid_barrier_sync(unsigned *ctr, unsigned &target) {
   __syncthreads();
   if (threadIdx.x == 0) {
     const unsigned G = gridDim.x * gridDim.y * gridDim.z;
     target += G;
-    if (mode == 2) {
-      unsigned *gen = ctr + 32;   // a different 128-byte line
-      unsigned prev;
-      asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], 1;" : "=r"(prev) : "l"(ctr) : "memory");
-      if (prev + 1 == target) {
-        asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(gen), "r"(target) : "memory");
-      } else {
-        unsigned v;
-        do {
-          __nanosleep(20);
-          asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(gen) : "memory");
-        } while ((int)(v - target) < 0);
-      }
+    unsigned *gen = ctr + 32;   // a different 128-byte line
+    unsigned prev;
+    asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], 1;" : "=r"(prev) : "l"(ctr) : "memory");
+    if (prev + 1 == target) {
+      asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(gen), "r"(target) : "memory");
     } else {
-      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
       unsigned v;
       do {
-        if (mode == 1) __nanosleep(40);
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(ctr) : "memory");
+        __nanosleep(20);
+        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(gen) : "memory");
       } while ((int)(v - target) < 0);
     }
   }

@@ -172,8 +172,7 @@ constexpr int LSTM_U = 4, LSTM_C = 4 * LSTM_U, LSTM_MAXB = 64;
 
 __global__ void __launch_bounds__(256, 1)
 lstm_layer_persistent_kernel(const float *__restrict__ xproj /*[T][B][4H]*/, const float *__restrict__ whh_t /*[H][4H]*/,
-                             int T, int B, int H, float *__restrict__ h_seq /*[T][B][H]*/, unsigned *__restrict__ sync,
-                             int barrier_mode) {
+                             int T, int B, int H, float *__restrict__ h_seq /*[T][B][H]*/, unsigned *__restrict__ sync) {
   extern __shared__ __align__(16) float sm[];
   const int HP = H + 1;                      // padded row of the h tile (bank spread over batch rows)
   float *wsl = sm;                           // [H][LSTM_C]  column c = gate * LSTM_U + u
@@ -248,7 +247,7 @@ lstm_layer_persistent_kernel(const float *__restrict__ xproj /*[T][B][4H]*/, con
       cst[i] = cn;
       h_seq[((int64_t)t * B + b) * H + u0 + u] = so * tanhf(cn);
     }
-    if (t + 1 < T) grid_barrier_sync(sync, bar_target, barrier_mode);
+    if (t + 1 < T) grid_barrier_sync(sync, bar_target);
   }
 }
 
@@ -427,12 +426,10 @@ VB_API int vb_lstm_layer(const float *xproj, const float *whh_t, int T, int B, i
     // all T steps in one cooperative launch; the grid-barrier word lives behind the cell-state scratch
     unsigned *sync = reinterpret_cast<unsigned *>(c_state + (size_t)B * H);
     VB_CUDA(cudaMemsetAsync(sync, 0, 64 * sizeof(unsigned), s));
-    int barrier_mode = tune("VB_GRID_BARRIER", 2);
     auto kern = ec::lstm_layer_persistent_kernel;
     static PerDeviceOnce once;
     if (once.first()) VB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    void *args[] = {(void *)&xproj, (void *)&whh_t, (void *)&T, (void *)&B, (void *)&H, (void *)&h_seq, (void *)&sync,
-                    (void *)&barrier_mode};
+    void *args[] = {(void *)&xproj, (void *)&whh_t, (void *)&T, (void *)&B, (void *)&H, (void *)&h_seq, (void *)&sync};
     VB_CUDA(cudaLaunchCooperativeKernel((const void *)kern, dim3(grid_p), dim3(256), args, smem_p, s));
     count_launch();
     return VB_OK;
