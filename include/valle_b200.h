@@ -674,7 +674,8 @@ size_t vb_scaled_adam_workspace(int n_tensors, int n_chunks);
  *      alpha (alpha = -lr (1 - beta1) max(param_rms, param_min_rms)); p += delta.  Scalars: the same with
  *      lr * scalar_lr_scale and p clamped to +-scalar_max before p += delta (optim.py:639-661).
  * tensors: DEVICE array of n_tensors entries; grads: HOST array of n_tensors gradient pointers (NULL = zeros);
- * chunk0: HOST array of n_tensors + 1 chunk offsets, equal to the table's (the last one is n_chunks). */
+ * chunk0: HOST array of n_tensors + 1 chunk offsets, equal to the table's (the last one is n_chunks).  A tensor with
+ * no elements (chunk0[t + 1] == chunk0[t]) is refused with VB_ERR_ARG before anything is launched. */
 int vb_scaled_adam_step(const vb_scaled_adam_tensor *tensors, const float *const *grads, const int32_t *chunk0,
                         const vb_scaled_adam_args *args, float *model_norms, vb_clip_state *clip, void *workspace,
                         size_t ws_bytes, vb_stream_t stream);

@@ -445,6 +445,10 @@ VB_API int vb_scaled_adam_step(const vb_scaled_adam_tensor *tensors, const float
   VB_CHECK_ARG(T > 0, "vb_scaled_adam_step: n_tensors = %d", T);
   VB_CHECK_ARG(chunk0[0] == 0 && chunk0[T] == A.n_chunks, "vb_scaled_adam_step: chunk0[0] = %d, chunk0[%d] = %d != "
                "n_chunks = %d", chunk0[0], T, chunk0[T], A.n_chunks);
+  // a zero-element parameter has no param_rms / scale_grads slot for sadam_coef_kernel to read and write
+  for (int t = 0; t < T; ++t)
+    VB_CHECK_ARG(chunk0[t + 1] > chunk0[t], "vb_scaled_adam_step: tensor %d has no elements (chunk0[%d] = %d, "
+                 "chunk0[%d] = %d)", t, t, chunk0[t], t + 1, chunk0[t + 1]);
   VB_CHECK_ARG(A.size_period >= 1 && A.step >= 0, "vb_scaled_adam_step: size_period = %d, step = %d", A.size_period,
                A.step);
   VB_CHECK_ARG(A.clip_mode >= 0 && A.clip_mode <= 2, "vb_scaled_adam_step: clip_mode = %d", A.clip_mode);

@@ -50,6 +50,17 @@ def _check_param(p: Tensor, name: str, opt: str) -> None:
         raise L.VbError(f"{opt}: parameter {name} is not contiguous")
 
 
+def _check_sadam_params(batches) -> None:
+    """ScaledAdam keeps a param_rms and scale_grads slot per parameter; a zero-element one has none (the reference
+    fails on it with a KeyError), so it is refused before any state or table is built."""
+    for _, ps, ns in batches:
+        for p, n in zip(ps, ns):
+            _check_param(p, n, "ScaledAdam")
+            if p.numel() == 0:
+                raise L.VbError(f"ScaledAdam: parameter {n} has no elements; ScaledAdam cannot step a zero-element "
+                                "parameter (it has no rms to scale its update by)")
+
+
 def _check_grad(g: Tensor, p: Tensor, name: str, opt: str) -> None:
     if g.is_sparse:
         raise RuntimeError(f"{opt} optimizer does not support sparse gradients")
@@ -237,9 +248,8 @@ class ScaledAdam(Optimizer):
             if not all(empty):
                 raise ValueError("ScaledAdam: some batches of a parameter group have state and others have none; "
                                  "the native step needs one step count per group")
-            for (_, ps, ns), st in zip(batches, states):
-                for p, n in zip(ps, ns):
-                    _check_param(p, n, "ScaledAdam")
+            _check_sadam_params(batches)
+            for (_, ps, _), st in zip(batches, states):
                 self._init_state(group, ps, st)
             plan = None
         fs = states[0]
@@ -250,9 +260,7 @@ class ScaledAdam(Optimizer):
                 raise ValueError(f"ScaledAdam: the batches of group {gi} are at different steps "
                                  f"({st['step']} vs {step}); the native step needs one step count per group")
         if plan is None or plan.key != _SadamPlan.signature(batches, states):
-            for (_, ps, ns) in batches:
-                for p, n in zip(ps, ns):
-                    _check_param(p, n, "ScaledAdam")
+            _check_sadam_params(batches)
             plan = _SadamPlan(batches, states, params[0].device)
             self._plans[gi] = plan
 
@@ -413,7 +421,8 @@ class Eden(LRScheduler):
 
 class Eve(Optimizer):
     """valle/modules/optim.py:836-985 (AdamW whose weight decay only applies while ||p|| > target_rms * sqrt(numel)),
-    stepped by vb_eve_step.  Parameters with a None gradient are skipped and get no state."""
+    stepped by vb_eve_step.  Parameters with a None gradient are skipped and get no state; a zero-element parameter
+    gets its state and its step count, and no table entry."""
 
     def __init__(self, params, lr=1e-3, betas=(0.9, 0.98), eps=1e-8, weight_decay=1e-3, target_rms=0.1):
         if not 0.0 <= lr:
@@ -457,9 +466,11 @@ class Eve(Optimizer):
                     state["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                     state["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
                 state["step"] += 1
+                n = p.numel()
+                if n == 0:  # the reference's update of an empty tensor changes nothing but its step
+                    continue
                 bc1 = 1 - beta1 ** state["step"]
                 bc2 = 1 - beta2 ** state["step"]
-                n = p.numel()
                 rows.append((p.data_ptr(), p.grad.data_ptr(), state["exp_avg"].data_ptr(),
                              state["exp_avg_sq"].data_ptr(), n, group["lr"] / bc1, bc2 ** -0.5,
                              group["target_rms"] * (n ** 0.5) if n > 1 else float("inf")))
